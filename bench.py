@@ -11,9 +11,9 @@ over one batch of `--batch` synthetic queries against the HBM-resident database.
                   bytes out; deserialization (ChaCha20 seed expansion), H2D and D2H are inside the timed region
   * `roofline`  : the dominant kernel (multiply_reg_by_database, server.rs:155-221), algorithmic bytes
                   per launch / its CUDA-event duration measured live in the timed region, against the
-                  measured HBM peak of MEASURED_PEAKS.json
+                  HBM peak of MEASURED_PEAKS.json when present, else the H100 SXM data sheet's 3.35 TB/s
   * `cpu_baseline` / `--impl reference` : the CPU restatement of the reference (oracle/, "port": no Rust
-                  toolchain exists in the image) on the host cores: FULL process_query calls on the same parameter set
+                  toolchain is assumed) on the host cores: FULL process_query calls on the same parameter set
                   (measured, one query at a time as the reference processes them), with the bounded-sample extrapolation
                   of round 1 beside it
 
@@ -62,6 +62,17 @@ def log(*a):
     print(*a, file=sys.stderr, flush=True)
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(directory, arrays):
+    """Write each array as directory/<name>.npy: bytes as float32, wider integers as float64 (both exact)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32 if a.dtype == np.uint8 else np.float64))
+
+
 def derived(kw):
     import math
     dim0, num_per = 1 << kw["nu_1"], 1 << kw["nu_2"]
@@ -92,7 +103,7 @@ def synthetic_pp(kw, rng):
 
 
 class ClockSampler:
-    """nvidia-smi sampler running during the timed region (B200_PROFILING.md 'clocks line')."""
+    """nvidia-smi sampler running during the timed region (median SM clock, throttle reasons)."""
 
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -152,18 +163,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(workload, batch, db_format):
-    """dram bytes per launch of the multiply kernel from the committed ncu --set full capture of this configuration, if any
-    (profiles/roofline_traffic.json; key = workload, queries per step, database format)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            d = json.load(f)
-        return d.get("%s_batch%d_format%d" % (workload, batch, db_format))
-    except Exception:
-        return None
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ------------------------------------------------------------------------------------------- CPU legs
@@ -312,7 +312,7 @@ def run_reference_arm(args, kw, workload_name, rank, world):
 
 # ------------------------------------------------------------------------------------------- kernel-level workloads
 def kernel_workload(args):
-    """BASELINE configs #4 (DoublePIR 2^24 x 1366 packed words, HBM GB/s vs roofline) and #5 (NTT / INTT throughput, poly_len
+    """BASELINE configs #4 (DoublePIR at 2^23 x 1366 packed words, HBM GB/s vs roofline) and #5 (NTT / INTT throughput, poly_len
     2048 and 4096, 2^16 polynomials x 2 CRT moduli) as bench lines: `--workload dpir`, `--workload ntt`.  Single GPU."""
     import ctypes as C
     import numpy as np
@@ -341,7 +341,7 @@ def kernel_workload(args):
     sampler.wait_first()
     t0 = time.time()
     if args.workload == "dpir":
-        rows, cols = 1 << 24, 1366                                   # 2^24 x ceil(2^12 / 3) u32 = 91.7 GB, larger than L2 by far
+        rows, cols = 1 << 23, 1366                                   # 2^23 x ceil(2^12 / 3) u32 = 45.8 GB (fits an 80 GB H100)
         m = D.PackedMatrix(rows=rows, cols=cols, synthetic_seed=7)
         check(LIB.b200pir_dpir_set_stream(m._h, C.c_void_p(stream.cuda_stream)))
         rng = np.random.default_rng(11)
@@ -349,6 +349,10 @@ def kernel_workload(args):
         b = torch.from_numpy(hb.view(np.int32)).cuda()
         out = torch.zeros(rows, dtype=torch.int32, device="cuda")
         ms = timed(lambda: check(LIB.b200pir_dpir_matvec_packed_dev(m._h, b.data_ptr(), out.data_ptr(), 0)))
+        if args.dump_outputs:
+            rows_sample = np.sort(np.random.default_rng(12).choice(rows, 1 << 20, replace=False))
+            dump_outputs(args.dump_outputs, {"row_index": rows_sample,
+                                             "matvec": out.cpu().numpy().view(np.uint32)[rows_sample]})
         alg = 4 * rows * cols + 12 * cols + 4 * rows
         ho = np.zeros(rows, dtype=np.uint32)
         t1 = time.perf_counter()
@@ -362,14 +366,14 @@ def kernel_workload(args):
         t1 = time.perf_counter()
         O.dpir_matvec_packed(a_s, hb, srows, cols)
         cpu_s = (time.perf_counter() - t1) * (rows / srows)
-        line = {"metric": "DoublePIR matrix_mul_vec_packed HBM GB/s (2^24 x 1366 packed words)", "value": alg / ms / 1e6, "unit": "GB/s",
-                "ms_per_step": ms, "dtype": "u32", "config": {"workload": "dpir: BASELINE configs[3], 2^24 rows x 1366 words (3 x 10 bit), 91.7 GB",
+        line = {"metric": "DoublePIR matrix_mul_vec_packed HBM GB/s (2^23 x 1366 packed words)", "value": alg / ms / 1e6, "unit": "GB/s",
+                "ms_per_step": ms, "dtype": "u32", "config": {"workload": "dpir: BASELINE configs[3] at 2^23 rows x 1366 words (3 x 10 bit), 45.8 GB",
                                                                "l2": "inputs larger than L2"},
                 "roofline": {"bound": "hbm", "kernel": "k_dpir_matvec_row", "achieved": alg / ms / 1e6, "peak": peak, "unit": "GB/s",
                              "frac": alg / ms / 1e6 / peak, "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg},
                 "e2e": {"value": alg / e2e_ms / 1e6, "unit": "GB/s", "h2d_bytes_per_step": 12 * cols, "d2h_bytes_per_step": 4 * rows},
                 "cpu_baseline": {"value": alg / cpu_s / 1e9, "unit": "GB/s", "cores": int(O.LIB.orc_num_threads()), "kind": "port",
-                                 "sample": "oracle matrix_mul_vec_packed (OpenMP) on 2^18 of 2^24 rows, scaled x64"},
+                                 "sample": "oracle matrix_mul_vec_packed (OpenMP) on 2^18 of 2^23 rows, scaled x32"},
                 "gpu_launches": args.steps}
         m.close()
     else:
@@ -377,17 +381,23 @@ def kernel_workload(args):
         G = S.Params(**kw)
         G.set_stream(stream.cuda_stream)
         count = 1 << 16
-        res = {}
+        res, dumps = {}, {}
         for poly_len, fn in ((2048, LIB.b200pir_ntt32_dev), (4096, LIB.b200pir_ntt4096_dev)):
-            x = torch.randint(0, Q1, (count * 2 * poly_len,), dtype=torch.int32, device="cuda")
+            gen = torch.Generator(device="cuda")
+            gen.manual_seed(poly_len)
+            x = torch.randint(0, Q1, (count * 2 * poly_len,), dtype=torch.int32, device="cuda", generator=gen)
             for name, inv in (("forward", 0), ("inverse", 1)):
                 if inv:
                     check(fn(G._h, x.data_ptr(), count, 0))               # inverse timed on canonical transform outputs
                 ms = timed(lambda: check(fn(G._h, x.data_ptr(), count, inv)))
+                if args.dump_outputs:
+                    dumps["ntt%d_%s" % (poly_len, name)] = x[: 1 << 20].cpu().numpy().view(np.uint32)
                 byt = 2 * count * 2 * poly_len * 4
                 res["%d_%s" % (poly_len, name)] = {"ms": ms, "polys_per_s": count / ms * 1e3, "GB/s_u32": byt / ms / 1e6,
                                                    "frac_of_hbm_peak_u32": byt / ms / 1e6 / peak}
             del x
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumps)
         f = res["2048_forward"]
         line = {"metric": "NTT throughput, 2^16 polynomials x 2 CRT moduli (28-bit), poly_len 2048 forward", "value": f["polys_per_s"],
                 "unit": "polynomials/s", "ms_per_step": f["ms"], "dtype": "u32",
@@ -432,20 +442,24 @@ def main():
                          "expanded queries overlaps the expansion / first dimension of the other")
     ap.add_argument("--mul-variant", type=int, default=0)
     ap.add_argument("--db-format", type=int, default=int(os.environ.get("B200PIR_BENCH_DB_FORMAT", "-1")),
-                    help="-1 = the library's choice (tcgen05 tile images wherever supported), 0 = IMAD layout, "
-                         "1 = mma.sync fragment order, 2 = tcgen05 tile images")
+                    help="-1 = the library's choice (wgmma tile images wherever supported), 0 = IMAD layout, "
+                         "1 = mma.sync fragment order, 2 = wgmma tile images")
     ap.add_argument("--fold-variant", type=int, default=2)
     ap.add_argument("--intt-variant", type=int, default=0)
     ap.add_argument("--imma-variant", type=int, default=0)
     ap.add_argument("--expand-variant", type=int, default=0)
     ap.add_argument("--queries-per-pass", type=int, default=None,
-                    help="queries per database pass (1, 2, 4, 8 or 16).  Default: 16 on the tcgen05 path (the pass stays "
+                    help="queries per database pass (1, 2, 4, 8 or 16).  Default: 16 on the wgmma path (the pass stays "
                          "HBM-bound), 8 on the mma.sync path (its 16-query pass is bound by the legacy tensor pipe)")
     ap.add_argument("--no-sweep", action="store_true", help="skip the concurrent-queries sweep (Q = 1, 32, 128; N = 1 only)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-verify", action="store_true",
                     help="N > 1: skip the correctness check of the NCCL flow (every rank recomputes its own queries of the last step "
                          "on an unsharded copy of the same database with the single-GPU path and compares the response bytes)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32 / float64): "
+                         "the response bytes of every query (main workloads), a seeded sample of the output rows (dpir), the "
+                         "transformed polynomials' first 2^20 words (ntt).  Inputs are seeded, so two builds compare output for output")
     ap.add_argument("--steps-only", action="store_true",
                     help="profiling aid: skip the single-query latency probe and the e2e leg (clean ncu launch lists)")
     args = ap.parse_args()
@@ -564,7 +578,7 @@ def main():
         exchange = args.exchange
         if exchange == "ce":
             try:
-                # tcgen05 databases: the expanded queries travel as UMMA tile images (one image per rank and wave, re-tiled once by
+                # wgmma databases: the expanded queries travel as operand tile images (one image per rank and wave, re-tiled once by
                 # the rank that expanded them); other layouts: uint4 [query][dim0][2048]
                 use_images = args.db_format == 2 and Blw <= 16
                 qexp_b = int(LIB.b200pir_query_image_bytes(G._h)) if use_images else Blw * d["dim0"] * POLY * 16
@@ -590,12 +604,11 @@ def main():
                         peer[(r,) + key] = ptr.value
                 copy_stream = torch.cuda.Stream()
                 # one stream per peer: pushes to different peers run on different copy engines at the same time (a single stream
-                # serialises them on one engine: 2.7 GB per step at N = 8 took ~14 ms, profiles/bench_r02_n8_single_copy_stream.json)
+                # serialises them on one engine)
                 peer_streams = {r: torch.cuda.Stream() for r in range(N) if r != rank}
                 tiny = [torch.zeros(1, dtype=torch.int32, device="cuda") for _ in range(W)]
                 # the "pushes landed" all-reduces get their own communicator: on the default one the survivors' all-gather of
-                # step k would queue behind barrier(k + 1), i.e. behind the whole transfer of step k + 1 (measured: 4.3 ms of a
-                # 12.8 ms step at N = 8, profiles/timeline_r02_n8.md)
+                # step k would queue behind barrier(k + 1), i.e. behind the whole transfer of step k + 1
                 bar_group = dist.new_group(backend="nccl")
                 prev_barrier = [None] * W
                 barriers = {}
@@ -749,6 +762,10 @@ def main():
     t_wall1 = time.time()
     clocks = sampler.stop(t_wall0, t_wall1)
     launches = LIB.b200pir_kernel_launches() - launches0
+    if args.dump_outputs:
+        # d_out = the responses of this rank's queries in the last timed step (Bl x response_bytes bytes)
+        keep = max(1, min(Bl, DUMP_LIMIT // (4 * rb * N)))        # the first queries' responses when all of them would exceed 64 MiB
+        dump_outputs(args.dump_outputs, {("responses" if N == 1 else "responses_rank%d" % rank): d_out.cpu().numpy().reshape(Bl, rb)[:keep]})
     ms_total = ev0.elapsed_time(ev1)
     if args.timeline and N > 1 and exchange == "ce":
         # where a step's time goes on this rank's streams (a separate, short pass; printed by every rank to stderr)
@@ -875,7 +892,7 @@ def main():
     db_bytes = d["slices"] * d["dim0"] * rows_local * POLY * 8
     if args.db_format == 0:
         operand_bytes = nq_per_launch * d["dim0"] * POLY * 16
-    elif args.db_format == 2:   # tcgen05 tile images of the query operand: [n][z][dim0/32][4096 B], 16 queries
+    elif args.db_format == 2:   # wgmma tile images of the query operand: [n][z][dim0/32][4096 B], 16 queries
         operand_bytes = 2 * POLY * ((d["dim0"] + 31) // 32) * 4096
     else:   # limb fragments of the query operand: [n][z][column tiles][dim0/32][4 limbs][32 lanes] x 8 B
         tiles = 4 if nq_per_launch > 8 else (2 if nq_per_launch > 4 else 1)
@@ -883,13 +900,12 @@ def main():
     alg_bytes = db_bytes + operand_bytes + nq_per_launch * d["slices"] * rows_local * 4 * POLY * 4
     peak, peak_src = measured_peak()
     achieved = alg_bytes / (mul_ms * 1e-3) / 1e9
-    kname = {0: "k_multiply (IMAD)", 1: "k_multiply_imma (INT8 MMA limbs)", 2: "k_multiply_tc5 (tcgen05 kind::i8 limbs)"}[args.db_format]
+    kname = {0: "k_multiply (IMAD)", 1: "k_multiply_imma (INT8 MMA limbs)", 2: "k_multiply_tc5 (wgmma u8 limbs)"}[args.db_format]
     roofline = {"bound": "hbm", "kernel": kname + " = multiply_reg_by_database, server.rs:155-221",
                 "queries_per_launch": nq_per_launch,
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic(name, B, args.db_format), "peak_source": peak_src,
+                "traffic": None, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": mul_ms,
-                "frac_of_nominal_8_tb_s": achieved / 8000.0,      # north_star quotes "~8 TB/s"; `frac` uses the measured copy peak
                 "kernel_share_of_step": stage["multiply"] / max(stage["total"], 1e-9),
                 "note": "kernel_ms = CUDA-event time of the multiply kernel alone; the re-tiling of the query operand that precedes it "
                         "is stage 'query_image'"}
@@ -919,7 +935,7 @@ def main():
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u64", "data": "synthetic",
             "config": {"workload": workload_name, "params": kw, "batch": B, "batch_per_gpu": B // N, "waves": W, "queries_per_pass": per_pass,
                        "exchange": (exchange if N > 1 else None), "pipelined": bool(N > 1 and exchange == "ce" and args.pipeline),
-                       "exchange_format": ("UMMA tile images" if (N > 1 and exchange == "ce" and use_images) else "uint4 [query][dim0][2048]") if N > 1 else None,
+                       "exchange_format": ("operand tile images" if (N > 1 and exchange == "ce" and use_images) else "uint4 [query][dim0][2048]") if N > 1 else None,
                        "db_bytes_per_gpu": db_bytes,
                        "plaintext_bytes": d["slices"] * d["dim0"] * d["num_per"] * POLY,
                        "first_dimension_kernel": kname,

@@ -1,4 +1,4 @@
-/* b200pir — C ABI of the B200-native server-side PIR query path.
+/* b200pir — C ABI of the GPU-native (H100, sm_90a) server-side PIR query path.
  *
  * This is the drop-in boundary: every entry point replaces one Rust function of blyssprivacy/sdk
  * (reference @ fdb7206); the Rust host code keeps its own signature and forwards here through a thin
@@ -53,13 +53,13 @@ int b200pir_ctx_set_stream(b200pir_ctx* ctx, void* cuda_stream);
 int b200pir_ctx_synchronize(b200pir_ctx* ctx);
 /* knobs: "mul_variant" (kernel tiling), "batch" (max queries per database pass: 1, 2, 4, 8 or 16;
  * the IMAD layout uses at most 4), "db_format" (layout of databases created afterwards: -1 = automatic (default): 2 wherever the
- * tcgen05 kernel supports the geometry, else 1; 0 = IMAD, 1 = mma.sync INT8 fragments, 2 = tcgen05 tile images, tc5_kernels.cu), "profile" (0 off, 1 per call,
+ * wgmma kernel supports the geometry, else 1; 0 = IMAD, 1 = mma.sync INT8 fragments, 2 = wgmma tile images, tc5_kernels.cu), "profile" (0 off, 1 per call,
  * 2 accumulate over calls until set again); A/B switches for kernel variants: "fold_variant", "intt_variant", "imma_variant",
  * "expand_variant" (0 = default everywhere); "coalesce" (1 = default: concurrent single-query callers
  * share database passes, see b200pir_coalesce_stats), "coalesce_window_us" (default 200: how long a batch that directly
  * follows a multi-query batch is held open for the callers of that batch to return; 0 = never), "sparse_fold" (1 = fold like lib/server's sparse server,
  * compute/fold.rs:15-65: an all-zero ciphertext short-cuts the external product; 0 = spiral-rs's dense fold, default); "expand_pair_min_ctas" (expansion rounds with at least this many active
- * ciphertexts use the paired kernel, default 592);
+ * ciphertexts use the paired kernel, default 528);
  * unknown keys -> B200PIR_E_BADARG */
 int b200pir_ctx_set_option(b200pir_ctx* ctx, const char* key, int64_t value);
 /* Size the context's workspace once, up front, for `queries` concurrent queries against a database with `rows_local`
@@ -103,7 +103,7 @@ int b200pir_db_fill_synthetic(b200pir_ctx* ctx, b200pir_db* db, uint64_t seed);
 int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes);
 /* lib/server's SparseDb (db/sparse_db.rs:5-47): an item exists once it has been written (upsert / update_item_raw; bulk uploads,
  * file loads and the synthetic fill write every item).  `items` = present items on this GPU, `capacity` = slices x local rows x
- * dim0.  Absent items are zero polynomials in HBM, so results equal the sparse server's sums; on the tcgen05 layout every
+ * dim0.  Absent items are zero polynomials in HBM, so results equal the sparse server's sums; on the wgmma layout every
  * 32-row x 32-j tile without a present item is neither fetched nor multiplied (multiply_reg_by_sparse_database skips absent
  * items, compute/dot_product.rs:35). */
 int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity);
@@ -210,7 +210,7 @@ int b200pir_expand_queries_dev(b200pir_ctx* ctx, b200pir_pp* pp, const uint64_t*
                                void* q_expanded_dev, uint32_t* v_folding_dev);
 int b200pir_first_dim_fold_dev(b200pir_ctx* ctx, b200pir_db* db, const void* q_expanded_dev, const uint32_t* v_folding_dev,
                                size_t count, uint32_t* partial_dev);
-/* The first two phases with the first-dimension operand exchanged as UMMA tile images (tcgen05-layout databases): the rank that
+/* The first two phases with the first-dimension operand exchanged as wgmma operand tile images (format-2 databases): the rank that
  * expands a group of <= 16 queries also re-tiles it, once (fused with reorient_reg_ciphertexts, util.rs:323-355); the receivers
  * multiply straight from the images.  image_dev: b200pir_query_image_bytes(ctx) bytes per group; partial_dev as above with
  * query index = group * per_group + i. */
@@ -247,7 +247,7 @@ int b200pir_dpir_create(int device, const uint32_t* a, uint64_t rows, uint64_t c
 /* synthetic a: word(i,k) = low 30 bits of splitmix64(seed, i*cols+k) */
 int b200pir_dpir_create_synthetic(int device, uint64_t rows, uint64_t cols, uint64_t seed, b200pir_dpir** out);
 /* Offline setup (lib/doublepir/src/doublepir/doublepir.rs:76-108): h_1 = db.data * a_1 and h_2 = h_1' * a_2 as exact 8-bit limb
- * products on the tcgen05 tensor cores (small signed left operand x 32-bit right operand, modulo 2^32), transpose / expand /
+ * products on the tensor cores (wgmma) (small signed left operand x 32-bit right operand, modulo 2^32), transpose / expand /
  * concat_cols / squish as small kernels.  Host pointers.  db: l x m, entries centred in [-p/2, p/2) as wrapping u32, p <= 2^10;
  * a1: m x n; a2: (l/x) x n; delta = params.delta(), x = db.info.x.  Outputs: db_squished l x ceil(m/3); h1_squished
  * (n delta x) x ceil((l/x)/3); a2_t n x ((l/x) rounded up to a multiple of 3); h2 (n delta x) x n. */

@@ -35,7 +35,7 @@ struct Rng {                       // xoshiro256**, seeded through splitmix64
 // ChaCha20 keystream as rand_chacha 0.3.1's ChaCha20Rng consumes it (lib/spiral-rs/Cargo.lock; call sites
 // client.rs:218, :309): RFC 8439 block function (20 rounds), 32-byte seed = key, 64-bit block counter in words 12-13
 // starting at 0, stream id (words 14-15) = 0, output words in keystream order, next_u64 = word[i] | word[i+1] << 32.
-// The crate is absent from /root/reference and the reference stores no serialized vectors, so this cannot be checked against
+// The crate is absent from the reference tree and the reference stores no serialized vectors, so this cannot be checked against
 // reference output here; it is pinned instead (tests/test_oracle_kats.py) by the RFC 8439 section 2.3.2 block vector and by
 // rand_chacha's own published known-answer test for ChaCha20Rng::from_seed([0; 32]) (first 32 output words = RFC 7539 A.1
 // vectors #1, #2), which fixes key placement, counter position / start / increment and word order.  How the call sites

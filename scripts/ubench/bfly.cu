@@ -1,7 +1,7 @@
-// Butterfly-rate microbenchmark on sm_100a: the NTT butterflies of sdk_b200/csrc/ntt_core.cuh on register-resident values
+// Butterfly-rate microbenchmark on sm_90a: the NTT butterflies of sdk_b200/csrc/ntt_core.cuh on register-resident values
 // (no shared memory, no barriers), i.e. the arithmetic bound of the transforms.  Prints warp-butterflies per clock per SM and the
 // equivalent clocks per 2048-point transform (11 264 butterflies = 352 warp-butterflies).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I ../../sdk_b200/csrc -o bfly bfly.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I ../../sdk_b200/csrc -o bfly bfly.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-// Pipe-rate microbenchmarks on sm_100a: legacy mma.sync variants and integer ops used by the NTT butterflies.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes pipes.cu ; prints per-SM per-clock rates.
+// Pipe-rate microbenchmarks on sm_90a: legacy mma.sync variants and integer ops used by the NTT butterflies.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes pipes.cu ; prints per-SM per-clock rates.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""In-tree build of libb200pir.so (sm_100a only).  Run as `python -m sdk_b200.build` or via
+"""In-tree build of libb200pir.so (sm_90a only).  Run as `python -m sdk_b200.build` or via
 __graft_entry__.build(); nvcc cross-compiles without a GPU."""
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libb200pir.so")
 SOURCES = ["api.cu", "poly_kernels.cu", "mul_kernels.cu", "imma_kernels.cu", "wire_kernels.cu", "tc5_kernels.cu", "dpir_gemm.cu"]
 HEADERS = ["common.cuh", "kernels.h", "ntt_core.cuh", "tc5_layout.cuh", "tc5_ptx.cuh", "ntt_core4096.cuh", "ntt_tables.hpp", os.path.join("..", "..", "include", "b200pir.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"]
 
 
@@ -37,7 +37,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError("nvcc failed on " + src)
-    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", SO] + objs + ["-ccbin", NVCC_FLAGS[-1]])
+    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", SO] + objs + ["-ccbin", NVCC_FLAGS[-1]])
     return SO
 
 

@@ -1,6 +1,6 @@
 // C-ABI implementation (include/b200pir.h): contexts, HBM-resident handles and the host-side
 // orchestration of spiral_rs::server::process_query (lib/spiral-rs/src/server.rs:650-741) as a
-// stream of sm_100a kernel launches.  No CPU fallback exists anywhere on this path: every entry
+// stream of sm_90a kernel launches.  No CPU fallback exists anywhere on this path: every entry
 // point either runs on the GPU or returns an error.
 #include "../../include/b200pir.h"
 #include "kernels.h"
@@ -96,13 +96,13 @@ struct b200pir_ctx {
   int fold_variant = 2;          // k_fold_res_lz at 3 CTAs per SM (default); 3: 2 CTAs per SM (A/B switch)
   int intt_variant = 0;
   int expand_variant = 0;        // wide rounds: 0 paired + residue pipeline (3 CTAs/SM), 2 paired single kernel; 1: never paired
-  long pair_min_ctas = 592;      // 4 x 148 SMs
+  long pair_min_ctas = 528;      // 4 x 132 SMs
   int sparse_fold = 0;           // 1: lib/server's fold (all-zero ciphertext shortcut, compute/fold.rs:37-43); 0: spiral-rs dense fold
   int imma_variant = 0;          // 0: cp.async-pipelined kernel for 5..8 queries per pass, 1: load-then-use kernel
-  int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the tcgen05 kernel
-                                 // supports the geometry, else 1), 0 = IMAD layout, 1 = mma.sync fragments, 2 = tcgen05 tile images
+  int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the wgmma kernel
+                                 // supports the geometry, else 1), 0 = IMAD layout, 1 = mma.sync fragments, 2 = wgmma tile images
   DevBuf<uint2> w_qf;            // B operand of the IMMA path (one group of <= 16 queries)
-  DevBuf<uint8_t> w_qt;          // B operand of the tcgen05 path (tile images, 16 queries)
+  DevBuf<uint8_t> w_qt;          // B operand of the wgmma path (tile images, 16 queries)
   int sm_count = 0;
   // workspace, sized for `ws_queries` queries
   size_t ws_queries = 0, ws_rows = 0;
@@ -219,7 +219,7 @@ struct b200pir_db {
   b200pir_ctx* ctx;
   Shard shard;
   int rows;                 // local second-dimension rows
-  int format = 0;           // 0: d (IMAD layout)  1: f (INT8 MMA fragment order)  2: t (tcgen05 tile images)
+  int format = 0;           // 0: d (IMAD layout)  1: f (INT8 MMA fragment order)  2: t (wgmma tile images)
   DevBuf<uint4> d;          // [slice][row][dim0/2][2048]
   DevBuf<uint4> f;          // [slice][n][z][mt][ks][limb][lane]
   DevBuf<uint8_t> t;        // format 2: [slice][n][z][mt][ks][4096 B] tile images (tc5_kernels.cu)
@@ -227,7 +227,7 @@ struct b200pir_db {
   ImmaGeom F;
   size_t slice_cells() const { return (size_t)rows * (ctx->dim0 / 2) * POLY; }
   // Presence (lib/server's SparseDb, db/sparse_db.rs:5-47: an item exists once it has been written).  Storage stays dense in HBM
-  // (absent = zero polynomial, so every sum is unchanged); what the map buys is COST: on the tcgen05 path whole 32-row x 32-j
+  // (absent = zero polynomial, so every sum is unchanged); what the map buys is COST: on the wgmma path whole 32-row x 32-j
   // tiles without a present item are neither fetched nor multiplied (tile_mask, one bit per tile, kept on the device).
   std::vector<uint64_t> present;          // bit ((slice * rows + il) * dim0 + j)
   uint64_t present_count = 0;
@@ -370,8 +370,8 @@ void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size
 }
 
 // server.rs:525-591 for `nq` queries.  v: [nq][2^g][4][2048]; writes v_fold of every query and the first-dimension operand:
-// q_dev (uint4 [query][dim0][2048], reorient_reg_ciphertexts util.rs:323-355) or, when `images` is given (tcgen05 databases),
-// the UMMA tile images of groups of 16 queries directly (image g = queries 16g .., tc5_query_bytes apart): no intermediate.
+// q_dev (uint4 [query][dim0][2048], reorient_reg_ciphertexts util.rs:323-355) or, when `images` is given (format-2 databases),
+// the operand tile images of groups of 16 queries directly (image g = queries 16g .., tc5_query_bytes apart): no intermediate.
 void run_expand_query(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_raw, uint32_t* v, uint4* q_dev,
                       uint32_t* v_fold, int nq, uint8_t* images = nullptr) {
   const auto& hp = c->hp;
@@ -464,7 +464,7 @@ void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const 
       launch_ntt32(c->dp, c->w_mult.p, count * c->slices * rows * 2, true, c->stream);
     }
   } else if (db->format == 2) {
-    // tcgen05 path: same z-major product as the mma.sync path, 16 queries per database pass
+    // wgmma path: same z-major product as the mma.sync path, 16 queries per database pass
     if (!images) c->w_qt.ensure(tc5_query_bytes(db->T));
     const size_t step = images ? per_group : 16;
     for (size_t qi = 0, g = 0; qi < count; qi += step, g++) {
@@ -750,7 +750,7 @@ int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count
     db->d.alloc(cells);
     B200_CUDA(cudaMemsetAsync(db->d.p, 0, cells * sizeof(uint4), c->stream));
   } else if (db->format == 2) {
-    if (!tc5_supported(db->T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the tcgen05 kernel");
+    if (!tc5_supported(db->T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
     size_t bytes = tc5_db_bytes(db->T, c->slices);
     db->t.alloc(bytes);
     B200_CUDA(cudaMemsetAsync(db->t.p, 0, bytes, c->stream));
@@ -1409,7 +1409,7 @@ int b200pir_encode(b200pir_ctx* c, const uint64_t* v_packed_raw, uint8_t* out, s
 
 // ---------------------------------------------------------------- process_query
 static void run_query_batch_resident(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, size_t count, uint8_t* out_dev) {
-  // queries are already in c->w_query; tcgen05 databases get their operand as tile images straight from the expansion
+  // queries are already in c->w_query; format-2 databases get their operand as tile images straight from the expansion
   const bool images = db->format == 2 && c->hp.expand_queries;
   run_prepare(c, pp, count, images);
   run_first_dim_and_fold(c, db, count, nullptr, nullptr, images ? c->w_qt.p : nullptr, 16);
@@ -1661,7 +1661,7 @@ int b200pir_first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* q_exp
   B200_CUDA(cudaGetLastError());
   API_END
 }
-// The same two phases with the first-dimension operand exchanged as UMMA tile images (tcgen05 databases): the rank that expands a
+// The same two phases with the first-dimension operand exchanged as operand tile images (format-2 databases): the rank that expands a
 // group of <= 16 queries also re-tiles it, once; the receivers multiply straight from the image.
 size_t b200pir_query_image_bytes(b200pir_ctx* c) { return c ? tc5_query_bytes(make_tc5_geom(c->dim0, 32)) : 0; }
 int b200pir_expand_queries_images_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count, void* image_dev,
@@ -1672,7 +1672,7 @@ int b200pir_expand_queries_images_dev(b200pir_ctx* c, b200pir_pp* pp, const uint
   check_pp(c, pp);
   if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "needs expand_queries");
   if (count == 0 || count > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
-  if (!tc5_supported(make_tc5_geom(c->dim0, 32))) throw Error(B200PIR_E_UNSUPPORTED, "dim0 too large for the tcgen05 kernel");
+  if (!tc5_supported(make_tc5_geom(c->dim0, 32))) throw Error(B200PIR_E_UNSUPPORTED, "dim0 too large for the wgmma kernel");
   c->w_v.ensure(count * c->v_words());
   c->prof_reset();
   {
@@ -1688,7 +1688,7 @@ int b200pir_first_dim_fold_images_dev(b200pir_ctx* c, b200pir_db* db, const void
   if (!c || !images_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
-  if (db->format != 2) throw Error(B200PIR_E_BADARG, "tile images need a tcgen05-layout database (db_format 2)");
+  if (db->format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
   if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
   const size_t count = groups * per_group;
   if (count == 0) return 0;

@@ -1,4 +1,4 @@
-// Shared device/host definitions for the B200 PIR kernels (sm_100a only).
+// Shared device/host definitions for the PIR kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

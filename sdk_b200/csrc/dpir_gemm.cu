@@ -1,4 +1,4 @@
-// DoublePIR offline setup (lib/doublepir/src/doublepir/doublepir.rs:76-108) on the 5th-generation tensor cores.
+// DoublePIR offline setup (lib/doublepir/src/doublepir/doublepir.rs:76-108) on the Hopper tensor cores (wgmma).
 //
 // The two products of setup(),  h_1 = db.data * a_1  and  h_2 = h_1' * a_2  (matrix/ops.rs:169-191, wrapping u32), have a SMALL
 // signed left operand (database entries / base-p digits centred in [-p/2, p/2), p <= 2^10) and a full 32-bit right operand.
@@ -6,15 +6,15 @@
 //     a = a0 + 2^8 a1        a0 = a & 255 (unsigned),  a1 = a >> 8 (arithmetic, signed, |a| < 2^15)
 //     b = b0 + 2^8 b1 + 2^16 b2 + 2^24 b3   (unsigned bytes)
 //     a b = sum_{i + j <= 3} a_i b_j 2^{8 (i + j)}            (terms with i + j >= 4 vanish mod 2^32)
-// Seven limb products per k-step, grouped by shift s = i + j into four s32 accumulators in TMEM (kind::i8 with the signedness of
-// each operand set per instruction; no saturation, so the accumulators wrap modulo 2^32 — and only their low 32 - 8 s bits
-// matter):  D0 = a0 b0,  D1 = a0 b1 + a1 b0,  D2 = a0 b2 + a1 b1,  D3 = a0 b3 + a1 b2;  c = D0 + D1 << 8 + D2 << 16 + D3 << 24.
+// Seven limb products per k-step, grouped by shift s = i + j into four s32 register accumulators (wgmma .u8.u8 or .s8.u8 per
+// instruction; no saturation, so the accumulators wrap modulo 2^32 — and only their low 32 - 8 s bits matter):  D0 = a0 b0,  D1 = a0 b1 + a1 b0,  D2 = a0 b2 + a1 b1,  D3 = a0 b3 + a1 b2;  c = D0 + D1 << 8 + D2 << 16 + D3 << 24.
 //
 // Operand images: each limb plane of A ([M][K] bytes) and of B' ([N][K] bytes, i.e. B transposed) is stored as 128 x 32 byte
-// tiles in the canonical K-major no-swizzle layout of tc5_layout.cuh, so a tile is one bulk copy.  One CTA per 128 x 128
-// output tile: warp 0 = producer (ring of k-steps: 2 A tiles + 4 B tiles = 24 KiB per stage), warp 1 = MMA issue, warps 2-5 =
-// epilogue (TMEM -> registers -> global).  This is an offline step; the kernel is written for exactness and clarity, not
-// tuned beyond keeping the tensor pipe fed.
+// tiles in the canonical K-major no-swizzle layout of tc5_layout.cuh, so a tile (or a 32-row quarter of it) is one bulk copy.
+// One CTA per 128 x 32 output tile (128 rows of A, one 32-row quarter of a B' tile): warpgroups 0 and 1 compute rows 0..63
+// and 64..127 (four 64 x 32 accumulators = 64 registers a thread: wider tiles push ptxas into spilling accumulators of
+// in-flight MMAs), warp 8 = producer (ring of k-steps: 2 A tiles + 4 B quarter tiles = 12 KiB per stage).  This is an offline step; the kernel is written for exactness and clarity, not tuned beyond
+// keeping the tensor pipe fed.
 #include "kernels.h"
 #include "tc5_ptx.cuh"
 
@@ -23,14 +23,11 @@ namespace b200pir {
 namespace {
 using namespace tc5;
 
-constexpr int G_STAGES = 6;
-constexpr int G_STAGE_BYTES = 6 * TC5_TILE;             // a0, a1, b0, b1, b2, b3
-constexpr int G_THREADS = 192;
-
-// instruction descriptor: D = s32, dense, no saturation, K-major operands, M = N = 128, with A's signedness selectable
-__host__ __device__ inline uint32_t gemm_idesc(bool a_signed) {
-  return (2u << 4) | ((a_signed ? 1u : 0u) << 7) | (0u << 10) | ((uint32_t)(TC5_N >> 3) << 17) | ((uint32_t)(TC5_M >> 4) << 24);
-}
+constexpr int G_STAGES = 8;
+constexpr int G_HALF = TC5_TILE / 2;                    // rows 64..127 of a tile image: 8 row groups = 2048 bytes
+constexpr int G_QUARTER = TC5_TILE / 4;                 // 32 rows of a tile image: 4 row groups = 1024 bytes
+constexpr int G_STAGE_BYTES = 2 * TC5_TILE + 4 * G_QUARTER; // a0, a1, b0, b1, b2, b3 (32 rows of B')
+constexpr int G_THREADS = 2 * 128 + 32;
 
 // limb planes of A (row-major rows x cols u32, small signed entries) as tile images [plane(2)][mt][ks][4096]
 __global__ void k_gemm_a_image(uint8_t* __restrict__ img, const uint32_t* __restrict__ a, size_t rows, size_t cols, int mt, int ks) {
@@ -77,103 +74,87 @@ __global__ void k_gemm_b_image(uint8_t* __restrict__ img, const uint32_t* __rest
 
 struct GemmSmem {
   uint64_t full[G_STAGES], empty[G_STAGES];
-  uint64_t done;
-  uint32_t tmem_base;
 };
 
-// c[m][n] = sum_k a[m][k] b[k][n] mod 2^32 for one 128 x 128 tile per CTA (grid = (nt, mt))
+// c[m][n] = sum_k a[m][k] b[k][n] mod 2^32 for one 128 x 32 tile per CTA (grid = (4 nt, mt))
 __global__ void __launch_bounds__(G_THREADS, 1)
 k_dpir_gemm(const uint8_t* __restrict__ a_img, const uint8_t* __restrict__ b_img, uint32_t* __restrict__ c, size_t rows, size_t n_cols,
             int mt, int nt, int ks) {
   extern __shared__ __align__(1024) uint8_t gsm[];
   GemmSmem* S = reinterpret_cast<GemmSmem*>(gsm + (size_t)G_STAGES * G_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_t = blockIdx.x, m_t = blockIdx.y;
+  const int n_t = blockIdx.x >> 2, n_q = blockIdx.x & 3, m_t = blockIdx.y;
   const size_t a_plane = (size_t)mt * ks * TC5_TILE, b_plane = (size_t)nt * ks * TC5_TILE;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < G_STAGES; s++) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 1); }
-    mbar_init(&S->done, 1);
+    for (int s = 0; s < G_STAGES; s++) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S->tmem_base)), "n"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S->tmem_base;
 
-  if (warp == 0) {
+  if (warp == 8) {
     int stage = 0; uint32_t phase = 0;
     for (int k = 0; k < ks; k++) {
       mbar_wait(&S->empty[stage], phase ^ 1);
       if (elect_one()) {
         uint8_t* dst = gsm + (size_t)stage * G_STAGE_BYTES;
         mbar_expect_tx(&S->full[stage], G_STAGE_BYTES);
-        const size_t a_off = ((size_t)m_t * ks + k) * TC5_TILE, b_off = ((size_t)n_t * ks + k) * TC5_TILE;
+        const size_t a_off = ((size_t)m_t * ks + k) * TC5_TILE, b_off = ((size_t)n_t * ks + k) * TC5_TILE + n_q * G_QUARTER;
         bulk_g2s(dst + 0 * TC5_TILE, a_img + a_off, TC5_TILE, &S->full[stage]);
         bulk_g2s(dst + 1 * TC5_TILE, a_img + a_plane + a_off, TC5_TILE, &S->full[stage]);
 #pragma unroll
-        for (int j = 0; j < 4; j++) bulk_g2s(dst + (2 + j) * TC5_TILE, b_img + j * b_plane + b_off, TC5_TILE, &S->full[stage]);
+        for (int j = 0; j < 4; j++) bulk_g2s(dst + 2 * TC5_TILE + j * G_QUARTER, b_img + j * b_plane + b_off, G_QUARTER, &S->full[stage]);
       }
       __syncwarp();
       if (++stage == G_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1) {
-    int stage = 0; uint32_t phase = 0;
-    const uint32_t id_u = gemm_idesc(false), id_s = gemm_idesc(true);
+  } else if (warp < 8) {
+    const int wg = warp >> 2, w = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint32_t d0[16], d1[16], d2[16], d3[16];                          // shift s accumulates into ds
+#pragma unroll
+    for (int i = 0; i < 16; i++) { d0[i] = 0; d1[i] = 0; d2[i] = 0; d3[i] = 0; }
+    int stage = 0, prev = -1; uint32_t phase = 0;
     for (int k = 0; k < ks; k++) {
       mbar_wait(&S->full[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t base = smem_u32(gsm + (size_t)stage * G_STAGE_BYTES);
-        const uint64_t a0 = tc5_smem_desc(base), a1 = tc5_smem_desc(base + TC5_TILE);
-        uint64_t bd[4];
+      const uint32_t base = smem_u32(gsm + (size_t)stage * G_STAGE_BYTES);
+      const uint64_t a0 = tc5_smem_desc(base + wg * G_HALF), a1 = tc5_smem_desc(base + TC5_TILE + wg * G_HALF);
+      uint64_t bd[4];
 #pragma unroll
-        for (int j = 0; j < 4; j++) bd[j] = tc5_smem_desc(base + (2 + j) * TC5_TILE);
-        const uint32_t acc = k > 0 ? 1u : 0u;
-        // shift s accumulates into TMEM columns [128 s, 128 s + 128)
-        tc_mma_i8(tmem_base + 0 * TC5_N, a0, bd[0], acc, id_u);
-        tc_mma_i8(tmem_base + 1 * TC5_N, a0, bd[1], acc, id_u);
-        tc_mma_i8(tmem_base + 1 * TC5_N, a1, bd[0], 1u, id_s);
-        tc_mma_i8(tmem_base + 2 * TC5_N, a0, bd[2], acc, id_u);
-        tc_mma_i8(tmem_base + 2 * TC5_N, a1, bd[1], 1u, id_s);
-        tc_mma_i8(tmem_base + 3 * TC5_N, a0, bd[3], acc, id_u);
-        tc_mma_i8(tmem_base + 3 * TC5_N, a1, bd[2], 1u, id_s);
-        tc_commit(&S->empty[stage]);
-        if (k == ks - 1) tc_commit(&S->done);
-      }
-      __syncwarp();
+      for (int j = 0; j < 4; j++) bd[j] = tc5_smem_desc(base + 2 * TC5_TILE + j * G_QUARTER);
+      wgmma_fence();
+      wgmma_m64n32k32<false>(d0, a0, bd[0]);
+      wgmma_m64n32k32<false>(d1, a0, bd[1]);
+      wgmma_m64n32k32<true>(d1, a1, bd[0]);
+      wgmma_m64n32k32<false>(d2, a0, bd[2]);
+      wgmma_m64n32k32<true>(d2, a1, bd[1]);
+      wgmma_m64n32k32<false>(d3, a0, bd[3]);
+      wgmma_m64n32k32<true>(d3, a1, bd[2]);
+      wgmma_commit();
+      wgmma_wait<1>();                                                // the previous stage's MMAs have completed: release it
+      if (prev >= 0 && leader) mbar_arrive(&S->empty[prev]);
+      prev = stage;
       if (++stage == G_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // epilogue: warp w owns TMEM lanes 32 (w % 4) .. + 31 = output rows of the tile
-    const int quad = warp & 3;
-    mbar_wait(&S->done, 0);
-    tc_fence_after();
-    const size_t row = (size_t)m_t * 128 + quad * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-    for (int cb = 0; cb < 4; cb++) {                     // 32 output columns at a time
-      uint32_t d0[32], d1[32], d2[32], d3[32];
-      tc_ld32(taddr + 0 * TC5_N + cb * 32, d0);
-      tc_ld32(taddr + 1 * TC5_N + cb * 32, d1);
-      tc_ld32(taddr + 2 * TC5_N + cb * 32, d2);
-      tc_ld32(taddr + 3 * TC5_N + cb * 32, d3);
-      tc_wait_ld();
-      if (row < rows) {
+    wgmma_wait<0>();
+    wgmma_fence_operands(d0);
+    wgmma_fence_operands(d1);
+    wgmma_fence_operands(d2);
+    wgmma_fence_operands(d3);
+    // accumulator fragment: d[4 i + 2 h + e] = D[16 w + lane/4 + 8 h][8 i + 2 (lane%4) + e]
 #pragma unroll
-        for (int i = 0; i < 32; i++) {
-          const size_t col = (size_t)n_t * 128 + cb * 32 + i;
-          if (col < n_cols) c[row * n_cols + col] = d0[i] + (d1[i] << 8) + (d2[i] << 16) + (d3[i] << 24);
+    for (int h = 0; h < 2; h++) {
+      const size_t row = (size_t)m_t * 128 + wg * 64 + w * 16 + (lane >> 2) + 8 * h;
+      if (row >= rows) continue;
+#pragma unroll
+      for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const int r = 4 * i + 2 * h + e;
+          const size_t col = (size_t)n_t * 128 + n_q * 32 + 8 * i + 2 * (lane & 3) + e;
+          if (col < n_cols) c[row * n_cols + col] = d0[r] + (d1[r] << 8) + (d2[r] << 16) + (d3[r] << 24);
         }
-      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
 }
 
 // doublepir.rs:83-85: transpose, expand (matrix/contract.rs:62-78: delta digits base p, centred), concat_cols (indexing.rs:82-101)
@@ -224,7 +205,7 @@ void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t 
   k_gemm_b_image<<<blocks((size_t)nt * ks * 1024, 256), 256, 0, s>>>(b_img, b, k_dim, n_cols, nt, ks);
   const size_t smem = (size_t)G_STAGES * G_STAGE_BYTES + sizeof(GemmSmem) + 16;
   opt_in_smem(k_dpir_gemm, (int)smem);
-  k_dpir_gemm<<<dim3(nt, mt), G_THREADS, smem, s>>>(a_img, b_img, c, rows, n_cols, mt, nt, ks);
+  k_dpir_gemm<<<dim3(4 * nt, mt), G_THREADS, smem, s>>>(a_img, b_img, c, rows, n_cols, mt, nt, ks);
   cudaError_t e = cudaStreamSynchronize(s);
   cudaFree(a_img);
   cudaFree(b_img);

@@ -1,4 +1,4 @@
-// Launch wrappers (host side) for the sm_100a kernels.  All pointers are DEVICE pointers unless
+// Launch wrappers (host side) for the sm_90a kernels.  All pointers are DEVICE pointers unless
 // noted; every launch goes to the given stream and returns immediately.
 //
 // Device formats
@@ -102,7 +102,7 @@ void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32
 // z-major product of one slice -> ntt32 [row][ct_row][n][z]
 void launch_zmajor_to_ntt32(const ImmaGeom& F, const uint32_t* in_zm, uint32_t* out, int slice, cudaStream_t s);
 
-// ---- first dimension on tcgen05 (tc5_kernels.cu): operands stored as shared-memory tile images (database format 2)
+// ---- first dimension on wgmma (tc5_kernels.cu): operands stored as shared-memory tile images (database format 2)
 size_t tc5_db_bytes(const Tc5Geom& T, int slices);
 size_t tc5_query_bytes(const Tc5Geom& T);                 // 16 queries
 bool tc5_supported(const Tc5Geom& T);
@@ -190,7 +190,7 @@ void launch_dpir_transpose_expand(uint32_t* out, const uint32_t* a, size_t rows,
 
 // ---- DoublePIR offline setup (dpir_gemm.cu): doublepir.rs:76-108
 // c (rows x n_cols) = a (rows x k_dim, entries in [-2^15, 2^15) as wrapping u32) * b (k_dim x n_cols) mod 2^32; device pointers;
-// 8-bit limb products on the tcgen05 tensor cores (exact); synchronises the stream
+// 8-bit limb products on the tensor cores (wgmma) (exact); synchronises the stream
 void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t rows, size_t k_dim, size_t n_cols, cudaStream_t s);
 // transpose + expand (contract.rs:62-78) + concat_cols (indexing.rs:82-101): h (l x n) -> out ((n delta x) x (l / x)), centred digits
 void launch_dpir_transpose_expand_concat(uint32_t* out, const uint32_t* h, size_t l, size_t n, uint32_t p, int delta, size_t x,

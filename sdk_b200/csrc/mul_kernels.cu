@@ -484,7 +484,7 @@ void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, siz
   }
   if ((cols & 1) == 0 && variant != 1 && variant != 4) {
     // default: one row per warp, 8 loads in flight per lane (variant 2: 4 loads)
-    unsigned g = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)148 * 8);
+    unsigned g = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)132 * 8);
     ++g_kernel_launches;
     if (variant == 2) {
       cudaFuncSetAttribute(k_dpir_matvec_row<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -497,7 +497,7 @@ void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, siz
   }
   const int rows_per_warp = variant == 1 ? 2 : 4;
   size_t warps_needed = (rows + rows_per_warp - 1) / rows_per_warp;
-  unsigned grid = (unsigned)std::min<size_t>((warps_needed + 7) / 8, (size_t)148 * 8);
+  unsigned grid = (unsigned)std::min<size_t>((warps_needed + 7) / 8, (size_t)132 * 8);
   if (grid == 0) return;
   if (rows_per_warp == 2) {
     cudaFuncSetAttribute(k_dpir_matvec<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -1,5 +1,5 @@
 // 2048-point negacyclic NTT over one 28-bit CRT modulus, computed cooperatively by a group of
-// 256 threads holding 8 coefficients each (sm_100a; also compiles as plain C++ so the index /
+// 256 threads holding 8 coefficients each (sm_90a; also compiles as plain C++ so the index /
 // twiddle logic can be emulated thread-by-thread on the CPU, tests/test_ntt_core_emulation.py).
 //
 // Semantics follow the reference's scalar transforms exactly (lib/spiral-rs/src/ntt.rs:67-113

@@ -1,4 +1,4 @@
-// Ring-arithmetic kernels for the Spiral second dimension, query expansion and packing (sm_100a).
+// Ring-arithmetic kernels for the Spiral second dimension, query expansion and packing (sm_90a).
 //
 // Every kernel here runs CTAs of 512 threads = two groups of 256; group g works modulo q_g, so the
 // two CRT halves of a polynomial are transformed side by side and can be CRT-lifted inside the CTA.

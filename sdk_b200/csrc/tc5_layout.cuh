@@ -1,6 +1,6 @@
-// Index / limb arithmetic of the tcgen05 first dimension (tc5_kernels.cu), as __host__ __device__ functions so that the
+// Index / limb arithmetic of the wgmma first dimension (tc5_kernels.cu), as __host__ __device__ functions so that the
 // operand images and the epilogue can be emulated thread by thread on the CPU (tests/cpp/tc5_emul.cpp) against the
-// canonical UMMA shared-memory layout (K-major, no swizzle: cute/atom/mma_traits_sm100.hpp, make_umma_desc<Major::K>).
+// canonical K-major, no-swizzle shared-memory layout of wgmma operands (PTX ISA, "Shared Memory Matrix Layout").
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -36,21 +36,14 @@ TC5_HD uint32_t tc5_limb4(const uint32_t (&r)[4], int l) {
   return ((r[0] >> sh) & 127u) | (((r[1] >> sh) & 127u) << 8) | (((r[2] >> sh) & 127u) << 16) | (((r[3] >> sh) & 127u) << 24);
 }
 
-// ---- descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp; cross-checked against those structs by
-// tests/cpp/tc5_desc_check.cu)
-// shared-memory matrix descriptor: start address, LBO, SBO in 16-byte units, version 1 (Blackwell), SWIZZLE_NONE (0)
+// ---- shared-memory matrix descriptor of wgmma (PTX ISA, "Matrix Descriptor Format"; checked field by field by
+// tests/cpp/tc5_desc_check.cpp): start address, LBO, SBO in 16-byte units, base offset 0, layout type 0 (no swizzle)
 TC5_HD uint64_t tc5_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);           // [0,14)   start address
   d |= (uint64_t)((TC5_LBO >> 4) & 0x3FFF) << 16;       // [16,30)  leading-dimension byte offset (K halves)
   d |= (uint64_t)((TC5_SBO >> 4) & 0x3FFF) << 32;       // [32,46)  stride byte offset (8-row groups)
-  d |= (uint64_t)1 << 46;                               // [46,48)  descriptor version
-  return d;
-}
-// instruction descriptor: D = s32, A = B = unsigned 8 bit, both K-major, dense, no saturation, M = 128, N = 128
-TC5_HD uint32_t tc5_instr_desc() {
-  return (2u << 4) /* c_format S32 */ | (0u << 7) /* a u8 */ | (0u << 10) /* b u8 */ | (0u << 15) | (0u << 16) |
-         ((uint32_t)(TC5_N >> 3) << 17) | ((uint32_t)(TC5_M >> 4) << 24);
+  return d;                                             // [49,52) base offset 0, [62,64) no swizzle
 }
 
 // ---- database image: thread tid of the CTA of row tile mt / k-step ks handles one row and four consecutive j
@@ -80,22 +73,29 @@ TC5_HD void tc5_query_store(uint8_t* tile, int q, int r, int k, uint32_t value) 
   for (int m = 0; m < 4; m++) tile[tc5_tile_off(tc5_n_index(2 * q + r, m), k)] = (uint8_t)((value >> (7 * m)) & 127u);
 }
 
-// ---- epilogue: TMEM lane = M index; a warp owns the quadrant `quad` (32 lanes), a chunk is 32 consecutive columns
-// (8 GEMM columns x 4 query limbs m).  Lane (row, l) holds D[4 row + l][4 col + m] = sum_j a_l(row, j) b_m(j, col) < 2^24.
-// The residue is  sum_{l,m} D_{l,m} 2^{7(l+m)} mod q:
-//   1. per lane and column: s = sum_m D_{l,m} 2^{7m} (< 2^47, shifts and adds), split at bit 23 and weighted with
-//      w_l = 2^{7l} mod q, w'_l = 2^{7l+23} mod q:  P = (s mod 2^23) w_l + (s >> 23) w'_l  < 2^53   (two wide multiply-adds)
-//   2. reduce-scatter over the four limb lanes of a row (xor 2, then xor 1): lane l ends with the sums (< 2^55) of the two
-//      columns 2l, 2l+1 it stores = both ciphertext rows of query 4 chunk + l
+// ---- epilogue.  Two consumer warpgroups; warpgroup wg computes M rows [64 wg, 64 wg + 64) of the 128 x 128 tile with
+// wgmma.m64n128k32, whose s32 accumulator fragment gives thread (warp w of the warpgroup, lane) the 64 values
+//     acc[4 i + 2 h + c] = D[64 wg + 16 w + lane/4 + 8 h][8 i + 2 (lane%4) + c]          (i < 16, h < 2, c < 2)
+// i.e. database row (M/4) 16 wg + 4 w + lane/16 + 2 h, limb l = (lane/4) % 4, GEMM column (N/4) 2 i + (lane/2) % 2 = query i,
+// ciphertext row (lane/2) % 2, and the two query limbs m = 2 (lane%2) + c.  The residue is  sum_{l,m} D_{l,m} 2^{7(l+m)} mod q:
+//   1. per (i, h): s = D_{l,m0} + D_{l,m0+1} 2^7 (< 2^32), split at bit 23 and weighted with w = 2^{7(l+m0)} mod q,
+//      w' = 2^{7(l+m0)+23} mod q:  P = (s mod 2^23) w + (s >> 23) w'  < 2^52            (two wide multiply-adds)
+//   2. reduce-scatter of the 32 partials over the eight lanes of a (row, column) that hold its four l and two m0
+//      (lane bits 0, 2, 3), halving the top bit of the partial index each round: each lane keeps four sums (< 2^55)
 //   3. one Barrett reduction per stored word, with 32-bit operations (tc5_barrett57).
-TC5_HD int tc5_lane_row(int quad, int lane) { return quad * 8 + (lane >> 2); }     // row_local of this lane
-TC5_HD int tc5_lane_limb(int lane) { return lane & 3; }
-TC5_HD int tc5_lane_query(int chunk, int lane) { return chunk * 4 + (lane & 3); }  // the query this lane stores
+TC5_HD int tc5_frag_row(int wg, int w, int lane, int h) { return 16 * wg + 4 * w + (lane >> 4) + 2 * h; }   // row_local
+TC5_HD int tc5_frag_limb(int lane) { return (lane >> 2) & 3; }
+TC5_HD int tc5_frag_ctrow(int lane) { return (lane >> 1) & 1; }
+// the query of the f-th kept sum (f < 4) after the reduce-scatter; its row half is h = f & 1
+TC5_HD int tc5_frag_query(int lane, int f) { return ((lane & 1) << 3) | (((lane >> 2) & 1) << 2) | (((lane >> 3) & 1) << 1) | (f >> 1); }
+// the lane bit each reduce-scatter round exchanges over (partner = lane ^ (1 << bit))
+TC5_HD int tc5_rs_lane_bit(int round) { return round == 0 ? 0 : (round == 1 ? 2 : 3); }
 struct Tc5Weights { uint32_t w, wp, mu; };
-TC5_HD Tc5Weights tc5_lane_weights(int l, uint32_t q) {
+TC5_HD Tc5Weights tc5_lane_weights(int lane, uint32_t q) {
+  const int e = 7 * (tc5_frag_limb(lane) + 2 * (lane & 1));
   Tc5Weights W;
-  W.w = (uint32_t)((1ull << (7 * l)) % q);
-  W.wp = (uint32_t)((1ull << (7 * l + 23)) % q);
+  W.w = (uint32_t)((1ull << e) % q);
+  W.wp = (uint32_t)((1ull << (e + 23)) % q);
   W.mu = (uint32_t)((1ull << 58) / q);                                             // q > 2^27, so mu < 2^31
   return W;
 }
@@ -112,21 +112,16 @@ TC5_HD uint32_t tc5_barrett57(uint64_t x, uint32_t mu, uint32_t q) {
   const uint32_t r2 = r - q;
   return r < r2 ? r : r2;
 }
-// step 1 for one GEMM column: v4 = the four m-limb accumulators of this lane
-TC5_HD uint64_t tc5_lane_partial(const uint32_t* v4, uint32_t w, uint32_t wp) {
-  const uint32_t a = v4[0] + (v4[1] << 7), b = v4[2] + (v4[3] << 7);               // < 2^32 each (D < 2^24)
-  const uint64_t s = (uint64_t)a + ((uint64_t)b << 14);                            // < 2^47
-  return (uint64_t)((uint32_t)s & 0x7FFFFFu) * w + (uint64_t)(uint32_t)(s >> 23) * wp;
+// step 1 for one (i, h): v0, v1 = the accumulators of query limbs m0, m0 + 1
+TC5_HD uint64_t tc5_lane_partial(uint32_t v0, uint32_t v1, uint32_t w, uint32_t wp) {
+  const uint32_t s = v0 + (v1 << 7);                                               // < 2^32 (D < 2^24)
+  return (uint64_t)(s & 0x7FFFFFu) * w + (uint64_t)(s >> 23) * wp;
 }
-// step 2, first exchange (partner = lane ^ 2): lanes with limb bit 1 clear keep columns 0..3 and send 4..7, the others the
-// opposite; second exchange (partner = lane ^ 1): of the four kept columns, lanes with limb bit 0 clear keep the first two.
-TC5_HD void tc5_rs_select_a(int l, const uint64_t (&P)[8], uint64_t (&send)[4], uint64_t (&keep)[4]) {
-  const bool up = (l & 2) != 0;
-  for (int i = 0; i < 4; i++) { send[i] = up ? P[i] : P[4 + i]; keep[i] = up ? P[4 + i] : P[i]; }
-}
-TC5_HD void tc5_rs_select_b(int l, const uint64_t (&K)[4], uint64_t (&send)[2], uint64_t (&keep)[2]) {
-  const bool odd = (l & 1) != 0;
-  for (int i = 0; i < 2; i++) { send[i] = odd ? K[i] : K[2 + i]; keep[i] = odd ? K[2 + i] : K[i]; }
+// step 2, one round over NIN partials: a lane whose exchange bit is `up` keeps the upper half of the index range and sends the
+// lower half, the others the opposite; the partner adds what it receives to what it keeps, entry by entry
+template <int NIN>
+TC5_HD void tc5_rs_split(bool up, const uint64_t (&in)[NIN], uint64_t (&send)[NIN / 2], uint64_t (&keep)[NIN / 2]) {
+  for (int r = 0; r < NIN / 2; r++) { send[r] = up ? in[r] : in[r + NIN / 2]; keep[r] = up ? in[r + NIN / 2] : in[r]; }
 }
 
 }  // namespace b200pir

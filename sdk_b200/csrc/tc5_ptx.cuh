@@ -1,5 +1,5 @@
-// Raw PTX wrappers for the Blackwell asynchronous machinery (mbarrier, bulk copy, tcgen05.mma / commit / ld, elect.sync),
-// shared by the tcgen05 kernels (tc5_kernels.cu: Spiral first dimension; dpir_gemm.cu: DoublePIR offline GEMMs).
+// Raw PTX wrappers for the Hopper asynchronous machinery (mbarrier, bulk copy, wgmma, elect.sync), shared by the wgmma
+// kernels (tc5_kernels.cu: Spiral first dimension; dpir_gemm.cu: DoublePIR offline GEMMs).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,24 +37,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
-// the previous form (1 ms suspend-time hint per try), kept selectable for A/B measurements (dbg_mode bit 2)
-__device__ __forceinline__ void mbar_wait_hinted(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  for (int tries = 0; tries < 20000; tries++) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, 0xF4240;\n\t"
-        "selp.u32 %0, 1, 0, P1;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) return;
-  }
-  asm volatile("trap;");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -78,36 +60,47 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// The wait names no registers, so without this the compiler may move reads of the accumulators above it: every accumulator
+// register goes through an (empty) asm that is ordered after the wait.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operands(uint32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate,
-                                          uint32_t idesc = tc5_instr_desc()) {
+
+#define TC5_R8(v, o) "+r"(v[o]), "+r"(v[o + 1]), "+r"(v[o + 2]), "+r"(v[o + 3]), "+r"(v[o + 4]), "+r"(v[o + 5]), "+r"(v[o + 6]), "+r"(v[o + 7])
+// D (64 x 128, s32 fragment of the warpgroup) += A (64 x 32 u8, K-major) * B (128 x 32 u8, K-major)^T, no saturation
+__device__ __forceinline__ void wgmma_m64n128k32_u8(uint32_t (&d)[64], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1;"
+      : TC5_R8(d, 0), TC5_R8(d, 8), TC5_R8(d, 16), TC5_R8(d, 24), TC5_R8(d, 32), TC5_R8(d, 40), TC5_R8(d, 48), TC5_R8(d, 56)
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
-// 32 lanes x 32 consecutive columns: thread t of the warp gets row (quadrant base + t)
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]),
-        "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]),
-        "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// D (64 x 32) += A (64 x 32, u8 or s8) * B (32 x 32 u8)^T, wrapping modulo 2^32
+template <bool A_SIGNED>
+__device__ __forceinline__ void wgmma_m64n32k32(uint32_t (&d)[16], uint64_t desc_a, uint64_t desc_b) {
+  if (A_SIGNED)
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.u8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1;"
+        : TC5_R8(d, 0), TC5_R8(d, 8)
+        : "l"(desc_a), "l"(desc_b)
+        : "memory");
+  else
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1;"
+        : TC5_R8(d, 0), TC5_R8(d, 8)
+        : "l"(desc_a), "l"(desc_b)
+        : "memory");
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef TC5_R8
 
 __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
   uint32_t lo = __shfl_xor_sync(0xffffffffu, (uint32_t)v, m), hi = __shfl_xor_sync(0xffffffffu, (uint32_t)(v >> 32), m);

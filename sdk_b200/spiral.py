@@ -114,8 +114,8 @@ class Database:
 
     def __init__(self, params, shard_index=0, shard_count=1, fmt=None):
         """fmt: 0 = IMAD layout (CUDA-core kernel, at most 4 queries per pass), 1 = mma.sync fragment order,
-        2 = tcgen05 tile images (16 queries per pass); None = the context's "db_format" option (default -1 = automatic:
-        2 wherever the tcgen05 kernel supports the geometry, else 1).  An explicit fmt applies to this database only."""
+        2 = wgmma tile images (16 queries per pass); None = the context's "db_format" option (default -1 = automatic:
+        2 wherever the wgmma kernel supports the geometry, else 1).  An explicit fmt applies to this database only."""
         self.params = params
         h = C.c_void_p()
         if fmt is not None:

@@ -1,8 +1,9 @@
-// CPU emulation of the tcgen05 first dimension's data path (sdk_b200/csrc/tc5_layout.cuh + the structure of
+// CPU emulation of the wgmma first dimension's data path (sdk_b200/csrc/tc5_layout.cuh + the structure of
 // tc5_kernels.cu): the operand images are built by running the per-thread functions for every thread, the MMA is replaced
 // by the DEFINITION of the canonical K-major no-swizzle shared-memory layout (byte (row, k) of an operand tile at
-// (row/8)*SBO + (k/16)*LBO + (row%8)*16 + k%16; D[M][N] += A[M][k] * B[N][k]; accumulator row M in TMEM lane M), and the
-// epilogue runs lane by lane with the two shuffle rounds of its reduce-scatter emulated.  Result compared with sum_j a*b mod q in 128-bit
+// (row/8)*SBO + (k/16)*LBO + (row%8)*16 + k%16; D[M][N] += A[M][k] * B[N][k]) and of the m64nNk32 s32 accumulator fragment
+// (thread (warp w, lane) of warpgroup wg holds D[64 wg + 16 w + lane/4 + 8 h][8 i + 2 (lane%4) + c] in register 4 i + 2 h + c),
+// and the epilogue runs lane by lane with the three shuffle rounds of its reduce-scatter emulated.  Result compared with sum_j a*b mod q in 128-bit
 // arithmetic.  This checks every index / limb / lane computation that is ours; what it cannot check is that the hardware
 // reads the descriptors the way the layout definition says.
 #include "../../sdk_b200/csrc/tc5_layout.cuh"
@@ -60,6 +61,7 @@ int main() {
             for (int r = 0; r < 2; r++) tc5_query_store(qt.data() + (size_t)ks * TC5_TILE, qc.q, r, qc.k, b[((size_t)qc.q * 2 + r) * dim0 + j]);
         }
       // ---- per row tile: MMA by the layout definition, then the epilogue
+      std::vector<int> covered((size_t)rows * 32, 0);
       for (int mt = 0; mt < T.mt; mt++) {
         std::vector<int32_t> D((size_t)TC5_M * TC5_N, 0);
         for (int ks = 0; ks < T.ks; ks++) {
@@ -76,40 +78,53 @@ int main() {
               D[(size_t)M * TC5_N + N] += s;
             }
         }
-        for (int quad = 0; quad < 4; quad++)
-          for (int chunk = 0; chunk < 4; chunk++) {
-            // step 1: per lane and GEMM column, the weighted partial sum; then the reduce-scatter of the kernel with both
-            // shuffle rounds emulated (every lane computes send/keep, then reads its partner's send)
-            uint64_t part[32][8], send4[32][4], keep4[32][4], send2[32][2], keep2[32][2];
+        for (int wg = 0; wg < 2; wg++)
+          for (int w = 0; w < 4; w++) {
+            // step 1: per lane, the 32 weighted partials of its accumulator fragment; then the three rounds of the
+            // reduce-scatter (every lane computes send/keep, then reads its partner's send)
+            uint64_t p32[32][32], s16[32][16], k16[32][16], s8[32][8], k8[32][8], s4[32][4], k4[32][4];
             Tc5Weights W[32];
             for (int lane = 0; lane < 32; lane++) {
-              const uint32_t* v = reinterpret_cast<const uint32_t*>(&D[(size_t)(quad * 32 + lane) * TC5_N + chunk * 32]);
-              W[lane] = tc5_lane_weights(tc5_lane_limb(lane), q);
-              for (int c = 0; c < 8; c++) {
-                part[lane][c] = tc5_lane_partial(v + 4 * c, W[lane].w, W[lane].wp);
-                if (part[lane][c] >> 53) { if (bad < 5) printf("partial sum bound exceeded\n"); bad++; }
-              }
-              tc5_rs_select_a(tc5_lane_limb(lane), part[lane], send4[lane], keep4[lane]);
+              uint32_t acc[64];
+              for (int i = 0; i < 16; i++)
+                for (int h = 0; h < 2; h++)
+                  for (int c = 0; c < 2; c++)
+                    acc[4 * i + 2 * h + c] = (uint32_t)D[(size_t)(64 * wg + 16 * w + lane / 4 + 8 * h) * TC5_N + 8 * i + 2 * (lane % 4) + c];
+              W[lane] = tc5_lane_weights(lane, q);
+              for (int i = 0; i < 16; i++)
+                for (int h = 0; h < 2; h++) {
+                  uint64_t& p = p32[lane][2 * i + h];
+                  p = tc5_lane_partial(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], W[lane].w, W[lane].wp);
+                  if (p >> 52) { if (bad < 5) printf("partial sum bound exceeded\n"); bad++; }
+                }
+              tc5_rs_split<32>((lane >> tc5_rs_lane_bit(0)) & 1, p32[lane], s16[lane], k16[lane]);
             }
             for (int lane = 0; lane < 32; lane++) {
-              uint64_t k[4];
-              for (int i = 0; i < 4; i++) k[i] = keep4[lane][i] + send4[lane ^ 2][i];
-              tc5_rs_select_b(tc5_lane_limb(lane), k, send2[lane], keep2[lane]);
+              for (int r = 0; r < 16; r++) k16[lane][r] += s16[lane ^ (1 << tc5_rs_lane_bit(0))][r];
+              tc5_rs_split<16>((lane >> tc5_rs_lane_bit(1)) & 1, k16[lane], s8[lane], k8[lane]);
             }
             for (int lane = 0; lane < 32; lane++) {
-              const int qi = tc5_lane_query(chunk, lane), ii = mt * 32 + tc5_lane_row(quad, lane);
-              if (qi >= nq || ii >= rows) continue;
-              for (int r = 0; r < 2; r++) {
-                const uint64_t tot = keep2[lane][r] + send2[lane ^ 1][r];
+              uint64_t k[8];
+              for (int r = 0; r < 8; r++) k[r] = k8[lane][r] + s8[lane ^ (1 << tc5_rs_lane_bit(1))][r];
+              tc5_rs_split<8>((lane >> tc5_rs_lane_bit(2)) & 1, k, s4[lane], k4[lane]);
+            }
+            for (int lane = 0; lane < 32; lane++)
+              for (int f = 0; f < 4; f++) {
+                const int qi = tc5_frag_query(lane, f), ii = mt * 32 + tc5_frag_row(wg, w, lane, f & 1), r = tc5_frag_ctrow(lane);
+                if (qi >= nq || ii >= rows) continue;
+                const uint64_t tot = k4[lane][f] + s4[lane ^ (1 << tc5_rs_lane_bit(2))][f];
                 if (tot >> 55) { if (bad < 5) printf("column sum bound exceeded\n"); bad++; }
                 const uint32_t got = tc5_barrett57(tot, W[lane].mu, q);
                 u128 ref = 0;
                 for (int j = 0; j < dim0; j++) ref += (u128)a[(size_t)ii * dim0 + j] * b[((size_t)qi * 2 + r) * dim0 + j];
                 if (got != (uint32_t)(ref % q)) { if (bad < 5) printf("mismatch trial %d n %d row %d query %d r %d\n", trial, n, ii, qi, r); bad++; }
+                covered[(size_t)ii * 32 + qi * 2 + r]++;
               }
-            }
           }
       }
+      for (int ii = 0; ii < rows; ii++)                            // every (row, query, ct row) output stored exactly once
+        for (int col = 0; col < 2 * nq; col++)
+          if (covered[(size_t)ii * 32 + col] != 1) { if (bad < 5) printf("output row %d column %d stored %d times\n", ii, col, covered[(size_t)ii * 32 + col]); bad++; }
     }
   }
   // tc5_barrett57 against % on random and extreme inputs below 2^57

@@ -12,8 +12,8 @@ times.  Checked over many random timings:
     are safe as well, but only because the survivors' all-gather of step k - 2 orders every rank's first dimension before
     anybody's expansion of step k; ONE set is not (the checker must find that hazard, which also shows it has teeth);
     one set is enough without the pipeline;
-  * the effect measured at N = 8 (profiles/timeline_r02_n8.md): with the "landed" all-reduces on the same communicator
-    as the survivors' all-gather, a step waits for the NEXT step's transfer; on their own communicator it does not.
+  * at N = 8: with the "landed" all-reduces on the same communicator as the survivors' all-gather, a step waits for the
+    NEXT step's transfer; on their own communicator it does not.
 No GPU, no torch: this is host logic."""
 import random
 
@@ -190,9 +190,9 @@ def test_one_set_is_enough_without_the_pipeline(n):
 
 
 def test_shared_communicator_queues_the_gather_behind_the_next_transfer():
-    """Durations as measured at N = 8 (profiles/timeline_r02_n8.md): expansion 2.6 ms, first dimension + local fold 5.75 ms,
-    pushes 6-10 ms, finish 0.3 ms.  Shared communicator: ~12.5 ms per step (measured 12.8); own communicator for the barriers:
-    ~9-10 ms (measured 10.1)."""
+    """Model durations of an 8-GPU step (expansion 2.6 ms, first dimension + local fold 5.75 ms, pushes 6-10 ms, finish
+    0.3 ms; stage proportions of the S8 workload, not an H100 measurement).  Shared communicator: ~12.5 ms per step; own
+    communicator for the barriers: ~9-10 ms."""
     dur = {"expand": (2.6, 2.65), "go": (0, 0), "push": (6.0, 10.0), "join": (0, 0), "barrier": (0.03, 0.05),
            "first_dim": (5.7, 5.8), "gather": (0.3, 0.5), "finish": (0.27, 0.3)}
 

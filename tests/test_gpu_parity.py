@@ -219,7 +219,7 @@ def test_expand_query_matches_oracle(name, pair_min):
     try:
         vreg, vf = S.expand_query(G, gpp, S.Query(ct=q["ct"]))
     finally:
-        G.set_option("expand_pair_min_ctas", 592)
+        G.set_option("expand_pair_min_ctas", 528)
     assert np.array_equal(vreg, vreg_ref)
     assert np.array_equal(vf, vf_ref)
 
@@ -239,7 +239,7 @@ def test_coefficient_expansion_matches_oracle_all_slots(name, pair_min, variant)
     try:
         S.coefficient_expansion(G, gpp, got)
     finally:
-        G.set_option("expand_pair_min_ctas", 592)
+        G.set_option("expand_pair_min_ctas", 528)
         G.set_option("expand_variant", 0)
     assert np.array_equal(got, ref)
 
@@ -252,7 +252,7 @@ def test_process_query_with_paired_expansion_everywhere():
     try:
         out = S.process_query_batch(G, gpp, qs, gdb)
     finally:
-        G.set_option("expand_pair_min_ctas", 592)
+        G.set_option("expand_pair_min_ctas", 528)
     for k, i in enumerate(idxs):
         assert np.array_equal(out[k], P.process_query(pp, dict(ct=qs[k * 2 * P.N:(k + 1) * 2 * P.N]), db)), k
         assert np.array_equal(cl.decode_response(out[k]), P.db_plain_item(SEED_DB, i))
@@ -561,7 +561,7 @@ def test_imma_multiply_many_tiles_long_k():
 
 @pytest.mark.parametrize("name,world", [("T0", 2), ("T1", 4), ("T", 2)])
 def test_three_phase_flow_with_tile_images_equals_oracle(name, world):
-    """bench.py's N>1 flow on tcgen05 databases: every "rank" expands its queries straight into a UMMA tile image (one image per
+    """bench.py's N>1 flow on format-2 databases: every "rank" expands its queries straight into an operand tile image (one image per
     rank), the images are concatenated (the copy-engine pushes), every rank multiplies from the images of ALL ranks on its row
     shard and folds, survivors are concatenated, each rank finishes its own queries.  Responses == oracle bytes."""
     import torch
@@ -654,7 +654,7 @@ def test_three_phase_multi_gpu_flow_equals_oracle(name, world, fmt):
 # ------------------------------------------------------------------ DoublePIR offline setup (doublepir.rs:76-108)
 @pytest.mark.parametrize("rows,kdim,cols", [(128, 32, 128), (45, 70, 33), (300, 257, 1024), (129, 1, 5)])
 def test_dpir_matmul_limb_gemm_matches_oracle(rows, kdim, cols):
-    """`&Matrix * &Matrix` (matrix/ops.rs:169-191) on the tcgen05 limb GEMM: small signed left operand (centred mod p, and the
+    """`&Matrix * &Matrix` (matrix/ops.rs:169-191) on the wgmma limb GEMM: small signed left operand (centred mod p, and the
     extremes -2^15 / 2^15 - 1), full 32-bit right operand including 0xffffffff; ragged shapes (zero padded tiles)."""
     import sdk_b200.doublepir as D
     rng = np.random.default_rng(rows * 7 + kdim)

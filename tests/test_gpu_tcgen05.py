@@ -1,7 +1,5 @@
-"""Parity of the tcgen05 first dimension (database format 2, sdk_b200/csrc/tc5_kernels.cu) against the oracle.
-
-First run on a B200 at the start of round 2 (gpurun_out/round2_bringup.log: raw accumulators match the assumed TMEM
-layout, 6/6 parity tests green); format 2 is now the default database format and these tests run with every `-m gpu`."""
+"""Parity of the wgmma first dimension (database format 2, sdk_b200/csrc/tc5_kernels.cu) against the oracle.  Format 2 is
+the default database format wherever the geometry fits."""
 import numpy as np
 import pytest
 

@@ -28,7 +28,7 @@ def test_dpir_matvec_wide_rows_match_oracle(rows, cols):
 
 
 def test_dpir_limb_gemm_with_wrapping_accumulators():
-    """The limb GEMM keeps four s32 accumulators in TMEM; with K beyond 2^15 and extreme operands they wrap.  Only the sum modulo
+    """The limb GEMM keeps four s32 register accumulators; with K beyond 2^15 and extreme operands they wrap.  Only the sum modulo
     2^32 is wanted, and a wrapped accumulator is still exact modulo 2^32 (DESIGN 4.5): K = 70016 with rows of all-255, all -2^15,
     all 2^15 - 1 against columns of 0xffffffff."""
     _gpu()

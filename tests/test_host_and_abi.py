@@ -72,8 +72,9 @@ def test_cooperative_ntt_emulation_matches_oracle(tmp_path):
 
 
 def test_tcgen05_operand_images_and_epilogue_emulation(tmp_path):
-    """tests/cpp/tc5_emul.cpp: the per-thread image builders and the epilogue lane arithmetic of the tcgen05 first
-    dimension, run on the CPU against the canonical UMMA K-major layout definition and 128-bit reference sums."""
+    """tests/cpp/tc5_emul.cpp: the per-thread image builders and the epilogue lane arithmetic of the wgmma first
+    dimension, run on the CPU against the canonical K-major layout definition, the accumulator fragment layout and 128-bit
+    reference sums."""
     exe = str(tmp_path / "tc5_emul")
     subprocess.check_call(["/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++", "-O2", "-std=c++17", "-o", exe,
                            os.path.join(ROOT, "tests", "cpp", "tc5_emul.cpp")])
@@ -82,19 +83,11 @@ def test_tcgen05_operand_images_and_epilogue_emulation(tmp_path):
 
 
 def test_tcgen05_descriptors_match_cutlass_bitfields(tmp_path):
-    """tests/cpp/tc5_desc_check.cu: our hand-packed instruction / shared-memory descriptors vs the vendored CUTLASS structs."""
-    import glob
-    import shutil
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    incs = [p for p in glob.glob("/opt/prime-rl/.venv/lib/python3*/site-packages/*/data/cutlass/include")
-            + glob.glob("/opt/prime-rl/.venv/lib/python3*/site-packages/*/3rdparty/cutlass/include")
-            if os.path.exists(os.path.join(p, "cute", "arch", "mma_sm100_desc.hpp"))]
-    if not (os.path.exists(nvcc) or shutil.which("nvcc")) or not incs:
-        pytest.skip("needs nvcc and a vendored CUTLASS header tree")
+    """tests/cpp/tc5_desc_check.cpp: our hand-packed shared-memory matrix descriptor vs a bit-field struct of the PTX ISA's
+    wgmma descriptor format."""
     exe = str(tmp_path / "tc5_desc_check")
-    subprocess.check_call([nvcc if os.path.exists(nvcc) else "nvcc", "-std=c++17", "-I" + incs[0], "-o", exe,
-                           os.path.join(ROOT, "tests", "cpp", "tc5_desc_check.cu"), "-ccbin",
-                           "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"])
+    subprocess.check_call(["/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++", "-O2", "-std=c++17", "-o", exe,
+                           os.path.join(ROOT, "tests", "cpp", "tc5_desc_check.cpp")])
     out = subprocess.check_output([exe], text=True)
     assert out.strip() == "descriptors ok", out
 

@@ -221,7 +221,7 @@ def test_chacha20_block_rfc8439_vector():
 
 def test_chacha20rng_stream_matches_rand_chacha_published_vectors():
     # rand_chacha's own known-answer test for ChaCha20Rng (chacha.rs, test_chacha_true_values_a; the crate is a third-party
-    # dependency absent from /root/reference, pinned at 0.3.1 in lib/spiral-rs/Cargo.lock): from_seed([0; 32]) yields the
+    # dependency absent from the reference tree, pinned at 0.3.1 in lib/spiral-rs/Cargo.lock): from_seed([0; 32]) yields the
     # keystream of the all-zero key, blocks 0 and 1 (= RFC 7539 appendix A.1 test vectors #1 and #2).  Pins what the block
     # vector above cannot: key placement, block counter in word 12 starting at 0 and incrementing per block, stream id 0,
     # output word order, and next_u64 = low word first (rand_core's BlockRng::next_u64).

@@ -1,16 +1,16 @@
-"""Discrete-event simulation of the barrier protocol of k_multiply_tc5 (sdk_b200/csrc/tc5_kernels.cu): the three roles
-(bulk-copy producer, MMA issuer, eight epilogue warps) are transcribed loop for loop as coroutines over a model of
-mbarrier phases / transaction counts, with randomised completion delays for the asynchronous agents (bulk copies,
-tcgen05.commit arrivals).  Checked: the run terminates (no deadlock), no shared-memory stage / B buffer / TMEM buffer is
-overwritten before its readers are done, nothing is read before it has been written, and no barrier ever runs two
-phases ahead of a waiter (which would make a parity wait miss its phase).  This is a model of the protocol, not of the
+"""Discrete-event simulation of the barrier protocol of k_multiply_tc5 (sdk_b200/csrc/tc5_kernels.cu): the roles
+(bulk-copy producer warp, two consumer warpgroups) are transcribed loop for loop as coroutines over a model of mbarrier
+phases / transaction counts, with randomised completion delays for the asynchronous agents (bulk copies, wgmma groups).
+Checked: the run terminates (no deadlock), no shared-memory stage / B buffer is overwritten before its readers are done,
+nothing is read before it has been written, and no barrier ever runs two phases ahead of a waiter (which would make a
+parity wait miss its phase).  This is a model of the protocol, not of the
 hardware: it guards the design against the one failure a GPU run cannot afford, a hang."""
 import heapq
 import random
 
 import pytest
 
-EPI_WARPS = 8
+CONSUMERS = 2                        # warpgroups; each arrives once on a ring stage / B buffer it has finished reading
 
 
 class Bar:
@@ -41,14 +41,13 @@ class Bar:
         return (self.phase & 1) != parity
 
 
-def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=2, ABUFS=2):
-    """STAGES ring stages of KS_PER_STAGE k-steps, BBUFS buffers of the query operand, ABUFS accumulator buffers: the template /
-    run-time parameters of k_multiply_tc5."""
+def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=2):
+    """STAGES ring stages of KS_PER_STAGE k-steps, BBUFS buffers of the query operand: the template / run-time parameters of
+    k_multiply_tc5."""
     rng = random.Random(seed)
     full = [Bar(1) for _ in range(STAGES)]
-    empty = [Bar(1) for _ in range(STAGES)]
-    bfull, bempty = [Bar(1) for _ in range(BBUFS)], [Bar(1) for _ in range(BBUFS)]
-    tfull, tempty = [Bar(1) for _ in range(ABUFS)], [Bar(EPI_WARPS) for _ in range(ABUFS)]
+    empty = [Bar(CONSUMERS) for _ in range(STAGES)]
+    bfull, bempty = [Bar(1) for _ in range(BBUFS)], [Bar(CONSUMERS) for _ in range(BBUFS)]
     stages_per_tile = (ks + KS_PER_STAGE - 1) // KS_PER_STAGE
     now = [0.0]
     events = []                      # (time, seq, fn)
@@ -60,10 +59,9 @@ def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=
 
     # ground truth for the hazard checks
     a_content = [None] * STAGES      # (item, tile, st) the stage currently holds, or ("loading", ...)
-    a_readers = [0] * STAGES         # MMAs issued on the stage and not yet complete
+    a_readers = [0] * STAGES         # MMA groups issued on the stage and not yet complete
     b_content, b_readers = [None] * BBUFS, [0] * BBUFS
-    t_content, t_writers, t_readers = [None] * ABUFS, [0] * ABUFS, [0] * ABUFS
-    log = {"tiles_done": 0, "max_lead": 0}
+    log = {"tiles_done": 0}
 
     def wait(bar, parity):
         while not bar.passed(parity):
@@ -98,70 +96,58 @@ def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=
                     yield
             it += 1
 
-    def commit(bars_and_hooks):      # tcgen05.commit: arrives when every MMA issued so far has completed
-        later(rng.uniform(0.1, 1.5), lambda: [h() for h in bars_and_hooks])
+    def consumer(wg):
+        stage, sphase, it = 0, 0, 0
+        groups = []                  # completion flags of this warpgroup's committed wgmma groups, oldest first
 
-    def mma():
-        stage, sphase, it, tile_no = 0, 0, 0, 0
+        def wait_groups(pending):    # wgmma.wait_group(pending): every group but the newest `pending` has completed
+            while not all(g[0] for g in groups[:len(groups) - pending]):
+                yield
+
         for item in range(n_items):
             bb = it % BBUFS
             yield from wait(bfull[bb], (it // BBUFS) & 1)
             assert b_content[bb] == item, "MMA reads a B buffer that does not hold this item"
             b_readers[bb] += 1
             for t in range(tiles_per_item):
-                ab = tile_no % ABUFS
-                yield from wait(tempty[ab], ((tile_no // ABUFS) & 1) ^ 1)
-                assert t_readers[ab] == 0, "accumulator overwritten while the epilogue still reads it"
-                t_content[ab] = ("accumulating", item, t)
-                t_writers[ab] += 1
+                prev = None
                 for st in range(stages_per_tile):
                     yield from wait(full[stage], sphase)
                     assert a_content[stage] == (item, t, st), "MMA reads an A stage that does not hold its tile"
                     a_readers[stage] += 1
-                    def freed(stage=stage):
+                    flag = [False]
+                    groups.append(flag)
+                    def complete(flag=flag, stage=stage):
+                        flag[0] = True
                         a_readers[stage] -= 1
-                        empty[stage].arrive()
-                    commit([freed])
+                    later(rng.uniform(0.1, 1.5), complete)
+                    yield from wait_groups(1)
+                    if prev is not None:
+                        empty[prev].arrive()
+                    prev = stage
                     stage += 1
                     if stage == STAGES:
                         stage, sphase = 0, sphase ^ 1
                     yield
-                def ready(ab=ab, item=item, t=t):
-                    t_writers[ab] -= 1
-                    t_content[ab] = (item, t)
-                    tfull[ab].arrive()
-                commit([ready])
-                tile_no += 1
-            def bfree(bb=bb):
-                b_readers[bb] -= 1
-                bempty[bb].arrive()
-            commit([bfree])
+                yield from wait_groups(0)
+                if prev is not None:
+                    empty[prev].arrive()
+                for _ in range(rng.randint(1, 4)):   # the epilogue works on registers only
+                    yield
+                if wg == 0:
+                    log["tiles_done"] += 1
+            b_readers[bb] -= 1
+            bempty[bb].arrive()
             it += 1
 
-    def epilogue(w):
-        tile_no = 0
-        for item in range(n_items):
-            for t in range(tiles_per_item):
-                ab = tile_no % ABUFS
-                yield from wait(tfull[ab], (tile_no // ABUFS) & 1)
-                assert t_content[ab] == (item, t) and t_writers[ab] == 0, "epilogue reads an accumulator that is not final"
-                t_readers[ab] += 1
-                for _ in range(rng.randint(1, 4)):
-                    yield
-                t_readers[ab] -= 1
-                tempty[ab].arrive()
-                if w == 0:
-                    log["tiles_done"] += 1
-                tile_no += 1
-
-    roles = [producer(), mma()] + [epilogue(w) for w in range(EPI_WARPS)]
+    roles = [producer()] + [consumer(wg) for wg in range(CONSUMERS)]
     alive = list(roles)
     idle_rounds = 0
     while alive:
         progressed = False
         order = list(alive)
         rng.shuffle(order)
-        before = (tuple(b.phase for b in full + empty + bfull + bempty + tfull + tempty), len(events))
+        before = (tuple(b.phase for b in full + empty + bfull + bempty), len(events))
         for r in order:
             try:
                 next(r)
@@ -173,10 +159,10 @@ def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=
             now[0] = tm
             fn()
             progressed = True
-        after = (tuple(b.phase for b in full + empty + bfull + bempty + tfull + tempty), len(events))
+        after = (tuple(b.phase for b in full + empty + bfull + bempty), len(events))
         idle_rounds = 0 if (progressed and before != after) or events else idle_rounds + 1
         assert idle_rounds < 10000, "deadlock: no role can make progress and no asynchronous event is pending"
-    while events:                    # drain trailing commits
+    while events:                    # drain trailing completions
         tm, _, fn = heapq.heappop(events)
         fn()
     return log["tiles_done"]
@@ -186,8 +172,8 @@ def simulate(n_items, tiles_per_item, ks, seed, STAGES=5, KS_PER_STAGE=4, BBUFS=
 def test_tc5_barrier_protocol_terminates_without_hazards(n_items, tiles, ks):
     for seed in range(6):
         assert simulate(n_items, tiles, ks, seed) == n_items * tiles
-        # the shipped configuration: 32 KiB stages, single-buffered query operand, four accumulator buffers (S8: 5 stages)
-        assert simulate(n_items, tiles, ks, seed, STAGES=5, KS_PER_STAGE=8, BBUFS=1, ABUFS=4) == n_items * tiles
-        assert simulate(n_items, tiles, ks, seed, STAGES=3, KS_PER_STAGE=8, BBUFS=2, ABUFS=4) == n_items * tiles
-        assert simulate(n_items, tiles, ks, seed, STAGES=10, KS_PER_STAGE=4, BBUFS=1, ABUFS=2) == n_items * tiles
-        assert simulate(n_items, tiles, ks, seed, STAGES=2, KS_PER_STAGE=4, BBUFS=1, ABUFS=4) == n_items * tiles
+        # the shipped configurations: 32 KiB stages beside a double- or single-buffered query operand, 16 KiB stages
+        assert simulate(n_items, tiles, ks, seed, STAGES=5, KS_PER_STAGE=8, BBUFS=1) == n_items * tiles
+        assert simulate(n_items, tiles, ks, seed, STAGES=3, KS_PER_STAGE=8, BBUFS=2) == n_items * tiles
+        assert simulate(n_items, tiles, ks, seed, STAGES=10, KS_PER_STAGE=4, BBUFS=1) == n_items * tiles
+        assert simulate(n_items, tiles, ks, seed, STAGES=2, KS_PER_STAGE=4, BBUFS=1) == n_items * tiles
