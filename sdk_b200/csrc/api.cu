@@ -93,10 +93,9 @@ struct b200pir_ctx {
   DevBuf<uint32_t> d_neg1;   // [11][2][2048] ntt32 (params.rs:98-107)
   // options
   int mul_variant = 0, max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
-  int fold_variant = 2;          // k_fold_res_lz at 3 CTAs per SM (default); 3: 2 CTAs per SM (A/B switch)
   int intt_variant = 0;
-  int expand_variant = 0;        // wide rounds: 0 paired + residue pipeline (3 CTAs/SM), 2 paired single kernel; 1: never paired
-  long pair_min_ctas = 528;      // 4 x 132 SMs
+  int expand_variant = 0;        // wide rounds: 0 paired + residue pipeline (2 CTAs/SM), 2 paired single kernel; 1: never paired
+  long pair_min_ctas = 1;        // every round paired: on H100 (S8, 16 queries) narrow rounds cost more at any width
   int sparse_fold = 0;           // 1: lib/server's fold (all-zero ciphertext shortcut, compute/fold.rs:37-43); 0: spiral-rs dense fold
   int imma_variant = 0;          // 0: cp.async-pipelined kernel for 5..8 queries per pass, 1: load-then-use kernel
   int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the wgmma kernel
@@ -419,7 +418,7 @@ const uint32_t* run_fold_res(b200pir_ctx* c, uint32_t* a, uint32_t* b, size_t ba
   }
   for (size_t half = num / 2; half >= 1; half /= 2, k--) {
     launch_fold_res(c->dp, src, dst, batch, batch_stride, (int)half, vfold + (size_t)k * mat, c->fold_words(),
-                    slices_per_query, (int)c->hp.t_gsw, c->bits_gsw, c->fold_variant, zero_flags, c->stream);
+                    slices_per_query, (int)c->hp.t_gsw, c->bits_gsw, zero_flags, c->stream);
     std::swap(src, dst);
   }
   return src;
@@ -703,7 +702,7 @@ int b200pir_ctx_set_option(b200pir_ctx* c, const char* key, int64_t value) {
   std::string k(key);
   if (k == "mul_variant") c->mul_variant = (int)value;
   else if (k == "batch") { if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) throw Error(B200PIR_E_BADARG, "batch must be 1, 2, 4, 8 or 16"); c->max_group = (int)value; }
-  else if (k == "fold_variant") c->fold_variant = (int)value;
+  else if (k == "fold_variant") {}   // one fold kernel now; the key stays accepted so existing callers keep working
   else if (k == "intt_variant") c->intt_variant = (int)value;
   else if (k == "imma_variant") c->imma_variant = (int)value;
   else if (k == "sparse_fold") c->sparse_fold = value != 0;
@@ -1290,7 +1289,7 @@ int b200pir_fold_ciphertexts(b200pir_ctx* c, uint64_t* v_cts, size_t num, const 
     int k = dims - 1;
     for (size_t half = num / 2; half >= 1; half /= 2, k--) {
       launch_fold_res(c->dp, a.p, b.p, 1, num * 4 * POLY, (int)half, vf.p + (size_t)k * mat, c->fold_words(), 1,
-                      (int)c->hp.t_gsw, c->bits_gsw, c->fold_variant, zflags.p, c->stream);
+                      (int)c->hp.t_gsw, c->bits_gsw, zflags.p, c->stream);
       B200_CUDA(cudaMemcpyAsync(a.p, b.p, half * 4 * POLY * 4, cudaMemcpyDeviceToDevice, c->stream));
     }
     launch_res_to_raw(c->dp, cts.p, a.p, num * 2, c->stream);

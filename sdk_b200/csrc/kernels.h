@@ -130,7 +130,7 @@ void launch_fold_round(const DevParams& P, uint64_t* cts, size_t batch, size_t b
 // in[i], in[half+i]; in != out.  Needs only v_folding (c_pos).
 void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size_t batch, size_t batch_stride /*u32*/,
                      int half, const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
-                     int variant, uint32_t* zero_flags /* null = dense semantics (spiral-rs); else scratch of batch*2*half words: lib/server fold.rs:37-43 */, cudaStream_t s);
+                     uint32_t* zero_flags /* null = dense semantics (spiral-rs); else scratch of batch*2*half words: lib/server fold.rs:37-43 */, cudaStream_t s);
 // server.rs:505-523 get_v_folding_neg, computed pointwise: neg = (q_n - C) + G  (NTT is linear and the
 // gadget matrix is constant-coefficient, so this is the same canonical value)
 void launch_folding_neg(const DevParams& P, uint32_t* out, const uint32_t* v_folding, int count, int t_gsw, int bits,

@@ -153,13 +153,25 @@ __device__ __forceinline__ uint32_t gadget_digit_fast(uint64_t v, int k, int bit
   return gadget_digit(v, k, bits, mask);
 }
 
+// The raw coefficients a digit loop decomposes: coef(a) = coefficient a*256 + tid (strided layout).  Kernels that already
+// hold them in shared memory read them there on every digit pair (SmemCoef) instead of keeping eight 64-bit values live
+// across the loop's transforms, which is what pushed the expansion kernels past their register budgets.
+struct RegCoef {
+  const uint64_t (&v)[8];
+  __device__ __forceinline__ uint64_t operator()(int a) const { return v[a]; }
+};
+struct SmemCoef {
+  const uint64_t* p;     // this thread's first coefficient
+  __device__ __forceinline__ uint64_t operator()(int a) const { return p[a * 256]; }
+};
+
 // acc[r][.] += sum_k  C[r][col0 + k*col_step] (.) NTT(digit_k(v))     (pointwise, this group's modulus)
-// v[a] = raw coefficient at index a*256 + tid (strided layout).  c0 points at element (row 0, first
+// v = coefficient source (RegCoef / SmemCoef).  c0 points at element (row 0, first
 // column) of this group's modulus, offset by tid*8.  `cnt` counts products held per accumulator.
 // Relaxed-range forward transforms (ntt_core.cuh "lz"): digits are < 2^19 < 2q (gadget dimensions >= 3), the outputs
 // (< 16q < 2^32) go straight into the 64-bit accumulators: products < 2^60, at most 16 per accumulator between reductions.
-template <int ROWS, bool SM, bool BYTE>
-__device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& cnt, const uint64_t (&v)[8], int ndig,
+template <int ROWS, bool SM, bool BYTE, typename Coef>
+__device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& cnt, Coef v, int ndig,
                                                 int bits, const uint32_t* c0, size_t col_step, size_t row_step,
                                                 const Grp& g) {
   const uint64_t mask = (1ull << bits) - 1;
@@ -172,19 +184,25 @@ __device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& c
       uint32_t x0[8], x1[8];
 #pragma unroll
       for (int a = 0; a < 8; a++) {
-        x0[a] = gadget_digit_fast<BYTE>(v[a], k, bits, mask);
-        x1[a] = gadget_digit_fast<BYTE>(v[a], k + 1, bits, mask);
+        const uint64_t va = v(a);
+        x0[a] = gadget_digit_fast<BYTE>(va, k, bits, mask);
+        x1[a] = gadget_digit_fast<BYTE>(va, k + 1, bits, mask);
       }
       ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x0, x1, g.smem, g.smem2, TwConst{g.n, 0}, TwShared{g.fwd_hi_sm}, g.q, CtaSync());
       if (cnt + 2 > 16) { acc_reduce<ROWS>(acc, g); cnt = 1; }
       cnt += 2;
       const uint32_t* c = c0 + (size_t)k * col_step;
+      // digit-major: x0 is dead before x1's key columns arrive
 #pragma unroll
       for (int r = 0; r < ROWS; r++) {
         uint32_t cv[8];
         ld8_ro(cv, c + (size_t)r * row_step);
 #pragma unroll
         for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x0[e] * cv[e];
+      }
+#pragma unroll
+      for (int r = 0; r < ROWS; r++) {
+        uint32_t cv[8];
         ld8_ro(cv, c + col_step + (size_t)r * row_step);
 #pragma unroll
         for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x1[e] * cv[e];
@@ -195,7 +213,7 @@ __device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& c
   for (; k < ndig; k++) {
     uint32_t x[8];
 #pragma unroll
-    for (int a = 0; a < 8; a++) x[a] = gadget_digit_fast<BYTE>(v[a], k, bits, mask);
+    for (int a = 0; a < 8; a++) x[a] = gadget_digit_fast<BYTE>(v(a), k, bits, mask);
     if (SM) ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x, g.smem, TwConst{g.n, 0}, TwShared{g.fwd_hi_sm}, g.q, CtaSync());
     else ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x, g.smem, TwConst{g.n, 0}, TwGlobal{g.fwd}, g.q, CtaSync());
     if (cnt + 1 > 16) { acc_reduce<ROWS>(acc, g); cnt = 1; }
@@ -212,8 +230,8 @@ __device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& c
 }
 
 // one warp-uniform branch per call (not per digit): the byte-permute and the funnel-shift digit extraction as two loop bodies
-template <int ROWS, bool SM>
-__device__ __forceinline__ void digits_mac(uint64_t (&acc)[ROWS][8], int& cnt, const uint64_t (&v)[8], int ndig,
+template <int ROWS, bool SM, typename Coef>
+__device__ __forceinline__ void digits_mac(uint64_t (&acc)[ROWS][8], int& cnt, Coef v, int ndig,
                                            int bits, const uint32_t* c0, size_t col_step, size_t row_step,
                                            const Grp& g) {
   if (bits == 8) digits_mac_impl<ROWS, SM, true>(acc, cnt, v, ndig, bits, c0, col_step, row_step, g);
@@ -381,7 +399,7 @@ k_fold_round(DevParams P, uint64_t* cts, size_t batch_stride, int half, const ui
       for (int a = 0; a < 8; a++) v[a] = ct[rho * POLY + a * 256 + g.tid];
       // G^-1 row index = rho + 2k  -> key-matrix column rho + 2k
       const uint32_t* c0 = C + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8;
-      digits_mac<2, false>(acc, cnt, v, t_gsw, bits, c0, col_step, row_step, g);
+      digits_mac<2, false>(acc, cnt, RegCoef{v}, t_gsw, bits, c0, col_step, row_step, g);
     }
   }
   uint64_t* dst = base + (size_t)i * 2 * POLY;
@@ -409,25 +427,31 @@ k_fold_round(DevParams P, uint64_t* cts, size_t batch_stride, int half, const ui
 // modulus n reads BOTH residues of its inputs (for the gadget digits) while the other CTA writes.
 // Digit k of vh minus digit k of vi, offset by q: in (q - 2^bits, q + 2^bits), a subset of [0, 2q) for bits <= 27 (the
 // context rejects gadget dimensions below 3, so bits <= 19) — the relaxed-range forward transform needs no more.
-// BYTE: bits == 8, where digit k is simply byte k; the values are < 2^56, so byte 7 serves as the zero filler.
-template <bool BYTE>
 __device__ __forceinline__ uint32_t digit_diff(uint64_t vh, uint64_t vi, int k, int bits, uint64_t mask, uint32_t q) {
-  if (BYTE) {
-    const uint32_t sel = 0x7770u | (uint32_t)k;
-    return __byte_perm((uint32_t)vh, (uint32_t)(vh >> 32), sel) - __byte_perm((uint32_t)vi, (uint32_t)(vi >> 32), sel) + q;
-  }
   return gadget_digit(vh, k, bits, mask) - gadget_digit(vi, k, bits, mask) + q;
 }
+// bits == 8, where digit k is simply byte k; the values are < 2^56, so byte 7 serves as the zero filler.  Digits k and k + 1
+// of vh minus those of vi, each offset by 256 into [1, 511], in the low and the high half of one word (no borrow crosses
+// the halves).  Half + q - 256 is digit_diff's value.
+__device__ __forceinline__ uint32_t byte_pair_diff(uint64_t vh, uint64_t vi, int k) {
+  const uint32_t sel = 0x7070u | ((uint32_t)(k + 1) << 8) | (uint32_t)k;
+  return __byte_perm((uint32_t)vh, (uint32_t)(vh >> 32), sel) + 0x01000100u -
+         __byte_perm((uint32_t)vi, (uint32_t)(vi >> 32), sel);
+}
+constexpr int kFoldPlanes = 4;   // byte-pair planes of the bits == 8 path: gadget dimensions up to 8
 
 // Same step as k_fold_res on the relaxed-range transforms (ntt_core.cuh "lz"): no per-butterfly range correction in the
 // forward transforms (outputs < 16q feed the 64-bit multiply-accumulate directly: 16 products of < 2^32 x < 2^28 fit),
-// no halving in the inverse transform, byte-permute digit extraction when bits_per = 8, 32-bit Barrett in the CRT lift.
-// Tried on top of this and measured without gain (S8, 16 queries; fold stage 3.53 ms): pass C / D twiddles held in registers at
-// 2 CTAs per SM (3.60 ms: 35 % less shared-memory traffic, so that is not the limit), key columns prefetched into L1 before the
-// pair's transforms (3.60 ms: the L2 latency ncu attributes to the multiply-accumulate is covered by the other CTAs).  The
-// kernel runs at ~80 % of its integer-multiply-pipe bound (DESIGN.md 4.3).
-template <int MINB, bool BYTE>
-__global__ void __launch_bounds__(256, MINB)
+// no halving in the inverse transform, 32-bit Barrett in the CRT lift.
+// BYTE (bits == 8, gadget dimension <= 8): the digit differences of both inputs are formed once per row and parked in
+// shared memory as byte-pair planes (32 KiB), one word per digit pair and coefficient, written and read by the same thread.
+// Only the accumulators then stay live across the digit loop.  Held in registers, the CRT-composed inputs (32 registers)
+// pushed the loop body into local memory, which shares the L1/shared-memory data path with the transforms' exchanges.
+// Other gadget widths keep them in registers.
+// 2 CTAs per SM (up to 128 registers): the byte path compiles without spills there.  At 3 CTAs per SM (80 registers) it
+// still spills in the multiply-accumulate and measured slower on H100 (S8, 16 queries: fold 5.22 against 5.12 ms per step).
+template <bool BYTE>
+__global__ void __launch_bounds__(256, 2)
 k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict__ out, size_t batch_stride, int half,
               const uint32_t* __restrict__ c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
               const uint32_t* __restrict__ zero_flags /* null, or [batch][2*half]: 1 = ciphertext is all zero */) {
@@ -462,6 +486,7 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
   const size_t row_step = (size_t)cols * 2 * POLY;
   const uint64_t mask = (1ull << bits) - 1;
   const uint32_t q = g.q;
+  uint32_t* planes = reinterpret_cast<uint32_t*>(tw + HI_TW) + g.tid;   // BYTE: [kFoldPlanes][POLY], this thread's column
 
   uint64_t acc[2][8];
 #pragma unroll
@@ -477,6 +502,11 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
       const int z = a * 256 + g.tid;
       vi[a] = crt_compose(__ldg(ci + (rho * 2 + 0) * POLY + z), __ldg(ci + (rho * 2 + 1) * POLY + z), P);
       vh[a] = crt_compose(__ldg(ch + (rho * 2 + 0) * POLY + z), __ldg(ch + (rho * 2 + 1) * POLY + z), P);
+      if (BYTE) {
+#pragma unroll
+        for (int p = 0; p < kFoldPlanes; p++)
+          if (2 * p < t_gsw) planes[p * POLY + a * 256] = byte_pair_diff(vh[a], vi[a], 2 * p);
+      }
     }
     const uint32_t* c0 = C + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8;       // key-matrix column of digit k: rho + 2k
     int k = 0;
@@ -485,18 +515,29 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
       uint32_t x0[8], x1[8];
 #pragma unroll
       for (int a = 0; a < 8; a++) {
-        x0[a] = digit_diff<BYTE>(vh[a], vi[a], k, bits, mask, q);
-        x1[a] = digit_diff<BYTE>(vh[a], vi[a], k + 1, bits, mask, q);
+        if (BYTE) {
+          const uint32_t w = planes[(k >> 1) * POLY + a * 256];
+          x0[a] = (w & 0xffffu) + (q - 256u);
+          x1[a] = (w >> 16) + (q - 256u);
+        } else {
+          x0[a] = digit_diff(vh[a], vi[a], k, bits, mask, q);
+          x1[a] = digit_diff(vh[a], vi[a], k + 1, bits, mask, q);
+        }
       }
       ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x0, x1, sm0, sm1, lo, hi, q, CtaSync());
       if (cnt + 2 > 16) { acc_reduce<2>(acc, g); cnt = 1; }
       cnt += 2;
+      // digit-major: x0 is dead before x1's key columns arrive
 #pragma unroll
       for (int r = 0; r < 2; r++) {
         uint32_t cv[8];
         ld8_ro(cv, c0 + (size_t)r * row_step + (size_t)k * 4 * POLY);
 #pragma unroll
         for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x0[e] * cv[e];
+      }
+#pragma unroll
+      for (int r = 0; r < 2; r++) {
+        uint32_t cv[8];
         ld8_ro(cv, c0 + (size_t)r * row_step + (size_t)(k + 1) * 4 * POLY);
 #pragma unroll
         for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x1[e] * cv[e];
@@ -505,7 +546,8 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
     if (k < t_gsw) {                            // odd t_gsw: last digit alone
       uint32_t x0[8];
 #pragma unroll
-      for (int a = 0; a < 8; a++) x0[a] = digit_diff<BYTE>(vh[a], vi[a], k, bits, mask, q);
+      for (int a = 0; a < 8; a++)
+        x0[a] = BYTE ? (planes[(k >> 1) * POLY + a * 256] & 0xffffu) + (q - 256u) : digit_diff(vh[a], vi[a], k, bits, mask, q);
       ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x0, sm0, lo, hi, q, CtaSync());
       if (cnt + 1 > 16) { acc_reduce<2>(acc, g); cnt = 1; }
       cnt += 1;
@@ -606,13 +648,10 @@ __global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* 
 
   stage_fwd_twiddles(g, tw + g.n * HI_TW);
   uint32_t* vi = v + (size_t)i * 4 * POLY;
-  uint32_t keep[2][8];
   // row 0: from_ntt + automorph (poly.rs:393-405), scattered into shared memory for the gadget digits
   {
     uint32_t x[8];
     ld8(x, vi + (size_t)g.n * POLY + g.tid * 8);
-#pragma unroll
-    for (int e = 0; e < 8; e++) keep[0][e] = x[e];
     grp_ntt_inv(g, x);
     const int t_auto = R.t_auto;
     const uint64_t Q = P.modulus;
@@ -622,14 +661,24 @@ __global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* 
       autom[rem] = (num & 1u) ? Q - val : val;           // zero maps to q, as in the reference
     });
   }
+  __syncthreads();
+  uint64_t acc[2][8];
+#pragma unroll
+  for (int r = 0; r < 2; r++)
+#pragma unroll
+    for (int e = 0; e < 8; e++) acc[r][e] = 0;
+  int cnt = 0;
+  // gadget_invert_rdim(.., rdim = 1): digit k -> key column k  (server.rs:82-89)
+  digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
+                      (size_t)t_exp * 2 * POLY, g);
   // row 1: the reference computes to_ntt(automorph(from_ntt(row 1))) (server.rs:80-88).  X -> X^t permutes the
   // roots of X^N + 1, so in the NTT domain the automorphism is a pure permutation of the evaluation slots:
   // slot s holds the value at psi^(2 br(s) + 1), and tau_t(a) there equals a at psi^((2 br(s) + 1) t).  The
   // values are canonical residues either way, so the gathered vector is bit-identical to the reference's.
+  // Gathered before any thread overwrites v[i].
   uint32_t y[8];
   {
     const uint32_t* row1 = vi + ((size_t)2 + g.n) * POLY;
-    ld8(keep[1], row1 + g.tid * 8);
 #pragma unroll
     for (int k = 0; k < 8; k++) {
       const unsigned sidx = (unsigned)(g.tid * 8 + k);
@@ -640,26 +689,13 @@ __global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* 
     }
   }
   __syncthreads();
-  uint64_t acc[2][8];
-#pragma unroll
-  for (int r = 0; r < 2; r++)
-#pragma unroll
-    for (int e = 0; e < 8; e++) acc[r][e] = 0;
-  int cnt = 0;
-  {
-    uint64_t vv[8];
-#pragma unroll
-    for (int a = 0; a < 8; a++) vv[a] = autom[a * 256 + g.tid];
-    // gadget_invert_rdim(.., rdim = 1): digit k -> key column k  (server.rs:82-89)
-    const uint32_t* c0 = W + (size_t)g.n * POLY + g.tid * 8;
-    digits_mac<2, true>(acc, cnt, vv, t_exp, bits, c0, (size_t)2 * POLY, (size_t)t_exp * 2 * POLY, g);
-  }
 #pragma unroll
   for (int rho = 0; rho < 2; rho++) {
     uint32_t o[8];
+    ld8(o, vi + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8);
 #pragma unroll
     for (int e = 0; e < 8; e++) {
-      uint32_t s = addmod(keep[rho][e], barrett64(acc[rho][e], g.cr1, g.q), g.q);
+      uint32_t s = addmod(o[e], barrett64(acc[rho][e], g.cr1, g.q), g.q);
       o[e] = rho ? addmod(s, y[e], g.q) : s;
     }
     st8(vi + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8, o);
@@ -765,13 +801,8 @@ k_expand_round_pair(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R, co
 #pragma unroll
       for (int e = 0; e < 8; e++) acc[r][e] = 0;
     int cnt = 0;
-    {
-      uint64_t vv[8];
-#pragma unroll
-      for (int a = 0; a < 8; a++) vv[a] = autom[a * 256 + g.tid];
-      const uint32_t* c0 = W + (size_t)g.n * POLY + g.tid * 8;
-      digits_mac<2, true>(acc, cnt, vv, t_exp, bits, c0, (size_t)2 * POLY, (size_t)t_exp * 2 * POLY, g);
-    }
+    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
+                        (size_t)t_exp * 2 * POLY, g);
     uint32_t* dst = half ? vo : vi;
 #pragma unroll
     for (int rho = 0; rho < 2; rho++) {
@@ -802,7 +833,7 @@ k_expand_round_pair(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R, co
 }
 
 // ---- paired rounds, residue pipeline: the same arithmetic as k_expand_round_pair split the way k_fold_res is, so that
-// the transforms run in 256-thread single-modulus CTAs at 3 CTAs per SM instead of one 512-thread CTA per SM.
+// the transforms run in 256-thread single-modulus CTAs at 2 CTAs per SM instead of one 512-thread CTA per SM.
 //   k_expand_intt:       inverse transform of row 0 of every processed v[i], residues in coefficient order -> xr
 //   k_expand_round_res:  CTA (i, n): CRT lift (+ negacyclic shift for the second output) + automorphism + gadget digits
 //                        + forward transforms and key products modulo q_n; writes rows (., n) of v[i] and v[i + num_in].
@@ -825,8 +856,9 @@ k_expand_intt(DevParams P, const uint32_t* __restrict__ v, size_t v_stride, uint
   for (int a = 0; a < 8; a++) dst[a * 256 + g.tid] = x[a];
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(256, MINB)
+// 2 CTAs per SM (up to 128 registers): compiles without spills; at 3 CTAs per SM (80 registers) it spilled and measured
+// slower on H100 (S8, 16 queries, every round paired: expansion 3.58 against 3.61 ms per step).
+__global__ void __launch_bounds__(256, 2)
 k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __restrict__ xr, size_t xr_stride,
                    ExpandRound R, const uint32_t* __restrict__ neg1) {
   v += (size_t)blockIdx.z * v_stride;
@@ -892,13 +924,8 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
 #pragma unroll
       for (int e = 0; e < 8; e++) acc[r][e] = 0;
     int cnt = 0;
-    {
-      uint64_t vv[8];
-#pragma unroll
-      for (int a = 0; a < 8; a++) vv[a] = autom[a * 256 + g.tid];
-      const uint32_t* c0 = W + (size_t)g.n * POLY + g.tid * 8;
-      digits_mac<2, true>(acc, cnt, vv, t_exp, bits, c0, (size_t)2 * POLY, (size_t)t_exp * 2 * POLY, g);
-    }
+    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
+                        (size_t)t_exp * 2 * POLY, g);
     // row 1 automorphism = slot permutation (see k_expand_round); gather before any thread overwrites v[i]
     uint32_t yy[8];
 #pragma unroll
@@ -982,11 +1009,8 @@ k_regev_to_gsw(DevParams P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* 
   const int ccols = 2 * t_conv;
 #pragma unroll 1
   for (int rho = 0; rho < 2; rho++) {
-    uint64_t vv[8];
-#pragma unroll
-    for (int a = 0; a < 8; a++) vv[a] = raw[rho * POLY + a * 256 + g.tid];
     const uint32_t* c0 = v_conv + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8;
-    digits_mac<2, true>(acc, cnt, vv, t_conv, bits_conv, c0, (size_t)2 * 2 * POLY, (size_t)ccols * 2 * POLY, g);
+    digits_mac<2, true>(acc, cnt, SmemCoef{raw + rho * POLY + g.tid}, t_conv, bits_conv, c0, (size_t)2 * 2 * POLY, (size_t)ccols * 2 * POLY, g);
   }
 #pragma unroll
   for (int r = 0; r < 2; r++) {
@@ -1039,7 +1063,7 @@ k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* fold
       uint64_t vv[8];
 #pragma unroll
       for (int a = 0; a < 8; a++) vv[a] = crt_compose(__ldg(ct + a * 256 + g.tid), __ldg(ct + POLY + a * 256 + g.tid), P);
-      digits_mac<ROWS, true>(acc, cnt, vv, t_conv, bits, W + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
+      digits_mac<ROWS, true>(acc, cnt, RegCoef{vv}, t_conv, bits, W + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
     }
     uint32_t y[8];
 #pragma unroll
@@ -1072,15 +1096,12 @@ k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* fold
         grp_ntt_inv(g, x);
         crt_lift(x, res, g, P, [&](int z, uint64_t val) { rawbuf[z] = val; });
         __syncthreads();
-        uint64_t vv[8];
-#pragma unroll
-        for (int a = 0; a < 8; a++) vv[a] = rawbuf[a * 256 + g.tid];
 #pragma unroll
         for (int m = 0; m < ROWS; m++)
 #pragma unroll
           for (int e = 0; e < 8; e++) acc[m][e] = 0;
         cnt = 0;
-        digits_mac<ROWS, true>(acc, cnt, vv, t_conv, bits, Wshift + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
+        digits_mac<ROWS, true>(acc, cnt, SmemCoef{rawbuf + g.tid}, t_conv, bits, Wshift + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
         uint32_t np[ROWS][8];
 #pragma unroll
         for (int m = 0; m < ROWS; m++)
@@ -1203,24 +1224,19 @@ void launch_res_to_raw(const DevParams& P, uint64_t* out, const uint32_t* res, s
 }
 void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size_t batch, size_t batch_stride, int half,
                      const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
-                     int variant, uint32_t* zero_flags, cudaStream_t s) {
+                     uint32_t* zero_flags, cudaStream_t s) {
   if (batch == 0 || half == 0) return;
   if (zero_flags) {            // scratch of batch * 2 * half words: recomputed every round, as the reference re-tests every step
     ++g_kernel_launches;
     k_ct_zero_flags<<<(unsigned)(batch * 2 * half), 256, 0, s>>>(in, batch_stride, 2 * half, zero_flags);
   }
   ++g_kernel_launches;
-  // variant 3: 2 CTAs per SM (128 registers); anything else: 3 CTAs per SM (80 registers) — same speed on S8, kept for A/B runs
   const dim3 grid((unsigned)(batch * half), 2);
-#define FOLD_LZ(MINB, BYTE)                                                                                             \
-  do {                                                                                                                  \
-    opt_in_smem(k_fold_res_lz<MINB, BYTE>, (int)kDynSmemFold);                                                          \
-    k_fold_res_lz<MINB, BYTE><<<grid, 256, kDynSmemFold, s>>>(P, in, out, batch_stride, half, c_pos, c_batch_stride,    \
-                                                             slices_per_query, t_gsw, bits, zero_flags);               \
-  } while (0)
-  if (variant == 3) { if (bits == 8) FOLD_LZ(2, true); else FOLD_LZ(2, false); }
-  else { if (bits == 8) FOLD_LZ(3, true); else FOLD_LZ(3, false); }
-#undef FOLD_LZ
+  const bool byte = bits == 8 && t_gsw <= 2 * kFoldPlanes;
+  const size_t smem = kDynSmemFold + (byte ? (size_t)kFoldPlanes * POLY * 4 : 0);
+  auto kern = byte ? k_fold_res_lz<true> : k_fold_res_lz<false>;
+  opt_in_smem(kern, (int)smem);
+  kern<<<grid, 256, smem, s>>>(P, in, out, batch_stride, half, c_pos, c_batch_stride, slices_per_query, t_gsw, bits, zero_flags);
 }
 void launch_from_ntt(const DevParams& P, uint64_t* out_raw, const uint32_t* in, size_t count, cudaStream_t s) {
   if (count) ++g_kernel_launches, k_from_ntt<<<(unsigned)count, CTA, 0, s>>>(P, out_raw, in);
@@ -1264,10 +1280,10 @@ void launch_expand_round_pair(const DevParams& P, uint32_t* v, size_t v_stride, 
 void launch_expand_round_res(const DevParams& P, uint32_t* v, size_t v_stride, uint32_t* xr, size_t xr_stride, int nq,
                              const ExpandRound& R, const uint32_t* neg1_r, cudaStream_t s) {
   const size_t smem = (size_t)2 * NTT_SMEM_WORDS * 4 + (size_t)POLY * 8 + (size_t)HI_TW * 8;
-  opt_in_smem(k_expand_round_res<3>, (int)smem);
+  opt_in_smem(k_expand_round_res, (int)smem);
   g_kernel_launches += 2;
   k_expand_intt<<<dim3((unsigned)R.num_in, 2, nq), 256, 0, s>>>(P, v, v_stride, xr, xr_stride, R);
-  k_expand_round_res<3><<<dim3((unsigned)R.num_in, 2, nq), 256, smem, s>>>(P, v, v_stride, xr, xr_stride, R, neg1_r);
+  k_expand_round_res<<<dim3((unsigned)R.num_in, 2, nq), 256, smem, s>>>(P, v, v_stride, xr, xr_stride, R, neg1_r);
 }
 void launch_reorient(const MulGeom& G, uint4* q_dev, size_t q_stride, const uint32_t* v, size_t v_stride, int nq,
                      int idx_factor, cudaStream_t s) {
