@@ -95,6 +95,14 @@ int b200pir_db_upsert_item(b200pir_ctx* ctx, b200pir_db* db, uint64_t slice, uin
  * of item db_idx (at most instances*n^2*bytes_per_chunk, zero padded); chunk c becomes the item polynomial of slice c
  * (convert_pt_to_poly :278-299: coefficient i = byte i, recenter_mod, NTT; pack_ntt_poly :34-41), all on the GPU. */
 int b200pir_db_update_item_raw(b200pir_ctx* ctx, b200pir_db* db, uint64_t db_idx, const uint8_t* data, size_t len);
+/* lib/server/src/db/loading.rs:361-377 update_many_items (the /update-row body): entries [u32 BE chunk_len][chunk_len bytes],
+ * each chunk = [u32 BE db_idx][raw bucket bytes] as update_item (:301-315).  *largest_update = max chunk_len (written on
+ * success; may be NULL).  The final database equals the reference's entry-by-entry loop: the entries before the first bad one
+ * are applied, nothing from it on, and its code is returned (B200PIR_E_SHAPE for a header or chunk past the end of the body,
+ * chunk_len < 4, chunk_len > 4 + instances*n^2*bytes_per_chunk or db_idx >= num_items; B200PIR_E_UNSUPPORTED for p != 256).
+ * A db_idx written more than once ends with its last bytes.  On a shard every entry is checked and only its own rows are
+ * written.  Conversion and placement run on the GPU; synchronises the context's stream before it returns. */
+int b200pir_db_update_many_items(b200pir_ctx* ctx, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update);
 /* Synthetic database generated on the GPU: plaintext coefficient = splitmix64(seed, ((slice*items+item)*2048+z)) % p,
  * then recenter_mod / NTT / pack as generate_random_db_and_get_item does (server.rs:223-275). */
 int b200pir_db_fill_synthetic(b200pir_ctx* ctx, b200pir_db* db, uint64_t seed);

@@ -88,6 +88,13 @@ struct Database {
   void upsert_item(uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
     check(b200pir_db_upsert_item(params.ctx, h, slice, item_idx, poly));
   }
+  // lib/server/src/db/loading.rs:361-377 update_many_items (the /update-row body); returns largest_update.  On a bad entry the
+  // entries before it stay applied and this throws.
+  uint64_t update_many_items(const uint8_t* body, size_t len) {
+    uint64_t largest_update = 0;
+    check(b200pir_db_update_many_items(params.ctx, h, body, len, &largest_update));
+    return largest_update;
+  }
 };
 
 namespace ntt {

@@ -5,6 +5,7 @@
 #include "../../include/b200pir.h"
 #include "kernels.h"
 #include "ntt_tables.hpp"
+#include "update_body.hpp"
 #include <cstdio>
 #include <algorithm>
 #include <cmath>
@@ -117,6 +118,12 @@ struct b200pir_ctx {
   size_t folded_stride = 0;           // u32 words between consecutive (query, slice) survivors
   DevBuf<uint64_t> w_packed;     // [Q][inst][n+1][n][2048]
   DevBuf<uint8_t> w_resp;        // [Q][response_bytes]
+  // database writers (update_item_raw, update_many_items, load_raw_file): raw item bytes and their item descriptors, one group
+  // of whole items at a time; sized on the first write, so later writes neither allocate nor free device memory
+  static constexpr size_t kWriteStageBytes = (size_t)64 << 20;
+  static constexpr size_t kWriteStageItems = 65536;
+  DevBuf<uint8_t> w_wbytes;
+  DevBuf<ItemWrite> w_witems;
   // Coalescing of concurrent callers ("coalesce", default on): lib/server takes a READ lock around process_query
   // (bin/server.rs:102), so actix workers call it concurrently.  Requests arriving while a batch runs queue up here; the
   // thread that finds no batch in flight becomes the leader and serves everything queued (up to kCoalesceMax) in ONE
@@ -240,16 +247,30 @@ struct b200pir_db {
     tile_mask.alloc(h_tile_mask.size());
     B200_CUDA(cudaMemset(tile_mask.p, 0, h_tile_mask.size() * 4));
   }
-  // one item written (stream-ordered update of the device mask word)
-  void mark(int slice, int il, int j, cudaStream_t s) {
+  // one item written, host side only: returns true when its tile-mask word changed (the device copy is then stale)
+  bool mark_host(int slice, int il, int j) {
     const uint64_t bit = ((uint64_t)slice * rows + il) * ctx->dim0 + j;
     if (!((present[bit >> 6] >> (bit & 63)) & 1)) { present[bit >> 6] |= 1ull << (bit & 63); present_count++; }
     const size_t w = (size_t)slice * T.mt + (il >> 5);
     const uint32_t nv = h_tile_mask[w] | (1u << (j >> 5));
-    if (nv != h_tile_mask[w]) {
-      h_tile_mask[w] = nv;
+    if (nv == h_tile_mask[w]) return false;
+    h_tile_mask[w] = nv;
+    return true;
+  }
+  // one item written (stream-ordered update of the device mask word)
+  void mark(int slice, int il, int j, cudaStream_t s) {
+    if (mark_host(slice, il, j)) {
+      const size_t w = (size_t)slice * T.mt + (il >> 5);
       B200_CUDA(cudaMemcpyAsync(tile_mask.p + w, &h_tile_mask[w], 4, cudaMemcpyHostToDevice, s));
     }
+  }
+  // every item of every slice of `items` written: one upload of the whole mask when any word changed
+  void mark_items(const ItemWrite* items, size_t count, cudaStream_t s) {
+    bool changed = false;
+    for (size_t k = 0; k < count; k++)
+      for (int sl = 0; sl < ctx->slices; sl++) changed |= mark_host(sl, (int)items[k].il, (int)items[k].j);
+    if (changed)
+      B200_CUDA(cudaMemcpyAsync(tile_mask.p, h_tile_mask.data(), h_tile_mask.size() * 4, cudaMemcpyHostToDevice, s));
   }
   // a whole slice written at once (bulk upload, file load, synthetic fill): every item of it exists from now on
   void mark_slice(int slice, cudaStream_t s) {
@@ -800,6 +821,21 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
   B200_CUDA(cudaStreamSynchronize(c->stream));
   B200_CUDA(cudaGetLastError());
 }
+
+// Stage `span` raw bytes from host memory `host` and write the `count` items that lie in them (ItemWrite offsets are relative
+// to `host`): one conversion-and-placement launch over (item, slice).  Presence is the caller's.  Stream-ordered: the staging
+// buffers are only overwritten by the next group's copies, which run after this launch.
+void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
+  if (count == 0) return;
+  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
+  c->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, count));
+  if (span) B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, host, span, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
+  const size_t chunks = (size_t)c->slices;
+  const size_t bpc = (c->hp.db_item_size + chunks - 1) / chunks;             // params.bytes_per_chunk()
+  const DbDst dst{db->format, c->geom(db->rows), db->F, db->T, db->d.p, db->f.p, db->t.p};
+  launch_write_items(c->dp, dst, c->w_wbytes.p, c->w_witems.p, (int)count, (int)chunks, (int)bpc, c->hp.p, c->stream);
+}
 }  // namespace
 }  // extern "C++"
 
@@ -881,26 +917,61 @@ int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, 
   if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
   const int ii = (int)(db_idx % c->num_per), j = (int)(db_idx / c->num_per);
   if (ii % db->shard.count != db->shard.index) return 0;                      // row lives on another GPU
-  DevBuf<uint8_t> bucket(chunks * pt_len);
-  DevBuf<uint64_t> polys(chunks * POLY);
-  B200_CUDA(cudaMemsetAsync(bucket.p, 0, bucket.n, c->stream));
-  if (len) B200_CUDA(cudaMemcpyAsync(bucket.p, data, len, cudaMemcpyHostToDevice, c->stream));
-  launch_item_from_bytes(c->dp, bucket.p, (int)chunks, (int)pt_len, hp.p, polys.p, c->stream);
-  for (size_t s = 0; s < chunks; s++) {
-    if (db->format == 0) launch_db_upsert(c->geom(db->rows), db->d.p, (int)s, ii / db->shard.count, j, polys.p + s * POLY, c->stream);
-    else if (db->format == 2) launch_db_upsert_tc5(db->T, db->t.p, (int)s, ii / db->shard.count, j, polys.p + s * POLY, c->stream);
-    else launch_db_upsert_frag(db->F, db->f.p, (int)s, ii / db->shard.count, j, polys.p + s * POLY, c->stream);
-    db->mark((int)s, ii / db->shard.count, j, c->stream);
-  }
+  const ItemWrite item{0, (uint32_t)len, (uint32_t)(ii / db->shard.count), (uint32_t)j};
+  write_items(c, db, data, len, &item, 1);
+  db->mark_items(&item, 1, c->stream);
   B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
   B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+// lib/server/src/db/loading.rs:361-377 update_many_items (the /update-row body).  The whole body is parsed on the host first
+// (update_body.hpp); the valid prefix is applied and the error of the first bad entry, if any, returned afterwards, which is
+// the database state the reference's entry-by-entry loop leaves.  Only the last occurrence of each db_idx is written, so how
+// the entries are split into staging groups cannot change the result.  Every shard checks every entry and writes its own rows.
+int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update) {
+  API_BEGIN
+  if (!c || (!body && len)) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  const auto& hp = c->hp;
+  const size_t chunks = (size_t)c->slices;
+  const size_t pt_len = (hp.db_item_size + chunks - 1) / chunks;            // params.bytes_per_chunk()
+  const BodyParse parsed = parse_update_body(body, len, 4 + chunks * pt_len, (uint64_t)c->dim0 * c->num_per);
+  // the reference reaches convert_pt_to_poly, which asserts logp == 8 (loading.rs:291), at the first well-formed entry
+  if (hp.p != 256 && !parsed.entries.empty()) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
+  if (pt_len > (size_t)POLY && !parsed.entries.empty()) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
+  const std::vector<BodyEntry> kept = keep_last_occurrence(parsed.entries);
+  std::vector<ItemWrite> all, group;
+  for (size_t k = 0; k < kept.size();) {
+    // one staging group: whole entries in body order, their bytes (dropped duplicates in between included) within the budget
+    const size_t k0 = k, base = kept[k].data_pos();
+    size_t end = base;
+    group.clear();
+    for (; k < kept.size() && group.size() < b200pir_ctx::kWriteStageItems; k++) {
+      const size_t e = kept[k].data_pos() + kept[k].data_len();
+      if (k > k0 && e - base > b200pir_ctx::kWriteStageBytes) break;
+      end = e;
+      const int ii = (int)(kept[k].db_idx % c->num_per), j = (int)(kept[k].db_idx / c->num_per);
+      if (ii % db->shard.count != db->shard.index) continue;                   // row lives on another GPU
+      group.push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)(ii / db->shard.count), (uint32_t)j});
+    }
+    write_items(c, db, body + base, end - base, group.data(), group.size());
+    all.insert(all.end(), group.begin(), group.end());
+  }
+  db->mark_items(all.data(), all.size(), c->stream);
+  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
+  B200_CUDA(cudaGetLastError());
+  if (parsed.error) throw Error(parsed.error, parsed.message);
+  if (largest_update) *largest_update = parsed.largest_update;
   API_END
 }
 
 // load_db_from_seek (lib/spiral-rs/src/server.rs:277-357; lib/server/src/db/loading.rs:192-247): `path` is the raw database,
 // item i at byte i * db_item_size.  Chunk c of item i is the bytes_per_chunk bytes at i * db_item_size + c * bytes_per_chunk,
 // clipped at the end of the FILE (as the reference's read does), each byte one plaintext coefficient; items past the end
-// of the file are zero polynomials.  Conversion (recenter, NTT, pack) and placement run on the GPU, `group` items per launch.
+// of the file are zero polynomials.  The file is read in groups of whole items (one read and one conversion-and-placement
+// launch per group, within the writers' staging budget); an item's bytes may overlap the next item's, as its chunks do.
 int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   API_BEGIN
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
@@ -918,34 +989,27 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   if (fbytes < 0) throw Error(B200PIR_E_BADARG, "cannot size the database file");
   const size_t flen = (size_t)fbytes;
   const size_t num_items = (size_t)c->dim0 * c->num_per;
-  const size_t group = 64;                                                    // items converted per launch
-  std::vector<uint8_t> host(group * chunks * bpc);
-  DevBuf<uint8_t> bucket(group * chunks * bpc);
-  DevBuf<uint64_t> polys(group * chunks * POLY);
+  const size_t item_span = chunks * bpc, isz = hp.db_item_size;
+  const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems,
+                                                    b200pir_ctx::kWriteStageBytes / std::max<size_t>(1, std::max(isz, item_span))));
+  std::vector<uint8_t> host;
+  std::vector<ItemWrite> items;
   for (size_t i0 = 0; i0 < num_items; i0 += group) {
     const size_t cnt = std::min(group, num_items - i0);
-    std::fill(host.begin(), host.end(), 0);
-    for (size_t k = 0; k < cnt; k++)
-      for (size_t ch = 0; ch < chunks; ch++) {
-        const size_t pos = (i0 + k) * hp.db_item_size + ch * bpc;
-        const size_t want = pos < flen ? std::min(bpc, flen - pos) : 0;
-        if (want && (fseeko(file.f, (off_t)pos, SEEK_SET) || fread(host.data() + (k * chunks + ch) * bpc, 1, want, file.f) != want))
-          throw Error(B200PIR_E_SHAPE, "short read from the database file");
-      }
-    B200_CUDA(cudaMemcpyAsync(bucket.p, host.data(), cnt * chunks * bpc, cudaMemcpyHostToDevice, c->stream));
-    launch_item_from_bytes(c->dp, bucket.p, (int)(cnt * chunks), (int)bpc, hp.p, polys.p, c->stream);
+    const size_t lo = i0 * isz, hi = std::min(flen, (i0 + cnt - 1) * isz + item_span);
+    const size_t span = hi > lo ? hi - lo : 0;
+    host.resize(span);
+    if (span && (fseeko(file.f, (off_t)lo, SEEK_SET) || fread(host.data(), 1, span, file.f) != span))
+      throw Error(B200PIR_E_SHAPE, "short read from the database file");
+    items.clear();
     for (size_t k = 0; k < cnt; k++) {
-      const size_t idx = i0 + k;
+      const size_t idx = i0 + k, pos = idx * isz;
       const int ii = (int)(idx % c->num_per), j = (int)(idx / c->num_per);
       if (ii % db->shard.count != db->shard.index) continue;                  // row lives on another GPU
-      for (size_t s = 0; s < chunks; s++) {
-        const uint64_t* poly = polys.p + (k * chunks + s) * POLY;
-        if (db->format == 0) launch_db_upsert(c->geom(db->rows), db->d.p, (int)s, ii / db->shard.count, j, poly, c->stream);
-        else if (db->format == 2) launch_db_upsert_tc5(db->T, db->t.p, (int)s, ii / db->shard.count, j, poly, c->stream);
-        else launch_db_upsert_frag(db->F, db->f.p, (int)s, ii / db->shard.count, j, poly, c->stream);
-      }
+      const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0;   // clipped at the end of the file
+      items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)(ii / db->shard.count), (uint32_t)j});
     }
-    B200_CUDA(cudaStreamSynchronize(c->stream));                              // `host` is refilled next
+    write_items(c, db, host.data(), span, items.data(), items.size());        // pageable `host`: staged before the call returns
   }
   for (int s = 0; s < c->slices; s++) db->mark_slice(s, c->stream);            // load_db_from_seek builds a dense database
   B200_CUDA(cudaStreamSynchronize(c->stream));

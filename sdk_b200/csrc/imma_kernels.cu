@@ -21,6 +21,7 @@
 // One CTA = one (slice, n, z): its 8 warps share the query operand B (<= 32 KiB, shared memory) and each streams
 // the fragments of two row tiles.
 #include "kernels.h"
+#include "item_place.cuh"
 
 namespace b200pir {
 
@@ -84,17 +85,8 @@ k_db_to_frag(ImmaGeom F, const uint4* __restrict__ db0_slice, uint4* __restrict_
 __global__ void k_db_upsert_frag(ImmaGeom F, uint4* dbf, int slice, int il, int j, const uint64_t* poly) {
   int z = blockIdx.x * blockDim.x + threadIdx.x;
   if (z >= POLY) return;
-  const int mt = il >> 4, row = il & 15, ks = j >> 5, k = j & 31;
-  const int g = row & 7, rh = row >> 3, kh = k >> 4, t = (k & 15) >> 2, i = k & 3;
-  const int lane = g * 4 + t, reg = rh + 2 * kh;       // a0..a3 = (row g,k lo), (row g+8,k lo), (row g,k hi), (row g+8,k hi)
-  uint64_t w = poly[z];
-#pragma unroll
-  for (int n = 0; n < 2; n++) {
-    uint32_t r = n ? (uint32_t)(w >> 32) : (uint32_t)w;
-    uint8_t* base = reinterpret_cast<uint8_t*>(dbf + (((((size_t)slice * 2 + n) * POLY + z) * F.mt + mt) * F.ks + ks) * 4 * 32);
-#pragma unroll
-    for (int l = 0; l < 4; l++) base[((size_t)l * 32 + lane) * 16 + reg * 4 + i] = (uint8_t)((r >> (7 * l)) & 127u);
-  }
+  const uint64_t w = poly[z];
+  place_frag(F, dbf, slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
 }
 
 // expanded queries (format of mul_kernels.cu: uint4 [jp][jb][z]) -> B fragments

@@ -72,9 +72,6 @@ void launch_db_retile_chunk(const MulGeom& G, Shard sh, uint4* db_dev_slice, con
                             cudaStream_t s);
 // one item poly (2048 packed words, lo|hi<<32) -> its place in db_dev   (lib/server db/loading.rs:317-359)
 void launch_db_upsert(const MulGeom& G, uint4* db_dev, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
-// lib/server db/loading.rs:278-299,34-41: `chunks` chunks of pt_len bytes -> packed item polynomials [chunks][2048]
-void launch_item_from_bytes(const DevParams& P, const uint8_t* bucket, int chunks, int pt_len, uint64_t pt_modulus,
-                            uint64_t* out, cudaStream_t s);
 // synthetic DB: plaintext coeff = splitmix64(seed, ((slice*items + item)*2048 + z)) % p, recentred, NTT'd, packed
 // (server.rs:223-275 with a counter PRNG; item = j*num_per_global + ii)
 void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_dev, uint64_t seed, uint64_t pt_modulus,
@@ -117,6 +114,20 @@ void launch_reorient_to_tc5(const Tc5Geom& T, const uint32_t* v, size_t v_stride
 // neither fetched nor multiplied (lib/server's sparse database: absent items cost nothing, db/sparse_db.rs, dot_product.rs:35)
 void launch_multiply_tc5(const DevParams& P, const Tc5Geom& T, const uint8_t* dbt, const uint32_t* tile_mask, const uint8_t* qt,
                          uint32_t* out_zm, size_t out_stride, int nq, int slice_begin, int slice_count, int sm_count, cudaStream_t s);
+
+// ---- raw item bytes -> database (lib/server db/loading.rs:317-359 update_item_raw, batched)
+// One database as the writer sees it: its layout and the geometry / storage of that layout (local rows).
+struct DbDst {
+  int format;               // 0: d (IMAD layout), 1: f (mma.sync fragments), 2: t (wgmma tile images)
+  MulGeom G; ImmaGeom F; Tc5Geom T;
+  uint4* d; uint4* f; uint8_t* t;
+};
+// item = the raw bytes [off, off + len) of the staged buffer, written to local row il, column j of every slice
+struct ItemWrite { uint32_t off, len, il, j; };
+// every (item, chunk c < chunks) pair: chunk c = bytes [c * bpc, (c + 1) * bpc) of the item, zero past its len, converted
+// (recenter_mod, NTT, pack: loading.rs:278-299, 34-41) and placed at the item's cell of slice c.  One launch.
+void launch_write_items(const DevParams& P, const DbDst& D, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
+                        int bpc, uint64_t pt_modulus, cudaStream_t s);
 
 // ---- second dimension
 // mult output ntt32 [cnt][r][n][z] -> raw ciphertexts u64 [cnt][r][z]   (server.rs:707-709)

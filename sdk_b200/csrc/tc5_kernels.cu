@@ -26,6 +26,7 @@
 // warp 8 = bulk-copy producer.  Pipelines: A ring (full/empty mbarriers), double-buffered B operand (bfull/bempty).  The ring
 // keeps the copies in flight while the consumers run the epilogue of a tile.
 #include "kernels.h"
+#include "item_place.cuh"
 #include "tc5_ptx.cuh"
 
 namespace b200pir {
@@ -60,15 +61,8 @@ k_db_to_tc5(Tc5Geom T, const uint4* __restrict__ db0_slice, uint8_t* __restrict_
 __global__ void k_db_upsert_tc5(Tc5Geom T, uint8_t* dbt, int slice, int il, int j, const uint64_t* poly) {
   const int z = blockIdx.x * blockDim.x + threadIdx.x;
   if (z >= POLY) return;
-  const int mt = il >> 5, row_local = il & 31, ks = j >> 5, k = j & 31;
   const uint64_t w = poly[z];
-#pragma unroll
-  for (int n = 0; n < 2; n++) {
-    const uint32_t r = n ? (uint32_t)(w >> 32) : (uint32_t)w;
-    uint8_t* tile = dbt + tc5_db_tile(T, slice, n, z, mt, ks) * TC5_TILE;
-#pragma unroll
-    for (int l = 0; l < 4; l++) tile[tc5_tile_off(tc5_m_index(row_local, l), k)] = (uint8_t)((r >> (7 * l)) & 127u);
-  }
+  place_tc5(T, dbt, slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
 }
 
 // expanded queries (uint4 [j][z] per query, q_stride apart) -> qT.  CTA = (pair of z, ks): every 32-byte sector it reads is

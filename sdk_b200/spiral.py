@@ -162,6 +162,15 @@ class Database:
         data = np.ascontiguousarray(data, dtype=np.uint8)
         check(LIB.b200pir_db_update_item_raw(self.params._h, self._h, db_idx, data.ctypes.data, data.size))
 
+    def update_many_items(self, body):
+        """lib/server/src/db/loading.rs:361-377: apply a whole /update-row body ([u32 BE chunk_len][u32 BE db_idx][bytes]
+        entries) in one call; returns largest_update.  On a bad entry the entries before it stay applied and this raises."""
+        body = np.ascontiguousarray(np.frombuffer(body, dtype=np.uint8) if isinstance(body, (bytes, bytearray)) else body,
+                                    dtype=np.uint8)
+        largest = C.c_uint64(0)
+        check(LIB.b200pir_db_update_many_items(self.params._h, self._h, body.ctypes.data, body.size, C.byref(largest)))
+        return largest.value
+
     def fill_synthetic(self, seed):
         check(LIB.b200pir_db_fill_synthetic(self.params._h, self._h, seed))
 
