@@ -58,7 +58,8 @@ int b200pir_ctx_synchronize(b200pir_ctx* ctx);
  * "expand_variant" (0 = default everywhere); "fold_variant" (accepted, no effect: there is one fold kernel); "coalesce" (1 = default: concurrent single-query callers
  * share database passes, see b200pir_coalesce_stats), "coalesce_window_us" (default 200: how long a batch that directly
  * follows a multi-query batch is held open for the callers of that batch to return; 0 = never), "sparse_fold" (1 = fold like lib/server's sparse server,
- * compute/fold.rs:15-65: an all-zero ciphertext short-cuts the external product; 0 = spiral-rs's dense fold, default); "expand_pair_min_ctas" (expansion rounds with at least this many active
+ * compute/fold.rs:15-65: an all-zero ciphertext short-cuts the external product; 0 = spiral-rs's dense fold, default; version-1
+ * servers set 1: with t_gsw = 7 the dense fold does not decode items whose row is folded against an empty one); "expand_pair_min_ctas" (expansion rounds with at least this many active
  * ciphertexts use the paired kernel, default 1: every round);
  * unknown keys -> B200PIR_E_BADARG */
 int b200pir_ctx_set_option(b200pir_ctx* ctx, const char* key, int64_t value);

@@ -337,6 +337,17 @@ int orc_client_decode_response(void* c, const uint8_t* data, size_t len, uint64_
   std::memcpy(out, r.data.data(), r.data.size() * 8);
   ORC_CATCH
 }
+uint64_t orc_q2_value(size_t q2_bits) { return Q2_VALUES[q2_bits]; }
+// out: the pre-rounding numerators of decode_response (client.rs:780-800), one int64 per coefficient of the
+// (instances*n) x n result
+int orc_client_decode_numerators(void* c, const uint8_t* data, size_t len, int64_t* out) {
+  ORC_TRY
+  Client& cl = *(Client*)c;
+  std::vector<uint8_t> buf(data, data + len);
+  buf.resize(len + 16, 0);
+  cl.decode_response_poly(buf.data(), out);
+  ORC_CATCH
+}
 // encrypt a raw 1x1 plaintext poly (already scaled) as a Regev ciphertext; returns NTT 2x1 (stage tests)
 int orc_client_encrypt_reg(void* c, const uint64_t* sigma_raw, uint64_t* out_ntt) {
   ORC_TRY

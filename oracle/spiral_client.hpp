@@ -325,8 +325,9 @@ struct Client {
     return q;
   }
   // client.rs:732-810.  Returns the decoded (instances*n) x n plaintext matrix (mod p), i.e.
-  // `result` before `to_vec` (:809).
-  PolyMatrix decode_response_poly(const uint8_t* data) {
+  // `result` before `to_vec` (:809).  `numer` (optional, same shape): the numerator each coefficient is rounded from,
+  // val_first * q1 + val_rest * q2 (:780-800); the coefficient is that divided by q2 * (q1 / p), rounded half away from zero.
+  PolyMatrix decode_response_poly(const uint8_t* data, int64_t* numer = nullptr) {
     u64 pm = p.pt_modulus;
     u64 q1 = 4 * p.pt_modulus;
     size_t q1_bits = log2_ceil(q1);
@@ -357,6 +358,7 @@ struct Client {
         if (val_rest >= q1_i / 2) val_rest -= q1_i;
         i64 denom = (i64)(q2 * (q1 / pm));
         i64 r = val_first * q1_i + val_rest * q2_i;
+        if (numer) numer[inst * p.n * p.n * N + i] = r;
         i64 sign = r >= 0 ? 1 : -1;
         i128 res = ((i128)(r + sign * (denom / 2))) / (i128)denom;
         res = (res + ((i128)denom / p_i) * p_i + 2 * p_i) % p_i;

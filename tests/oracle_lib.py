@@ -49,6 +49,8 @@ def _load():
     lib.orc_splitmix64_at.argtypes = [C.c_uint64] * 2
     lib.orc_read_bits.argtypes = [u8p, C.c_size_t, C.c_size_t]
     lib.orc_write_bits.argtypes = [u8p, C.c_uint64, C.c_size_t, C.c_size_t]
+    lib.orc_q2_value.restype = C.c_uint64
+    lib.orc_q2_value.argtypes = [C.c_size_t]
     lib.orc_response_bytes.restype = C.c_size_t
     lib.orc_response_bytes.argtypes = [C.c_void_p]
     lib.orc_time_multiply.restype = C.c_double
@@ -130,6 +132,7 @@ class Params:
         self.W = self.crt_count * self.poly_len
         self.num_packing = self.n if self.version == 0 else 2
         self.has_right = expand_queries and (self.version == 0 or self.t_exp_right != self.t_exp_left)
+        self.q2 = int(LIB.orc_q2_value(self.q2_bits))
 
     @staticmethod
     def named(name, **over):
@@ -378,6 +381,16 @@ class Client:
         out = np.zeros(p.instances * p.n * p.n * p.N, dtype=np.uint64)
         resp = np.ascontiguousarray(resp, dtype=np.uint8)
         _ck(LIB.orc_client_decode_response(C.c_void_p(self.h), _p8(resp), C.c_size_t(resp.size), _p64(out)))
+        return out
+
+    def decode_numerators(self, resp):
+        """The numerators decode_response rounds (client.rs:780-800): int64, same layout as decode_response's output.
+        Coefficient k decodes to round(numer[k] / denom) mod p with denom = q2 * (q1 / p) = q2 * 4."""
+        p = self.p
+        out = np.zeros(p.instances * p.n * p.n * p.N, dtype=np.int64)
+        resp = np.ascontiguousarray(resp, dtype=np.uint8)
+        _ck(LIB.orc_client_decode_numerators(C.c_void_p(self.h), _p8(resp), C.c_size_t(resp.size),
+                                             out.ctypes.data_as(C.POINTER(C.c_int64))))
         return out
 
     def encrypt_reg(self, sigma_raw):

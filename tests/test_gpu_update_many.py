@@ -79,8 +79,10 @@ def test_update_many_items_matches_oracle(name, fmt):
         assert np.array_equal(S.multiply_reg_by_database(G, gdb, s, v), S.multiply_reg_by_database(G, seq, s, v)), (name, fmt, s)
     distinct = {idx for idx, _ in applied}
     assert gdb.info()["present_items"] == len(distinct) * P.slices == seq.info()["present_items"]
-    # a private read of written items: response bytes == the oracle's process_query over the restated database, and (version 0
-    # parameter sets) the response decodes to the last bytes written to the item
+    # a private read of written items: response bytes == the oracle's process_query over the restated database, and the
+    # response decodes to what the fold reads back (update_rows_oracle.read_back).  Decoded with the fold each version is
+    # served with: spiral-rs's dense fold (the default) on version 0, lib/server's ("sparse_fold") on version 1, where the
+    # dense fold loses the margin next to empty rows (test_oracle_written_items_decode.py).
     last = {idx: data for idx, data in applied}
     pt_len = P.bytes_per_chunk
     for idx in sorted(distinct)[:4]:
@@ -88,11 +90,16 @@ def test_update_many_items_matches_oracle(name, fmt):
         resp = S.process_query(G, gpp, S.Query(ct=q["ct"]), gdb)
         assert np.array_equal(resp, P.process_query(pp, q, ref_db.reshape(-1))), (name, fmt, idx)
         assert np.array_equal(resp, S.process_query(G, gpp, S.Query(ct=q["ct"]), seq)), (name, fmt, idx)
-        if P.version == 0:
-            got = cl.decode_response(resp).reshape(P.slices, P.N)[:, :pt_len].astype(np.uint8).reshape(-1)
-            exp = np.zeros(P.slices * pt_len, dtype=np.uint8)
-            exp[:last[idx].size] = last[idx]
-            assert np.array_equal(got, exp), (name, fmt, idx, int(np.count_nonzero(got != exp)))
+        if P.version == 1:
+            G.set_option("sparse_fold", 1)
+            try:
+                resp = S.process_query(G, gpp, S.Query(ct=q["ct"]), gdb)
+            finally:
+                G.set_option("sparse_fold", 0)
+            assert np.array_equal(resp, P.process_query(pp, q, ref_db.reshape(-1), sparse_fold=True)), (name, fmt, idx)
+        got = cl.decode_response(resp).reshape(P.slices, P.N)[:, :pt_len].astype(np.uint8).reshape(-1)
+        exp = U.read_back(P, ref_db, last, idx, sparse_fold=P.version == 1)
+        assert np.array_equal(got, exp), (name, fmt, idx, int(np.count_nonzero(got != exp)))
     gdb.close()
     seq.close()
 

@@ -65,6 +65,35 @@ def update_many_items(P, body, db=None):
     return db, largest, err, applied
 
 
+def read_back(P, db, items, idx, sparse_fold):
+    """The bytes ([slices * bytes_per_chunk] uint8) a private read of item `idx` decodes to from `db` (as update_many_items
+    returns it), where `items` maps every written db_idx to its bytes.  The dense fold returns item idx.  lib/server's fold
+    (compute/fold.rs:37-43) keeps the non-zero ciphertext of a pair when the other is all-zero, whichever one the query
+    selects, so in a slice where the target's second-dimension row is empty it can return another row's item of the same
+    column."""
+    num_per, bpc = P.num_per, P.bytes_per_chunk
+    ii, j = idx % num_per, idx // num_per
+    nonzero = (db.reshape(P.slices, P.N, num_per, P.dim0) != 0).any(axis=(1, 3))
+    out = np.zeros((P.slices, bpc), dtype=np.uint8)
+    for s in range(P.slices):
+        row = ii
+        if sparse_fold:
+            cand = [r if nonzero[s, r] else None for r in range(num_per)]
+            half, bit = num_per // 2, P.nu_2 - 1           # round k folds rows i and i + half by bit nu_2 - 1 - k of ii
+            while half >= 1:
+                sel = (ii >> bit) & 1
+                for i in range(half):
+                    a, b = cand[i], cand[i + half]
+                    cand[i] = b if a is None else a if b is None else (b if sel else a)
+                half, bit = half // 2, bit - 1
+            row = cand[0]
+        data = items.get(j * num_per + row) if row is not None else None
+        if data is not None:
+            chunk = np.asarray(data, dtype=np.uint8)[s * bpc:(s + 1) * bpc]
+            out[s, :chunk.size] = chunk
+    return out.reshape(-1)
+
+
 def entry(db_idx, data):
     """One /update-row entry: [u32 BE chunk_len][u32 BE db_idx][data]."""
     data = bytes(data) if isinstance(data, (bytes, bytearray)) else np.asarray(data, dtype=np.uint8).tobytes()
