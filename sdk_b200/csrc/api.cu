@@ -605,6 +605,12 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   c->g = (int)log2_ceil_u64(hp.t_gsw * hp.nu_2 + c->dim0);
   c->stop_round = hp.nu_2 ? (int)log2_ceil_u64(hp.t_gsw * hp.nu_2) : 0;
   if (c->g > 11) throw Error(B200PIR_E_UNSUPPORTED, "expansion needs more than 2048 slots");
+  // expand_query takes the first-dimension ciphertexts from the even slots and the GSW inputs from the odd slots
+  // (server.rs:565-571), so each half must fit in 2^(g-1) slots; 2^g only bounds their sum.  With t_gsw * nu_2 = 18 and
+  // dim0 = 4, for instance, g = 5 and the odd slots run to 35: the reference panics on the index, and the expansion and
+  // conversion kernels would read past the query's workspace.
+  if (hp.expand_queries && hp.nu_2 > 0 && 2 * std::max<uint64_t>(c->dim0, hp.t_gsw * hp.nu_2) > (1ull << c->g))
+    throw Error(B200PIR_E_UNSUPPORTED, "expansion: dim0 and t_gsw * nu_2 must each fit in half of the 2^g slots");
   c->num_packing = hp.version == 0 ? (int)hp.n : 2;
   c->has_right = hp.expand_queries && (hp.version == 0 || hp.t_exp_right != hp.t_exp_left);
   c->bits_gsw = bits_per((int)hp.t_gsw);
@@ -1335,11 +1341,19 @@ int b200pir_fold_ciphertexts(b200pir_ctx* c, uint64_t* v_cts, size_t num, const 
   B200_CUDA(cudaMemcpyAsync(cts.p, v_cts, cts.n * 8, cudaMemcpyHostToDevice, c->stream));
   B200_CUDA(cudaMemcpyAsync(wide.p, v_folding, wide.n * 8, cudaMemcpyHostToDevice, c->stream));
   launch_narrow(vf.p, wide.p, wide.n, c->stream);
-  if (v_folding_neg && !c->sparse_fold) {
+  // The fast path works on residues, where a raw coefficient q (kernels.h) is stored as 0: its gadget digits would be 0's, and
+  // a slot the loop never folds would come back as 0.  process_query never hands q to the fold (its inputs come out of from_ntt),
+  // but a caller of this stage may: such inputs take the raw-coefficient path with v_folding_neg computed from v_folding.
+  const bool has_q = std::find(v_cts, v_cts + cts.n, c->dp.modulus) != v_cts + cts.n;
+  if ((v_folding_neg || has_q) && !c->sparse_fold) {
     // general path: honours an arbitrary v_folding_neg exactly as server.rs:405-425 does
     DevBuf<uint32_t> vfn(c->fold_words());
-    B200_CUDA(cudaMemcpyAsync(wide.p, v_folding_neg, wide.n * 8, cudaMemcpyHostToDevice, c->stream));
-    launch_narrow(vfn.p, wide.p, wide.n, c->stream);
+    if (v_folding_neg) {
+      B200_CUDA(cudaMemcpyAsync(wide.p, v_folding_neg, wide.n * 8, cudaMemcpyHostToDevice, c->stream));
+      launch_narrow(vfn.p, wide.p, wide.n, c->stream);
+    } else {
+      launch_folding_neg(c->dp, vfn.p, vf.p, dims, (int)c->hp.t_gsw, c->bits_gsw, c->stream);
+    }
     run_fold(c, cts.p, 1, num * 2 * POLY, num, dims - 1, vf.p, vfn.p, 1);
   } else {
     // fast path (what process_query uses): v_folding_neg = get_v_folding_neg(v_folding) implied.
@@ -1443,7 +1457,8 @@ int b200pir_pack(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* v_ct, uint64_t*
   DevBuf<uint32_t> o(outp * 2 * POLY), res(nn * 4 * POLY);
   B200_CUDA(cudaMemcpyAsync(cts.p, v_ct, cts.n * 8, cudaMemcpyHostToDevice, c->stream));
   launch_raw_to_res(c->dp, res.p, cts.p, nn * 2, c->stream);
-  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, c->pp_table(pp, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, (int)hp.version, c->stream);
+  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, c->pp_table(pp, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, (int)hp.version, c->stream,
+              cts.p);
   // the reference's pack returns the NTT-form matrix (server.rs:467); the kernel already applied .raw()
   launch_to_ntt(c->dp, o.p, raw.p, outp, c->stream);
   launch_widen(wide.p, o.p, o.n, c->stream);

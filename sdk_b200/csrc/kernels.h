@@ -182,9 +182,11 @@ void launch_regev_to_gsw(const DevParams& P, uint32_t* v_gsw, size_t gsw_stride,
 // folded: residue-form ciphertexts, ct (inst, t) at folded + (inst*n*n + t)*ct_stride (u32 words);
 // w: ntt32 packing matrices; out: raw [inst][n+1][n][2048]
 // nq queries per launch: query k reads folded + k*in_q_stride and writes out_raw + k*out_q_stride
+// raw_cts (optional, nq = 1): the same ciphertexts as raw u64 [inst][n*n][2][2048]; row 0 is then decomposed from these values,
+// so a coefficient q (which the residue form stores as 0) yields q's gadget digits, as the reference's pack does
 void launch_pack(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride,
                  size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int n, int instances, int t_conv, int bits_conv,
-                 int version, cudaStream_t s);
+                 int version, cudaStream_t s, const uint64_t* raw_cts = nullptr);
 // out: nq x out_bytes; packed_raw: nq matrices packed_q_stride words apart
 void launch_encode(const DevParams& P, uint8_t* out, size_t out_bytes, const uint64_t* packed_raw, size_t packed_q_stride,
                    int nq, int n, int instances, uint64_t q2, int q2_bits, uint64_t q1, int q1_bits, cudaStream_t s);

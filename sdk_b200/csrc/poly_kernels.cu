@@ -1025,7 +1025,7 @@ k_regev_to_gsw(DevParams P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* 
 template <int ROWS>
 __global__ void __launch_bounds__(CTA, 1)
 k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride, size_t in_q_stride,
-       const uint32_t* const* tab_pack, int t_conv, int bits, int version) {
+       const uint32_t* const* tab_pack, int t_conv, int bits, int version, const uint64_t* __restrict__ raw_cts) {
   const uint32_t* v_packing = tab_pack[blockIdx.y];
   out_raw += (size_t)blockIdx.y * out_q_stride;
   folded += (size_t)blockIdx.y * in_q_stride;
@@ -1061,8 +1061,14 @@ k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* fold
     int cnt = 0;
     {
       uint64_t vv[8];
+      if (raw_cts) {          // row 0 as given: a coefficient q decomposes into q's digits (gadget.rs:34-60), not 0's
+        const uint64_t* ct0 = raw_cts + ((size_t)inst * n * n + (size_t)r * n + c) * 2 * POLY;
 #pragma unroll
-      for (int a = 0; a < 8; a++) vv[a] = crt_compose(__ldg(ct + a * 256 + g.tid), __ldg(ct + POLY + a * 256 + g.tid), P);
+        for (int a = 0; a < 8; a++) vv[a] = __ldg(ct0 + a * 256 + g.tid);
+      } else {
+#pragma unroll
+        for (int a = 0; a < 8; a++) vv[a] = crt_compose(__ldg(ct + a * 256 + g.tid), __ldg(ct + POLY + a * 256 + g.tid), P);
+      }
       digits_mac<ROWS, true>(acc, cnt, RegCoef{vv}, t_conv, bits, W + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
     }
     uint32_t y[8];
@@ -1304,20 +1310,21 @@ void launch_regev_to_gsw(const DevParams& P, uint32_t* v_gsw, size_t gsw_stride,
 template <int ROWS>
 static void launch_pack_t(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded,
                           size_t ct_stride, size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int instances,
-                          int t_conv, int bits_conv, int version, cudaStream_t s) {
+                          int t_conv, int bits_conv, int version, const uint64_t* raw_cts, cudaStream_t s) {
   opt_in_smem(k_pack<ROWS>, (int)kDynSmemBig);
   ++g_kernel_launches;
   k_pack<ROWS><<<dim3((unsigned)(instances * (ROWS - 1)), nq), CTA, kDynSmemBig, s>>>(
-      P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, tab_pack, t_conv, bits_conv, version);
+      P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, tab_pack, t_conv, bits_conv, version, raw_cts);
 }
 void launch_pack(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride,
                  size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int n, int instances, int t_conv, int bits_conv,
-                 int version, cudaStream_t s) {
+                 int version, cudaStream_t s, const uint64_t* raw_cts) {
+  if (raw_cts && nq != 1) throw Error(-2, "pack: raw ciphertexts are taken for one query");
   switch (n) {
-    case 1: launch_pack_t<2>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, s); break;
-    case 2: launch_pack_t<3>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, s); break;
-    case 3: launch_pack_t<4>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, s); break;
-    case 4: launch_pack_t<5>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, s); break;
+    case 1: launch_pack_t<2>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
+    case 2: launch_pack_t<3>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
+    case 3: launch_pack_t<4>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
+    case 4: launch_pack_t<5>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
     default: throw Error(-2, "pack: n must be 1..4");
   }
 }
