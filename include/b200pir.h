@@ -104,6 +104,27 @@ int b200pir_db_update_item_raw(b200pir_ctx* ctx, b200pir_db* db, uint64_t db_idx
  * A db_idx written more than once ends with its last bytes.  On a shard every entry is checked and only its own rows are
  * written.  Conversion and placement run on the GPU; synchronises the context's stream before it returns. */
 int b200pir_db_update_many_items(b200pir_ctx* ctx, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update);
+/* ---- reading the database back (the inverse of the loaders above) ----
+ * Write slice `slice` in the reference layout [z][ii][j] (n_words = dim0*num_per*2048), the inverse of b200pir_db_upload_slice.
+ * Only the words of the rows this database holds are written (ii = shard_index mod shard_count); the words of other shards'
+ * rows are left untouched, so the G shards of a database downloading into one buffer assemble the whole slice.  Absent items
+ * are zero words.  Round trip: a word whose halves are canonical residues (lo < q0, hi < q1), the only words any writer of this
+ * library produces, comes back exactly as it was uploaded.  Format 0 stores both 32-bit halves verbatim and returns any
+ * uploaded word unchanged; formats 1 and 2 store four 7-bit limbs per residue and return the low 28 bits of each half.
+ * Read-only: the database, its presence map and b200pir_db_present_items are unchanged.  The context lock is held only while
+ * one staging chunk (<= 64 MiB) is un-tiled and copied to pinned host memory, not while it is scattered into `words`, so
+ * queries on the same context keep being served during an export; exports on one context run one at a time.  Consistency
+ * with writers is the caller's: hold the read side of the lock that writers take exclusively (INTEGRATION.md §4).
+ * Null pointers -> B200PIR_E_BADARG; wrong n_words or slice >= slices -> B200PIR_E_SHAPE. */
+int b200pir_db_download_slice(b200pir_ctx* ctx, b200pir_db* db, uint64_t slice, uint64_t* words, size_t n_words);
+/* Every slice: the `db: &[u64]` that b200pir_db_upload takes (n_words = slices*dim0*num_per*2048). */
+int b200pir_db_download(b200pir_ctx* ctx, b200pir_db* db, uint64_t* words, size_t n_words);
+/* Write the whole database to `path` as the native-endian u64 stream that b200pir_db_load_file and the reference's
+ * load_preprocessed_db_from_file read.  Atomic: the words go to a temporary file in the same directory (mode 0600), which is
+ * fsync'ed and renamed over `path`; if the save fails, an earlier file at `path` is intact and no temporary file is left.
+ * Locking as b200pir_db_download.  Unsharded databases only (B200PIR_E_UNSUPPORTED otherwise); a file that cannot be created
+ * or written -> B200PIR_E_BADARG, with the path in b200pir_last_error(). */
+int b200pir_db_save_file(b200pir_ctx* ctx, b200pir_db* db, const char* path);
 /* Synthetic database generated on the GPU: plaintext coefficient = splitmix64(seed, ((slice*items+item)*2048+z)) % p,
  * then recenter_mod / NTT / pack as generate_random_db_and_get_item does (server.rs:223-275). */
 int b200pir_db_fill_synthetic(b200pir_ctx* ctx, b200pir_db* db, uint64_t seed);

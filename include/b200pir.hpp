@@ -95,6 +95,15 @@ struct Database {
     check(b200pir_db_update_many_items(params.ctx, h, body, len, &largest_update));
     return largest_update;
   }
+  // read back: the reference layout of every slice (b200pir_db_download; a shard writes only its own rows of `words`)
+  void download(uint64_t* words, size_t n_words) const { check(b200pir_db_download(params.ctx, h, words, n_words)); }
+  std::vector<uint64_t> words() const {
+    std::vector<uint64_t> w(params.slices() * params.dim0() * params.num_per() * 2048, 0);
+    download(w.data(), w.size());
+    return w;
+  }
+  // the file b200pir_db_load_file reads, written atomically (unsharded databases)
+  void save_file(const char* path) const { check(b200pir_db_save_file(params.ctx, h, path)); }
 };
 
 namespace ntt {

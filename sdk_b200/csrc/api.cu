@@ -7,6 +7,9 @@
 #include "ntt_tables.hpp"
 #include "update_body.hpp"
 #include <cstdio>
+#include <cerrno>
+#include <fcntl.h>
+#include <unistd.h>
 #include <algorithm>
 #include <cmath>
 #include <memory>
@@ -124,6 +127,27 @@ struct b200pir_ctx {
   static constexpr size_t kWriteStageItems = 65536;
   DevBuf<uint8_t> w_wbytes;
   DevBuf<ItemWrite> w_witems;
+  // database exports (download, save_file): chunks are un-tiled into w_wbytes and copied to one of two pinned buffers, one
+  // event each; allocated on the first export, freed in b200pir_ctx_destroy.  Exports share them, so export_mu serialises
+  // exports with each other; queries only contend for `mu`, which an export holds per chunk.
+  std::mutex export_mu;
+  uint8_t* h_export[2] = {nullptr, nullptr};
+  size_t h_export_bytes = 0;
+  cudaEvent_t export_done[2] = {nullptr, nullptr};
+  void ensure_export_staging(size_t bytes) {
+    w_wbytes.ensure(std::max(kWriteStageBytes, bytes));
+    if (!export_done[0])
+      for (auto& e : export_done) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming | cudaEventBlockingSync));
+    if (bytes <= h_export_bytes) return;
+    release_export_pinned();
+    const size_t n = std::max(kWriteStageBytes, bytes);
+    for (auto& h : h_export) B200_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h), n, cudaHostAllocDefault));
+    h_export_bytes = n;
+  }
+  void release_export_pinned() {
+    for (auto& h : h_export) { if (h) cudaFreeHost(h); h = nullptr; }
+    h_export_bytes = 0;
+  }
   // Coalescing of concurrent callers ("coalesce", default on): lib/server takes a READ lock around process_query
   // (bin/server.rs:102), so actix workers call it concurrently.  Requests arriving while a batch runs queue up here; the
   // thread that finds no batch in flight becomes the leader and serves everything queued (up to kCoalesceMax) in ONE
@@ -690,6 +714,8 @@ void b200pir_ctx_destroy(b200pir_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   for (auto e : c->event_pool) cudaEventDestroy(e);
+  c->release_export_pinned();
+  for (auto e : c->export_done) if (e) cudaEventDestroy(e);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
   delete c;
 }
@@ -842,6 +868,63 @@ void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t spa
   const DbDst dst{db->format, c->geom(db->rows), db->F, db->T, db->d.p, db->f.p, db->t.p};
   launch_write_items(c->dp, dst, c->w_wbytes.p, c->w_witems.p, (int)count, (int)chunks, (int)bpc, c->hp.p, c->stream);
 }
+
+// Database export, shared by b200pir_db_download(_slice) and b200pir_db_save_file.  A chunk is one slice and a range of z of
+// the local rows, at most the writers' 64 MiB device staging (w_wbytes).  Under the context lock one launch un-tiles it into
+// [zc][rows][dim0] u64 there and the chunk is queued for a copy to one of the two pinned buffers; the lock is then released and
+// `sink(slice, z0, zc, words)` consumes the previous chunk once its copy has landed, while the GPU un-tiles and copies this
+// one.  Everything is ordered on the context's stream, so a chunk's un-tiling never overwrites staging its copy still reads.
+template <typename Sink>
+void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
+  std::lock_guard<std::mutex> ex(c->export_mu);
+  const size_t per_z = (size_t)db->rows * c->dim0;
+  const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
+  struct Chunk { int slice, z0, zc; };
+  std::vector<Chunk> chunks;
+  for (int s = slice_begin; s < slice_end; s++)
+    for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
+  {
+    Guard gd(c);
+    c->ensure_export_staging(per_z * zc * 8);
+  }
+  auto consume = [&](size_t k) {
+    const int b = (int)(k & 1);
+    B200_CUDA(cudaEventSynchronize(c->export_done[b]));
+    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<const uint64_t*>(c->h_export[b]));
+  };
+  try {
+    for (size_t k = 0; k < chunks.size(); k++) {
+      {
+        Guard gd(c);
+        const DbDst dst{db->format, c->geom(db->rows), db->F, db->T, db->d.p, db->f.p, db->t.p};
+        uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
+        launch_db_export(dst, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
+        B200_CUDA(cudaMemcpyAsync(c->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, c->stream));
+        B200_CUDA(cudaEventRecord(c->export_done[k & 1], c->stream));
+      }
+      if (k > 0) consume(k - 1);
+    }
+    if (!chunks.empty()) consume(chunks.size() - 1);
+  } catch (...) {
+    for (auto e : c->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
+    throw;
+  }
+  B200_CUDA(cudaGetLastError());
+}
+
+// the local rows of slices [slice_begin, slice_end) into `words` (the reference layout of those slices): ii = il * G + index
+void download_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, uint64_t* words) {
+  const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per, rows = (size_t)db->rows;
+  const size_t G = (size_t)db->shard.count, gi = (size_t)db->shard.index;
+  const size_t slice_words = d0 * npg * POLY;
+  export_impl(c, db, slice_begin, slice_end, [&](int s, int z0, int zc, const uint64_t* src) {
+    uint64_t* dst = words + (size_t)(s - slice_begin) * slice_words + (size_t)z0 * npg * d0;
+    if (G == 1) { std::memcpy(dst, src, (size_t)zc * rows * d0 * 8); return; }
+    for (size_t zl = 0; zl < (size_t)zc; zl++)
+      for (size_t il = 0; il < rows; il++)
+        std::memcpy(dst + (zl * npg + il * G + gi) * d0, src + (zl * rows + il) * d0, d0 * 8);
+  });
+}
 }  // namespace
 }  // extern "C++"
 
@@ -890,6 +973,68 @@ int b200pir_db_upload(b200pir_ctx* c, b200pir_db* db, const uint64_t* words, siz
     if (rc) return rc;
   }
   return 0;
+}
+int b200pir_db_download_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t* words, size_t n_words) {
+  API_BEGIN
+  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  const size_t slice_words = (size_t)c->dim0 * c->num_per * POLY;
+  if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
+  if (n_words != slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
+  download_impl(c, db, (int)slice, (int)slice + 1, words);
+  API_END
+}
+int b200pir_db_download(b200pir_ctx* c, b200pir_db* db, uint64_t* words, size_t n_words) {
+  API_BEGIN
+  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  if (n_words != (size_t)c->dim0 * c->num_per * POLY * c->slices) throw Error(B200PIR_E_SHAPE, "db must hold slices*dim0*num_per*2048 words");
+  download_impl(c, db, 0, c->slices, words);
+  API_END
+}
+// The file b200pir_db_load_file reads, written atomically: a temporary file in the target's directory is written chunk by
+// chunk (an unsharded chunk is a contiguous run of the file), flushed to disk and renamed over `path`; on any failure it is
+// removed, so `path` holds either its earlier content or the complete new snapshot.
+int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
+  API_BEGIN
+  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
+  const std::string target(path);
+  std::string tmp = target + ".tmp.XXXXXX";
+  const int fd = mkstemp(&tmp[0]);
+  if (fd < 0) throw Error(B200PIR_E_BADARG, "cannot create a temporary file next to " + target + ": " + std::strerror(errno));
+  FILE* f = fdopen(fd, "wb");
+  if (!f) close(fd);
+  // drop the temporary file and report `why`: `path` is left as it was
+  auto discard = [&](const std::string& why, int code) {
+    if (f) fclose(f);
+    f = nullptr;
+    unlink(tmp.c_str());
+    throw Error(code, code == B200PIR_E_BADARG ? "cannot write " + target + ": " + why : why);
+  };
+  if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
+  try {
+    export_impl(c, db, 0, c->slices, [&](int, int, int zc, const uint64_t* src) {
+      const size_t n = (size_t)zc * db->rows * c->dim0;
+      if (fwrite(src, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
+    });
+  } catch (const Error& e) {
+    discard(e.what(), e.code);
+  } catch (const std::exception& e) {
+    discard(e.what(), B200PIR_E_CUDA);
+  }
+  if (fflush(f) != 0 || fsync(fileno(f)) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  const int closed = fclose(f);
+  f = nullptr;
+  if (closed != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  if (rename(tmp.c_str(), target.c_str()) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  // make the rename itself durable
+  const size_t slash = target.find_last_of('/');
+  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : target.substr(0, slash));
+  const int dfd = open(dir.c_str(), O_RDONLY);
+  if (dfd >= 0) { fsync(dfd); close(dfd); }
+  API_END
 }
 int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
   API_BEGIN

@@ -86,7 +86,7 @@ __global__ void k_db_upsert_frag(ImmaGeom F, uint4* dbf, int slice, int il, int 
   int z = blockIdx.x * blockDim.x + threadIdx.x;
   if (z >= POLY) return;
   const uint64_t w = poly[z];
-  place_frag(F, dbf, slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
+  place_frag(F, reinterpret_cast<uint8_t*>(dbf), slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
 }
 
 // expanded queries (format of mul_kernels.cu: uint4 [jp][jb][z]) -> B fragments

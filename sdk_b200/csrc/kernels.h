@@ -8,11 +8,9 @@
 //   matrices   : row-major [row][col] of polys, as PolyMatrixRaw / PolyMatrixNTT (poly.rs:59-71)
 #pragma once
 #include "common.cuh"
-#include "tc5_layout.cuh"
+#include "item_place.cuh"    // POLY, MulGeom, ImmaGeom and where an item lives in each layout
 
 namespace b200pir {
-
-static const int POLY = 2048;
 
 // number of kernels this library has launched from the calling thread (bench.py reports it)
 extern thread_local unsigned long long g_kernel_launches;
@@ -54,7 +52,6 @@ void launch_widen(uint64_t* out, const uint32_t* in, size_t words, cudaStream_t 
 void launch_narrow(uint32_t* out, const uint64_t* in, size_t words, cudaStream_t s);
 
 // ---- first dimension (K1): server.rs:155-221
-struct MulGeom { int dim0, num_per, slices; };
 // db_dev : uint4 [slice][ii][jp = j/2][z] = {w(2jp).lo, w(2jp).hi, w(2jp+1).lo, w(2jp+1).hi}
 // q_dev  : uint4 [jp][jb][z] = {a[j][r0].lo, a[j][r0].hi, a[j][r1].lo, a[j][r1].hi},  j = 2jp+jb
 // out    : ntt32 [slice][ii][r][n][z]
@@ -78,8 +75,6 @@ void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_d
                      int slice_begin, int slice_count, cudaStream_t s);
 
 // ---- first dimension on INT8 tensor cores (imma_kernels.cu): database in MMA fragment order
-struct ImmaGeom { int dim0, rows, mt /* ceil(rows/16) */, ks /* ceil(dim0/32) */; };
-inline ImmaGeom make_imma_geom(int dim0, int rows) { return ImmaGeom{dim0, rows, (rows + 15) / 16, (dim0 + 31) / 32}; }
 size_t imma_db_cells(const ImmaGeom& F, int slices);      // uint4 cells of the whole database
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
 bool imma_supports_16(const ImmaGeom& F);                 // 16 queries per database pass fit one CTA's shared memory
@@ -128,6 +123,9 @@ struct ItemWrite { uint32_t off, len, il, j; };
 // (recenter_mod, NTT, pack: loading.rs:278-299, 34-41) and placed at the item's cell of slice c.  One launch.
 void launch_write_items(const DevParams& P, const DbDst& D, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
                         int bpc, uint64_t pt_modulus, cudaStream_t s);
+// ---- database export (export_kernels.cu), the inverse of the loaders: the local rows of slice `slice` at z in [z0, z0 + zc) ->
+// out u64 [zc][rows][dim0] (the reference layout [z][ii][j] restricted to this GPU's rows), words lo | hi << 32.  One launch.
+void launch_db_export(const DbDst& D, int slice, int z0, int zc, uint64_t* out, cudaStream_t s);
 
 // ---- second dimension
 // mult output ntt32 [cnt][r][n][z] -> raw ciphertexts u64 [cnt][r][z]   (server.rs:707-709)

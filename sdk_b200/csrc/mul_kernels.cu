@@ -159,7 +159,7 @@ __global__ void k_db_upsert(MulGeom G, uint4* db, int slice, int ii, int j, cons
   int z = blockIdx.x * blockDim.x + threadIdx.x;
   if (z >= POLY) return;
   const uint64_t w = poly[z];
-  place_imad(G, db, slice, ii, j, z, (uint32_t)w, (uint32_t)(w >> 32));
+  place_imad(G, reinterpret_cast<uint32_t*>(db), slice, ii, j, z, (uint32_t)w, (uint32_t)(w >> 32));
 }
 
 __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index) {
@@ -235,9 +235,9 @@ k_write_items(DevParams P, DbDst D, const uint8_t* __restrict__ bytes, const Ite
   const int il = (int)it.il, j = (int)it.j;
   for (int z = threadIdx.x; z < POLY; z += 512) {
     const uint32_t lo = halves[0][z], hi = halves[1][z];
-    if (D.format == 0) place_imad(D.G, D.d, slice, il, j, z, lo, hi);
+    if (D.format == 0) place_imad(D.G, reinterpret_cast<uint32_t*>(D.d), slice, il, j, z, lo, hi);
     else if (D.format == 2) place_tc5(D.T, D.t, slice, il, j, z, lo, hi);
-    else place_frag(D.F, D.f, slice, il, j, z, lo, hi);
+    else place_frag(D.F, reinterpret_cast<uint8_t*>(D.f), slice, il, j, z, lo, hi);
   }
 }
 

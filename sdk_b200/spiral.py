@@ -171,6 +171,34 @@ class Database:
         check(LIB.b200pir_db_update_many_items(self.params._h, self._h, body.ctypes.data, body.size, C.byref(largest)))
         return largest.value
 
+    def download_slice(self, slice_idx, out=None):
+        """The inverse of upload_slice: slice `slice_idx` in the reference layout [z][ii][j].  With `out`, only this shard's rows
+        are written (the other words are left as they are) and `out` is returned."""
+        P = self.params
+        words = P.dim0 * P.num_per * POLY_LEN
+        if out is None:
+            out = np.zeros(words, dtype=np.uint64)
+        _need(out, words, "out")
+        check(LIB.b200pir_db_download_slice(P._h, self._h, slice_idx, _ptr(out), out.size))
+        return out
+
+    def to_words(self, out=None):
+        """The flat uint64 array from_words takes ([instance][trial][z][ii][j]), read back from HBM.  With `out`, only this
+        shard's rows are written (the other words are left as they are, so every shard downloading into one array assembles
+        the whole database) and `out` is returned.  Formats 1 and 2 return the low 28 bits of each 32-bit half."""
+        P = self.params
+        words = P.slices * P.dim0 * P.num_per * POLY_LEN
+        if out is None:
+            out = np.zeros(words, dtype=np.uint64)
+        _need(out, words, "out")
+        check(LIB.b200pir_db_download(P._h, self._h, _ptr(out), out.size))
+        return out
+
+    def save_file(self, path):
+        """Write the file from_file (load_preprocessed_db_from_file) reads, atomically (temporary file, fsync, rename).
+        Unsharded databases only."""
+        check(LIB.b200pir_db_save_file(self.params._h, self._h, str(path).encode()))
+
     def fill_synthetic(self, seed):
         check(LIB.b200pir_db_fill_synthetic(self.params._h, self._h, seed))
 
