@@ -6,6 +6,7 @@
 #include "kernels.h"
 #include "ntt_tables.hpp"
 #include "update_body.hpp"
+#include "gadget.hpp"
 #include <cstdio>
 #include <cerrno>
 #include <fcntl.h>
@@ -47,10 +48,8 @@ thread_local std::string g_last_error;
 using b200pir::tables::build_tables;
 using b200pir::tables::invmod;
 uint64_t log2_ceil_u64(uint64_t a) { return (uint64_t)std::ceil(std::log2((double)a)); }
-int bits_per(int t) {                        // gadget.rs:3-9 with modulus_log2 = 56
-  if (t == 56) return 1;
-  return 56 / t + 1;
-}
+using b200pir::bits_per;
+using b200pir::live_digits;
 const uint64_t kQ2Values[37] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 12289ULL, 12289ULL, 61441ULL, 65537ULL,
                                 65537ULL, 520193ULL, 786433ULL, 786433ULL, 3604481ULL, 7340033ULL, 16515073ULL,
                                 33292289ULL, 67043329ULL, 132120577ULL, 268369921ULL, 469762049ULL, 1073479681ULL,
@@ -88,6 +87,7 @@ struct b200pir_ctx {
   // derived (params.rs:116-200)
   int dim0, num_per, slices, trials, g, stop_round, num_packing;
   int bits_gsw, bits_conv, bits_left, bits_right;
+  int live_gsw, live_conv, live_left, live_right;     // live_digits() of each gadget
   bool has_right;
   uint64_t q2, q1, setup_bytes, query_bytes, response_bytes;
   int q1_bits;
@@ -393,16 +393,16 @@ void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size
     R.r = r; R.num_in = num_in; R.stop_round = stop_round; R.max_bits_to_gen_right = max_right;
     R.fill_skipped = all_slots ? 1 : 0;
     R.t_auto = (POLY >> r) + 1;
-    R.t_left = (int)hp.t_exp_left; R.bits_left = c->bits_left;
+    R.t_left = (int)hp.t_exp_left; R.bits_left = c->bits_left; R.live_left = c->live_left;
     R.tab_left = T.left; R.off_left = (size_t)r * 2 * hp.t_exp_left * 2 * POLY;
     if (hp.nu_2 > 0 && c->has_right) {
       // v_w_right has stop_round+1 matrices; rounds beyond that never take the right branch for a
       // processed (even) index except r == 0 (server.rs:60-73), so clamp the pointer for safety.
       int rr = r <= c->stop_round ? r : c->stop_round;
-      R.t_right = (int)hp.t_exp_right; R.bits_right = c->bits_right;
+      R.t_right = (int)hp.t_exp_right; R.bits_right = c->bits_right; R.live_right = c->live_right;
       R.tab_right = T.right; R.off_right = (size_t)rr * 2 * hp.t_exp_right * 2 * POLY;
     } else {
-      R.t_right = R.t_left; R.bits_right = R.bits_left; R.tab_right = T.left; R.off_right = R.off_left;   // unwrap_or(v_w_left), server.rs:549
+      R.t_right = R.t_left; R.bits_right = R.bits_left; R.live_right = R.live_left; R.tab_right = T.left; R.off_right = R.off_left;   // unwrap_or(v_w_left), server.rs:549
     }
     if (pair && c->expand_variant == 0) {
       const size_t xr_stride = (size_t)num_in * 2 * POLY;
@@ -434,7 +434,7 @@ void run_expand_query(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_raw,
   }
   if (hp.nu_2 > 0)
     launch_regev_to_gsw(c->dp, v_fold, c->fold_words(), v, c->v_words(), nq, (int)hp.nu_2, 2, 1, c->pp_table(pp, (size_t)nq).conv,
-                        (int)hp.t_gsw, (int)hp.t_conv, c->bits_conv, s);
+                        (int)hp.t_gsw, (int)hp.t_conv, c->bits_conv, c->live_conv, s);
 }
 
 // fold `num` ciphertexts per batch entry with matrices k = k0, k0-1, ...
@@ -463,7 +463,7 @@ const uint32_t* run_fold_res(b200pir_ctx* c, uint32_t* a, uint32_t* b, size_t ba
   }
   for (size_t half = num / 2; half >= 1; half /= 2, k--) {
     launch_fold_res(c->dp, src, dst, batch, batch_stride, (int)half, vfold + (size_t)k * mat, c->fold_words(),
-                    slices_per_query, (int)c->hp.t_gsw, c->bits_gsw, zero_flags, c->stream);
+                    slices_per_query, (int)c->hp.t_gsw, c->bits_gsw, c->live_gsw, zero_flags, c->stream);
     std::swap(src, dst);
   }
   return src;
@@ -567,7 +567,7 @@ void run_pack_encode(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* folded, siz
   {
     b200pir_ctx::Scope sc(c, ST_PACK);
     launch_pack(c->dp, c->w_packed.p, packed_words, folded, ct_stride, (size_t)c->slices * ct_stride, (int)count, c->pp_table(pp, count).pack,
-                (int)hp.n, (int)hp.instances, (int)hp.t_conv, c->bits_conv, (int)hp.version, c->stream);
+                (int)hp.n, (int)hp.instances, (int)hp.t_conv, c->bits_conv, c->live_conv, (int)hp.version, c->stream);
   }
   {
     b200pir_ctx::Scope sc(c, ST_ENCODE);
@@ -641,6 +641,10 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   c->bits_conv = bits_per((int)hp.t_conv);
   c->bits_left = bits_per((int)hp.t_exp_left);
   c->bits_right = bits_per((int)hp.t_exp_right);
+  c->live_gsw = live_digits((int)hp.t_gsw);
+  c->live_conv = live_digits((int)hp.t_conv);
+  c->live_left = live_digits((int)hp.t_exp_left);
+  c->live_right = live_digits((int)hp.t_exp_right);
   c->q2 = kQ2Values[hp.q2_bits];
   c->q1 = 4 * hp.p;
   c->q1_bits = (int)log2_ceil_u64(c->q1);
@@ -1512,7 +1516,7 @@ int b200pir_fold_ciphertexts(b200pir_ctx* c, uint64_t* v_cts, size_t num, const 
     int k = dims - 1;
     for (size_t half = num / 2; half >= 1; half /= 2, k--) {
       launch_fold_res(c->dp, a.p, b.p, 1, num * 4 * POLY, (int)half, vf.p + (size_t)k * mat, c->fold_words(), 1,
-                      (int)c->hp.t_gsw, c->bits_gsw, zflags.p, c->stream);
+                      (int)c->hp.t_gsw, c->bits_gsw, c->live_gsw, zflags.p, c->stream);
       B200_CUDA(cudaMemcpyAsync(a.p, b.p, half * 4 * POLY * 4, cudaMemcpyDeviceToDevice, c->stream));
     }
     launch_res_to_raw(c->dp, cts.p, a.p, num * 2, c->stream);
@@ -1602,7 +1606,7 @@ int b200pir_pack(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* v_ct, uint64_t*
   DevBuf<uint32_t> o(outp * 2 * POLY), res(nn * 4 * POLY);
   B200_CUDA(cudaMemcpyAsync(cts.p, v_ct, cts.n * 8, cudaMemcpyHostToDevice, c->stream));
   launch_raw_to_res(c->dp, res.p, cts.p, nn * 2, c->stream);
-  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, c->pp_table(pp, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, (int)hp.version, c->stream,
+  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, c->pp_table(pp, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, c->live_conv, (int)hp.version, c->stream,
               cts.p);
   // the reference's pack returns the NTT-form matrix (server.rs:467); the kernel already applied .raw()
   launch_to_ntt(c->dp, o.p, raw.p, outp, c->stream);

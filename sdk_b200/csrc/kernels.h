@@ -132,13 +132,15 @@ void launch_db_export(const DbDst& D, int slice, int z0, int zc, uint64_t* out, 
 // (== launch_from_ntt with 2*cnt polys)
 // fold (server.rs:388-427): one launch per round.  cts: raw [batch][num][2][2048] (in place);
 // step (b,i) : ct[i] <- from_ntt(Cneg * G^-1(ct[i]) + C * G^-1(ct[half+i]))
+// The words come from the caller unchecked and may exceed q, so all t_gsw digits are decomposed (at bits_per = 8 the byte
+// path reads bits 56..63 as zero, as it always has).
 void launch_fold_round(const DevParams& P, uint64_t* cts, size_t batch, size_t batch_stride /*u64 words*/, int half,
                        const uint32_t* c_pos, const uint32_t* c_neg, size_t c_batch_stride /*u32 words, per query*/,
                        int slices_per_query, int t_gsw, int bits, cudaStream_t s);
 // Fast path on residue-form ciphertexts u32 [batch][num][row][n][z] (see k_fold_res): out[i] (i < half) from
-// in[i], in[half+i]; in != out.  Needs only v_folding (c_pos).
+// in[i], in[half+i]; in != out.  Needs only v_folding (c_pos).  The CRT-composed inputs are < q: live = live_digits(t_gsw).
 void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size_t batch, size_t batch_stride /*u32*/,
-                     int half, const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
+                     int half, const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits, int live,
                      uint32_t* zero_flags /* null = dense semantics (spiral-rs); else scratch of batch*2*half words: lib/server fold.rs:37-43 */, cudaStream_t s);
 // server.rs:505-523 get_v_folding_neg, computed pointwise: neg = (q_n - C) + G  (NTT is linear and the
 // gadget matrix is constant-coefficient, so this is the same canonical value)
@@ -159,6 +161,7 @@ struct ExpandRound {
   const uint32_t* const* tab_right;   // starts off_left / off_right words further
   size_t off_left, off_right;
   int t_left, t_right, bits_left, bits_right;
+  int live_left, live_right;   // live_digits(t_left / t_right): the automorphed coefficients are <= q
   int fill_skipped;         // paired kernel: also write v[i + num_in] = v[i] (.) neg1 for skipped i (stage-level parity)
 };
 void launch_expand_round(const DevParams& P, uint32_t* v, size_t v_stride, int nq, const ExpandRound& R, cudaStream_t s);
@@ -174,17 +177,19 @@ void launch_reorient(const MulGeom& G, uint4* q_dev, size_t q_stride, const uint
 // server.rs:123-151: v_gsw[i] (ntt32 [2][2 t_gsw]) from v_inp[idx_factor*(i t_gsw + j) + idx_offset]
 void launch_regev_to_gsw(const DevParams& P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* v, size_t v_stride,
                          int nq, int count, int idx_factor, int idx_offset, const uint32_t* const* tab_conv, int t_gsw,
-                         int t_conv, int bits_conv, cudaStream_t s);
+                         int t_conv, int bits_conv, int live_conv, cudaStream_t s);
 
 // ---- packing + encoding (server.rs:429-503; lib/server compute/pack.rs)
 // folded: residue-form ciphertexts, ct (inst, t) at folded + (inst*n*n + t)*ct_stride (u32 words);
 // w: ntt32 packing matrices; out: raw [inst][n+1][n][2048]
 // nq queries per launch: query k reads folded + k*in_q_stride and writes out_raw + k*out_q_stride
 // raw_cts (optional, nq = 1): the same ciphertexts as raw u64 [inst][n*n][2][2048]; row 0 is then decomposed from these values,
-// so a coefficient q (which the residue form stores as 0) yields q's gadget digits, as the reference's pack does
+// so a coefficient q (which the residue form stores as 0) yields q's gadget digits, as the reference's pack does.  Those words
+// are the caller's, unchecked, so they are decomposed into all t_conv digits (at bits_per = 8 the byte path reads bits 56..63
+// as zero, as it always has); CRT-composed rows take the live_conv ones.
 void launch_pack(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride,
                  size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int n, int instances, int t_conv, int bits_conv,
-                 int version, cudaStream_t s, const uint64_t* raw_cts = nullptr);
+                 int live_conv, int version, cudaStream_t s, const uint64_t* raw_cts = nullptr);
 // out: nq x out_bytes; packed_raw: nq matrices packed_q_stride words apart
 void launch_encode(const DevParams& P, uint8_t* out, size_t out_bytes, const uint64_t* packed_raw, size_t packed_q_stride,
                    int nq, int n, int instances, uint64_t q2, int q2_bits, uint64_t q1, int q1_bits, cudaStream_t s);

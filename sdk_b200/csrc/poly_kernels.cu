@@ -165,9 +165,28 @@ struct SmemCoef {
   __device__ __forceinline__ uint64_t operator()(int a) const { return p[a * 256]; }
 };
 
+// acc[r][.] += C[r][this column] (.) x for one transformed digit polynomial x; c = row 0 of the column, offset by tid*8
+template <int ROWS>
+__device__ __forceinline__ void mac_digit(uint64_t (&acc)[ROWS][8], const uint32_t (&x)[8], const uint32_t* c, size_t row_step) {
+#pragma unroll
+  for (int r = 0; r < ROWS; r++) {
+    uint32_t cv[8];
+    ld8_ro(cv, c + (size_t)r * row_step);
+#pragma unroll
+    for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x[e] * cv[e];
+  }
+}
+// make room for n more products in every accumulator (16 at most between reductions)
+template <int ROWS>
+__device__ __forceinline__ void acc_room(uint64_t (&acc)[ROWS][8], int& cnt, int n, const Grp& g) {
+  if (cnt + n > 16) { acc_reduce<ROWS>(acc, g); cnt = 1; }
+  cnt += n;
+}
+
 // acc[r][.] += sum_k  C[r][col0 + k*col_step] (.) NTT(digit_k(v))     (pointwise, this group's modulus)
 // v = coefficient source (RegCoef / SmemCoef).  c0 points at element (row 0, first
 // column) of this group's modulus, offset by tid*8.  `cnt` counts products held per accumulator.
+// ndig = the digits decomposed: live_digits(t) (gadget.hpp) when every value is <= q, t otherwise.
 // Relaxed-range forward transforms (ntt_core.cuh "lz"): digits are < 2^19 < 2q (gadget dimensions >= 3), the outputs
 // (< 16q < 2^32) go straight into the 64-bit accumulators: products < 2^60, at most 16 per accumulator between reductions.
 template <int ROWS, bool SM, bool BYTE, typename Coef>
@@ -189,24 +208,11 @@ __device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& c
         x1[a] = gadget_digit_fast<BYTE>(va, k + 1, bits, mask);
       }
       ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x0, x1, g.smem, g.smem2, TwConst{g.n, 0}, TwShared{g.fwd_hi_sm}, g.q, CtaSync());
-      if (cnt + 2 > 16) { acc_reduce<ROWS>(acc, g); cnt = 1; }
-      cnt += 2;
+      acc_room<ROWS>(acc, cnt, 2, g);
       const uint32_t* c = c0 + (size_t)k * col_step;
       // digit-major: x0 is dead before x1's key columns arrive
-#pragma unroll
-      for (int r = 0; r < ROWS; r++) {
-        uint32_t cv[8];
-        ld8_ro(cv, c + (size_t)r * row_step);
-#pragma unroll
-        for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x0[e] * cv[e];
-      }
-#pragma unroll
-      for (int r = 0; r < ROWS; r++) {
-        uint32_t cv[8];
-        ld8_ro(cv, c + col_step + (size_t)r * row_step);
-#pragma unroll
-        for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x1[e] * cv[e];
-      }
+      mac_digit<ROWS>(acc, x0, c, row_step);
+      mac_digit<ROWS>(acc, x1, c + col_step, row_step);
     }
   }
 #pragma unroll 1
@@ -216,16 +222,8 @@ __device__ __forceinline__ void digits_mac_impl(uint64_t (&acc)[ROWS][8], int& c
     for (int a = 0; a < 8; a++) x[a] = gadget_digit_fast<BYTE>(v(a), k, bits, mask);
     if (SM) ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x, g.smem, TwConst{g.n, 0}, TwShared{g.fwd_hi_sm}, g.q, CtaSync());
     else ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x, g.smem, TwConst{g.n, 0}, TwGlobal{g.fwd}, g.q, CtaSync());
-    if (cnt + 1 > 16) { acc_reduce<ROWS>(acc, g); cnt = 1; }
-    cnt += 1;
-    const uint32_t* c = c0 + (size_t)k * col_step;
-#pragma unroll
-    for (int r = 0; r < ROWS; r++) {
-      uint32_t cv[8];
-      ld8_ro(cv, c + (size_t)r * row_step);
-#pragma unroll
-      for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x[e] * cv[e];
-    }
+    acc_room<ROWS>(acc, cnt, 1, g);
+    mac_digit<ROWS>(acc, x, c0 + (size_t)k * col_step, row_step);
   }
 }
 
@@ -423,7 +421,7 @@ k_fold_round(DevParams P, uint64_t* cts, size_t batch_stride, int half, const ui
 // because v_folding_neg[k] = G - C_k (server.rs:505-523), G . G^-1(x) = x and the NTT is linear over
 // Z_{q_n}; canonical representatives are unique, so the bytes agree.  It needs half the forward
 // transforms, no CRT lift on the way out, and no v_folding_neg at all.
-// grid = (batch*half, 2 moduli), 256 threads.  in/out are distinct buffers (ping-pong): the CTA of
+// grid = (2 moduli, half, batch), 256 threads.  in/out are distinct buffers (ping-pong): the CTA of
 // modulus n reads BOTH residues of its inputs (for the gadget digits) while the other CTA writes.
 // Digit k of vh minus digit k of vi, offset by q: in (q - 2^bits, q + 2^bits), a subset of [0, 2q) for bits <= 27 (the
 // context rejects gadget dimensions below 3, so bits <= 19) — the relaxed-range forward transform needs no more.
@@ -438,34 +436,41 @@ __device__ __forceinline__ uint32_t byte_pair_diff(uint64_t vh, uint64_t vi, int
   return __byte_perm((uint32_t)vh, (uint32_t)(vh >> 32), sel) + 0x01000100u -
          __byte_perm((uint32_t)vi, (uint32_t)(vi >> 32), sel);
 }
-constexpr int kFoldPlanes = 4;   // byte-pair planes of the bits == 8 path: gadget dimensions up to 8
+constexpr int kFoldPlanes = 3;   // byte-pair planes of the bits == 8 path: the 3 full digit pairs of t = 8's 7 live digits
 
 // Same step as k_fold_res on the relaxed-range transforms (ntt_core.cuh "lz"): no per-butterfly range correction in the
 // forward transforms (outputs < 16q feed the 64-bit multiply-accumulate directly: 16 products of < 2^32 x < 2^28 fit),
 // no halving in the inverse transform, 32-bit Barrett in the CRT lift.
-// BYTE (bits == 8, gadget dimension <= 8): the digit differences of both inputs are formed once per row and parked in
-// shared memory as byte-pair planes (32 KiB), one word per digit pair and coefficient, written and read by the same thread.
+// Only the live digits (gadget.hpp) are transformed: the inputs are CRT-composed, < q.  A skipped digit's difference would be
+// the constant q, whose transform is a multiple of q_n, so the canonical sums are unchanged.
+// BYTE (bits == 8, gadget dimension 8): the digit differences of both inputs are formed once per row and parked in
+// shared memory as byte-pair planes (24 KiB), one word per digit pair and coefficient, written and read by the same thread.
 // Only the accumulators then stay live across the digit loop.  Held in registers, the CRT-composed inputs (32 registers)
 // pushed the loop body into local memory, which shares the L1/shared-memory data path with the transforms' exchanges.
 // Other gadget widths keep them in registers.
+// With an odd live count the last live digit of each row is parked in `spare` (8 KiB per row, digit differences offset by q)
+// and the two go through one paired transform after both rows (on H100 no faster or slower than a lone transform per row,
+// within the run-to-run spread; DESIGN §4.3).
 // 2 CTAs per SM (up to 128 registers): the byte path compiles without spills there.  At 3 CTAs per SM (80 registers) it
 // still spills in the multiply-accumulate and measured slower on H100 (S8, 16 queries: fold 5.22 against 5.12 ms per step).
 template <bool BYTE>
 __global__ void __launch_bounds__(256, 2)
 k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict__ out, size_t batch_stride, int half,
-              const uint32_t* __restrict__ c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
+              const uint32_t* __restrict__ c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits, int live,
               const uint32_t* __restrict__ zero_flags /* null, or [batch][2*half]: 1 = ciphertext is all zero */) {
+  // grid (modulus, i, b): the two CTAs of a step read the same inputs (both residues of both ciphertexts) and run side by
+  // side, so the second one finds them in L2
+  const int n = blockIdx.x, i = blockIdx.y, b = blockIdx.z;
   if (zero_flags) {            // lib/server/src/compute/fold.rs:37-43, see k_fold_res
-    const int bz = blockIdx.x / half, iz = blockIdx.x % half;
-    const uint32_t fa = zero_flags[(size_t)bz * 2 * half + iz], fb = zero_flags[(size_t)bz * 2 * half + half + iz];
+    const uint32_t fa = zero_flags[(size_t)b * 2 * half + i], fb = zero_flags[(size_t)b * 2 * half + half + i];
     if (fa | fb) {
-      const uint32_t* src = in + (size_t)bz * batch_stride + (size_t)((fa ? half : 0) + iz) * 4 * POLY;
-      uint32_t* dst = out + (size_t)bz * batch_stride + (size_t)iz * 4 * POLY;
+      const uint32_t* src = in + (size_t)b * batch_stride + (size_t)((fa ? half : 0) + i) * 4 * POLY;
+      uint32_t* dst = out + (size_t)b * batch_stride + (size_t)i * 4 * POLY;
 #pragma unroll
       for (int rho = 0; rho < 2; rho++) {
         uint32_t x[8];
-        ld8_ro(x, src + ((size_t)rho * 2 + blockIdx.y) * POLY + threadIdx.x * 8);
-        st8(dst + ((size_t)rho * 2 + blockIdx.y) * POLY + threadIdx.x * 8, x);
+        ld8_ro(x, src + ((size_t)rho * 2 + n) * POLY + threadIdx.x * 8);
+        st8(dst + ((size_t)rho * 2 + n) * POLY + threadIdx.x * 8, x);
       }
       return;
     }
@@ -474,11 +479,10 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
   uint32_t* sm0 = reinterpret_cast<uint32_t*>(dyn_smem);
   uint32_t* sm1 = sm0 + NTT_SMEM_WORDS;
   Twiddle* tw = reinterpret_cast<Twiddle*>(sm1 + NTT_SMEM_WORDS);
-  Grp g = make_grp_single(P, sm0, blockIdx.y);
+  Grp g = make_grp_single(P, sm0, n);
   stage_fwd_twiddles(g, tw);
   const TwConst lo{g.n, 0};
   const TwShared hi{tw};
-  const int b = blockIdx.x / half, i = blockIdx.x % half;
   const uint32_t* ci = in + (size_t)b * batch_stride + (size_t)i * 4 * POLY;
   const uint32_t* ch = in + (size_t)b * batch_stride + (size_t)(half + i) * 4 * POLY;
   const uint32_t* C = c_pos + (size_t)(b / slices_per_query) * c_batch_stride;
@@ -487,6 +491,8 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
   const uint64_t mask = (1ull << bits) - 1;
   const uint32_t q = g.q;
   uint32_t* planes = reinterpret_cast<uint32_t*>(tw + HI_TW) + g.tid;   // BYTE: [kFoldPlanes][POLY], this thread's column
+  uint32_t* spare = planes + (BYTE ? kFoldPlanes : 0) * POLY;           // [row][POLY], this thread's column
+  const uint32_t* cb = C + (size_t)g.n * POLY + g.tid * 8;            // key-matrix column 0 of this modulus
 
   uint64_t acc[2][8];
 #pragma unroll
@@ -505,13 +511,13 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
       if (BYTE) {
 #pragma unroll
         for (int p = 0; p < kFoldPlanes; p++)
-          if (2 * p < t_gsw) planes[p * POLY + a * 256] = byte_pair_diff(vh[a], vi[a], 2 * p);
+          if (2 * p + 1 < live) planes[p * POLY + a * 256] = byte_pair_diff(vh[a], vi[a], 2 * p);
       }
+      if (live & 1) spare[rho * POLY + a * 256] = digit_diff(vh[a], vi[a], live - 1, bits, mask, q);
     }
-    const uint32_t* c0 = C + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8;       // key-matrix column of digit k: rho + 2k
-    int k = 0;
+    const uint32_t* c0 = cb + (size_t)rho * 2 * POLY;       // key-matrix column of digit k: rho + 2k
 #pragma unroll 1
-    for (; k + 1 < t_gsw; k += 2) {
+    for (int k = 0; k + 1 < live; k += 2) {
       uint32_t x0[8], x1[8];
 #pragma unroll
       for (int a = 0; a < 8; a++) {
@@ -525,40 +531,24 @@ k_fold_res_lz(DevParams P, const uint32_t* __restrict__ in, uint32_t* __restrict
         }
       }
       ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x0, x1, sm0, sm1, lo, hi, q, CtaSync());
-      if (cnt + 2 > 16) { acc_reduce<2>(acc, g); cnt = 1; }
-      cnt += 2;
+      acc_room<2>(acc, cnt, 2, g);
       // digit-major: x0 is dead before x1's key columns arrive
-#pragma unroll
-      for (int r = 0; r < 2; r++) {
-        uint32_t cv[8];
-        ld8_ro(cv, c0 + (size_t)r * row_step + (size_t)k * 4 * POLY);
-#pragma unroll
-        for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x0[e] * cv[e];
-      }
-#pragma unroll
-      for (int r = 0; r < 2; r++) {
-        uint32_t cv[8];
-        ld8_ro(cv, c0 + (size_t)r * row_step + (size_t)(k + 1) * 4 * POLY);
-#pragma unroll
-        for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x1[e] * cv[e];
-      }
+      mac_digit<2>(acc, x0, c0 + (size_t)k * 4 * POLY, row_step);
+      mac_digit<2>(acc, x1, c0 + (size_t)(k + 1) * 4 * POLY, row_step);
     }
-    if (k < t_gsw) {                            // odd t_gsw: last digit alone
-      uint32_t x0[8];
+  }
+  if (live & 1) {                               // digit live - 1 of row 0 (column 2k) and of row 1 (column 2k + 1)
+    const int k = live - 1;
+    uint32_t x0[8], x1[8];
 #pragma unroll
-      for (int a = 0; a < 8; a++)
-        x0[a] = BYTE ? (planes[(k >> 1) * POLY + a * 256] & 0xffffu) + (q - 256u) : digit_diff(vh[a], vi[a], k, bits, mask, q);
-      ntt_forward_group_lz<NTT_OUT_LAZY16>(g.tid, x0, sm0, lo, hi, q, CtaSync());
-      if (cnt + 1 > 16) { acc_reduce<2>(acc, g); cnt = 1; }
-      cnt += 1;
-#pragma unroll
-      for (int r = 0; r < 2; r++) {
-        uint32_t cv[8];
-        ld8_ro(cv, c0 + (size_t)r * row_step + (size_t)k * 4 * POLY);
-#pragma unroll
-        for (int e = 0; e < 8; e++) acc[r][e] += (uint64_t)x0[e] * cv[e];
-      }
+    for (int a = 0; a < 8; a++) {
+      x0[a] = spare[a * 256];
+      x1[a] = spare[POLY + a * 256];
     }
+    ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x0, x1, sm0, sm1, lo, hi, q, CtaSync());
+    acc_room<2>(acc, cnt, 2, g);
+    mac_digit<2>(acc, x0, cb + (size_t)k * 4 * POLY, row_step);
+    mac_digit<2>(acc, x1, cb + (size_t)k * 4 * POLY + 2 * POLY, row_step);
   }
   uint32_t y0[8], y1[8];
 #pragma unroll
@@ -645,6 +635,7 @@ __global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* 
   const uint32_t* W = left ? R.tab_left[blockIdx.y] + R.off_left : R.tab_right[blockIdx.y] + R.off_right;
   const int t_exp = left ? R.t_left : R.t_right;
   const int bits = left ? R.bits_left : R.bits_right;
+  const int live = left ? R.live_left : R.live_right;
 
   stage_fwd_twiddles(g, tw + g.n * HI_TW);
   uint32_t* vi = v + (size_t)i * 4 * POLY;
@@ -669,7 +660,7 @@ __global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* 
     for (int e = 0; e < 8; e++) acc[r][e] = 0;
   int cnt = 0;
   // gadget_invert_rdim(.., rdim = 1): digit k -> key column k  (server.rs:82-89)
-  digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
+  digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, live, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
                       (size_t)t_exp * 2 * POLY, g);
   // row 1: the reference computes to_ntt(automorph(from_ntt(row 1))) (server.rs:80-88).  X -> X^t permutes the
   // roots of X^N + 1, so in the NTT domain the automorphism is a pure permutation of the evaluation slots:
@@ -748,6 +739,7 @@ k_expand_round_pair(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R, co
   const uint32_t* W = left ? R.tab_left[blockIdx.y] + R.off_left : R.tab_right[blockIdx.y] + R.off_right;
   const int t_exp = left ? R.t_left : R.t_right;
   const int bits = left ? R.bits_left : R.bits_right;
+  const int live = left ? R.live_left : R.live_right;
 
   stage_fwd_twiddles(g, tw + g.n * HI_TW);
   uint32_t* vi = v + (size_t)i * 4 * POLY;
@@ -801,7 +793,7 @@ k_expand_round_pair(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R, co
 #pragma unroll
       for (int e = 0; e < 8; e++) acc[r][e] = 0;
     int cnt = 0;
-    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
+    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, live, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
                         (size_t)t_exp * 2 * POLY, g);
     uint32_t* dst = half ? vo : vi;
 #pragma unroll
@@ -858,6 +850,9 @@ k_expand_intt(DevParams P, const uint32_t* __restrict__ v, size_t v_stride, uint
 
 // 2 CTAs per SM (up to 128 registers): compiles without spills; at 3 CTAs per SM (80 registers) it spilled and measured
 // slower on H100 (S8, 16 queries, every round paired: expansion 3.58 against 3.61 ms per step).
+// Both halves' automorphed coefficients are formed up front (autom[half], 2 x 16 KiB), so that with an odd live count the last
+// live digit of both halves goes through one paired transform at the end of half 1; half 0's transformed digit waits in
+// `carry` (8 registers) and starts half 0's accumulators.
 __global__ void __launch_bounds__(256, 2)
 k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __restrict__ xr, size_t xr_stride,
                    ExpandRound R, const uint32_t* __restrict__ neg1) {
@@ -866,8 +861,8 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   uint32_t* sm0 = reinterpret_cast<uint32_t*>(dyn_smem);
   uint32_t* sm1 = sm0 + NTT_SMEM_WORDS;
-  uint64_t* autom = reinterpret_cast<uint64_t*>(sm1 + NTT_SMEM_WORDS);     // [2048]
-  Twiddle* tw = reinterpret_cast<Twiddle*>(autom + POLY);                   // [HI_TW]
+  uint64_t* autom = reinterpret_cast<uint64_t*>(sm1 + NTT_SMEM_WORDS);     // [half][2048]
+  Twiddle* tw = reinterpret_cast<Twiddle*>(autom + 2 * POLY);               // [HI_TW]
   Grp g = make_grp_single(P, sm0, blockIdx.y);
   g.smem2 = sm1;
   const int i = blockIdx.x;
@@ -894,6 +889,7 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
   const uint32_t* W = left ? R.tab_left[blockIdx.z] + R.off_left : R.tab_right[blockIdx.z] + R.off_right;
   const int t_exp = left ? R.t_left : R.t_right;
   const int bits = left ? R.bits_left : R.bits_right;
+  const int live = left ? R.live_left : R.live_right;
   stage_fwd_twiddles(g, tw);
   const uint32_t* x0r = xr + (size_t)i * 2 * POLY;         // residues mod q_0 / q_1 of from_ntt(row 0 of v[i])
   const uint32_t* x1r = x0r + POLY;
@@ -915,17 +911,39 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
       const uint64_t val = crt_compose(a0, a1, P);
       const unsigned prod = (unsigned)k * (unsigned)R.t_auto;
       const unsigned num = prod >> NTT_LOG_N, rem = prod & (POLY - 1);
-      autom[rem] = (num & 1u) ? Q - val : val;             // zero maps to q, as in the reference
+      autom[half * POLY + rem] = (num & 1u) ? Q - val : val;   // zero maps to q, as in the reference
     }
-    __syncthreads();                                       // autom complete (and the staged twiddles visible)
+  }
+  __syncthreads();                                         // autom complete (and the staged twiddles visible)
+  const uint32_t* Wn = W + (size_t)g.n * POLY + g.tid * 8;
+  const size_t row_step = (size_t)t_exp * 2 * POLY;
+  const int kl = live - 1;                                 // odd live: the digit the two halves transform together
+  uint32_t carry[8];
+#pragma unroll 1
+  for (int half = 1; half >= 0; half--) {
     uint64_t acc[2][8];
 #pragma unroll
     for (int r = 0; r < 2; r++)
 #pragma unroll
       for (int e = 0; e < 8; e++) acc[r][e] = 0;
     int cnt = 0;
-    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, t_exp, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
-                        (size_t)t_exp * 2 * POLY, g);
+    if (!half && (live & 1)) {
+      mac_digit<2>(acc, carry, Wn + (size_t)kl * 2 * POLY, row_step);
+      cnt = 1;
+    }
+    digits_mac<2, true>(acc, cnt, SmemCoef{autom + half * POLY + g.tid}, live & ~1, bits, Wn, (size_t)2 * POLY, row_step, g);
+    if (half && (live & 1)) {
+      const uint64_t mask = (1ull << bits) - 1;
+      uint32_t x[8];
+#pragma unroll
+      for (int a = 0; a < 8; a++) {
+        x[a] = gadget_digit(autom[POLY + a * 256 + g.tid], kl, bits, mask);
+        carry[a] = gadget_digit(autom[a * 256 + g.tid], kl, bits, mask);
+      }
+      ntt_forward_group2_lz<NTT_OUT_LAZY16>(g.tid, x, carry, sm0, sm1, TwConst{g.n, 0}, TwShared{tw}, g.q, CtaSync());
+      acc_room<2>(acc, cnt, 1, g);
+      mac_digit<2>(acc, x, Wn + (size_t)kl * 2 * POLY, row_step);
+    }
     // row 1 automorphism = slot permutation (see k_expand_round); gather before any thread overwrites v[i]
     uint32_t yy[8];
 #pragma unroll
@@ -973,7 +991,7 @@ __global__ void k_reorient(MulGeom G, uint4* q_dev, size_t q_stride, const uint3
 // server.rs:134-150.  CTA = (gsw index i, digit j).
 __global__ void __launch_bounds__(CTA, 1)
 k_regev_to_gsw(DevParams P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* v, size_t v_stride, int idx_factor,
-               int idx_offset, const uint32_t* const* tab_conv, int t_gsw, int t_conv, int bits_conv) {
+               int idx_offset, const uint32_t* const* tab_conv, int t_gsw, int t_conv, int bits_conv, int live_conv) {
   const uint32_t* v_conv = tab_conv[blockIdx.y];
   v_gsw += (size_t)blockIdx.y * gsw_stride;
   v += (size_t)blockIdx.y * v_stride;
@@ -1010,7 +1028,7 @@ k_regev_to_gsw(DevParams P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* 
 #pragma unroll 1
   for (int rho = 0; rho < 2; rho++) {
     const uint32_t* c0 = v_conv + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8;
-    digits_mac<2, true>(acc, cnt, SmemCoef{raw + rho * POLY + g.tid}, t_conv, bits_conv, c0, (size_t)2 * 2 * POLY, (size_t)ccols * 2 * POLY, g);
+    digits_mac<2, true>(acc, cnt, SmemCoef{raw + rho * POLY + g.tid}, live_conv, bits_conv, c0, (size_t)2 * 2 * POLY, (size_t)ccols * 2 * POLY, g);
   }
 #pragma unroll
   for (int r = 0; r < 2; r++) {
@@ -1025,7 +1043,7 @@ k_regev_to_gsw(DevParams P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* 
 template <int ROWS>
 __global__ void __launch_bounds__(CTA, 1)
 k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride, size_t in_q_stride,
-       const uint32_t* const* tab_pack, int t_conv, int bits, int version, const uint64_t* __restrict__ raw_cts) {
+       const uint32_t* const* tab_pack, int t_conv, int bits, int live, int version, const uint64_t* __restrict__ raw_cts) {
   const uint32_t* v_packing = tab_pack[blockIdx.y];
   out_raw += (size_t)blockIdx.y * out_q_stride;
   folded += (size_t)blockIdx.y * in_q_stride;
@@ -1069,7 +1087,10 @@ k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* fold
 #pragma unroll
         for (int a = 0; a < 8; a++) vv[a] = crt_compose(__ldg(ct + a * 256 + g.tid), __ldg(ct + POLY + a * 256 + g.tid), P);
       }
-      digits_mac<ROWS, true>(acc, cnt, RegCoef{vv}, t_conv, bits, W + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
+      // the caller's raw words are not checked against q: all t_conv digits (the bits == 8 byte path still reads bits
+      // 56..63 as zero, as it always has)
+      digits_mac<ROWS, true>(acc, cnt, RegCoef{vv}, raw_cts ? t_conv : live, bits, W + (size_t)g.n * POLY + g.tid * 8, col_step,
+                             row_step, g);
     }
     uint32_t y[8];
 #pragma unroll
@@ -1107,7 +1128,7 @@ k_pack(DevParams P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* fold
 #pragma unroll
           for (int e = 0; e < 8; e++) acc[m][e] = 0;
         cnt = 0;
-        digits_mac<ROWS, true>(acc, cnt, SmemCoef{rawbuf + g.tid}, t_conv, bits, Wshift + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
+        digits_mac<ROWS, true>(acc, cnt, SmemCoef{rawbuf + g.tid}, live, bits, Wshift + (size_t)g.n * POLY + g.tid * 8, col_step, row_step, g);
         uint32_t np[ROWS][8];
 #pragma unroll
         for (int m = 0; m < ROWS; m++)
@@ -1229,7 +1250,7 @@ void launch_res_to_raw(const DevParams& P, uint64_t* out, const uint32_t* res, s
   if (polys) ++g_kernel_launches, k_res_to_raw<<<grid1d(polys * POLY, 256), 256, 0, s>>>(P, out, res, polys);
 }
 void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size_t batch, size_t batch_stride, int half,
-                     const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits,
+                     const uint32_t* c_pos, size_t c_batch_stride, int slices_per_query, int t_gsw, int bits, int live,
                      uint32_t* zero_flags, cudaStream_t s) {
   if (batch == 0 || half == 0) return;
   if (zero_flags) {            // scratch of batch * 2 * half words: recomputed every round, as the reference re-tests every step
@@ -1237,12 +1258,16 @@ void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size
     k_ct_zero_flags<<<(unsigned)(batch * 2 * half), 256, 0, s>>>(in, batch_stride, 2 * half, zero_flags);
   }
   ++g_kernel_launches;
-  const dim3 grid((unsigned)(batch * half), 2);
-  const bool byte = bits == 8 && t_gsw <= 2 * kFoldPlanes;
-  const size_t smem = kDynSmemFold + (byte ? (size_t)kFoldPlanes * POLY * 4 : 0);
+  if (batch > 65535) throw Error(-2, "fold: more than 65535 ciphertext batches in one launch");
+  const dim3 grid(2, (unsigned)half, (unsigned)batch);
+  const bool byte = bits == 8 && live / 2 <= kFoldPlanes;
+  const size_t planes = (size_t)(byte ? kFoldPlanes : 0) * POLY * 4, spare = (size_t)2 * POLY * 4;
+  const size_t smem = kDynSmemFold + planes + ((live & 1) ? spare : 0);
   auto kern = byte ? k_fold_res_lz<true> : k_fold_res_lz<false>;
-  opt_in_smem(kern, (int)smem);
-  kern<<<grid, 256, smem, s>>>(P, in, out, batch_stride, half, c_pos, c_batch_stride, slices_per_query, t_gsw, bits, zero_flags);
+  // the opt-in is made once per kernel and device, so it covers the larger size: contexts with either live parity share it
+  opt_in_smem(kern, (int)(kDynSmemFold + planes + spare));
+  kern<<<grid, 256, smem, s>>>(P, in, out, batch_stride, half, c_pos, c_batch_stride, slices_per_query, t_gsw, bits, live,
+                               zero_flags);
 }
 void launch_from_ntt(const DevParams& P, uint64_t* out_raw, const uint32_t* in, size_t count, cudaStream_t s) {
   if (count) ++g_kernel_launches, k_from_ntt<<<(unsigned)count, CTA, 0, s>>>(P, out_raw, in);
@@ -1285,7 +1310,7 @@ void launch_expand_round_pair(const DevParams& P, uint32_t* v, size_t v_stride, 
 }
 void launch_expand_round_res(const DevParams& P, uint32_t* v, size_t v_stride, uint32_t* xr, size_t xr_stride, int nq,
                              const ExpandRound& R, const uint32_t* neg1_r, cudaStream_t s) {
-  const size_t smem = (size_t)2 * NTT_SMEM_WORDS * 4 + (size_t)POLY * 8 + (size_t)HI_TW * 8;
+  const size_t smem = (size_t)2 * NTT_SMEM_WORDS * 4 + (size_t)2 * POLY * 8 + (size_t)HI_TW * 8;
   opt_in_smem(k_expand_round_res, (int)smem);
   g_kernel_launches += 2;
   k_expand_intt<<<dim3((unsigned)R.num_in, 2, nq), 256, 0, s>>>(P, v, v_stride, xr, xr_stride, R);
@@ -1299,32 +1324,32 @@ void launch_reorient(const MulGeom& G, uint4* q_dev, size_t q_stride, const uint
 }
 void launch_regev_to_gsw(const DevParams& P, uint32_t* v_gsw, size_t gsw_stride, const uint32_t* v, size_t v_stride,
                          int nq, int count, int idx_factor, int idx_offset, const uint32_t* const* tab_conv, int t_gsw,
-                         int t_conv, int bits_conv, cudaStream_t s) {
+                         int t_conv, int bits_conv, int live_conv, cudaStream_t s) {
   if (count == 0) return;
   opt_in_smem(k_regev_to_gsw, (int)kDynSmemBig);
   ++g_kernel_launches;
   k_regev_to_gsw<<<dim3((unsigned)(count * t_gsw), nq), CTA, kDynSmemBig, s>>>(P, v_gsw, gsw_stride, v, v_stride,
                                                                                idx_factor, idx_offset, tab_conv, t_gsw,
-                                                                               t_conv, bits_conv);
+                                                                               t_conv, bits_conv, live_conv);
 }
 template <int ROWS>
 static void launch_pack_t(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded,
                           size_t ct_stride, size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int instances,
-                          int t_conv, int bits_conv, int version, const uint64_t* raw_cts, cudaStream_t s) {
+                          int t_conv, int bits_conv, int live_conv, int version, const uint64_t* raw_cts, cudaStream_t s) {
   opt_in_smem(k_pack<ROWS>, (int)kDynSmemBig);
   ++g_kernel_launches;
   k_pack<ROWS><<<dim3((unsigned)(instances * (ROWS - 1)), nq), CTA, kDynSmemBig, s>>>(
-      P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, tab_pack, t_conv, bits_conv, version, raw_cts);
+      P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, tab_pack, t_conv, bits_conv, live_conv, version, raw_cts);
 }
 void launch_pack(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, const uint32_t* folded, size_t ct_stride,
                  size_t in_q_stride, int nq, const uint32_t* const* tab_pack, int n, int instances, int t_conv, int bits_conv,
-                 int version, cudaStream_t s, const uint64_t* raw_cts) {
+                 int live_conv, int version, cudaStream_t s, const uint64_t* raw_cts) {
   if (raw_cts && nq != 1) throw Error(-2, "pack: raw ciphertexts are taken for one query");
   switch (n) {
-    case 1: launch_pack_t<2>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
-    case 2: launch_pack_t<3>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
-    case 3: launch_pack_t<4>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
-    case 4: launch_pack_t<5>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, version, raw_cts, s); break;
+    case 1: launch_pack_t<2>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, live_conv, version, raw_cts, s); break;
+    case 2: launch_pack_t<3>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, live_conv, version, raw_cts, s); break;
+    case 3: launch_pack_t<4>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, live_conv, version, raw_cts, s); break;
+    case 4: launch_pack_t<5>(P, out_raw, out_q_stride, folded, ct_stride, in_q_stride, nq, tab_pack, instances, t_conv, bits_conv, live_conv, version, raw_cts, s); break;
     default: throw Error(-2, "pack: n must be 1..4");
   }
 }
