@@ -33,7 +33,7 @@ def test_stage_level_sparse_fold_matches_oracle():
         assert np.array_equal(got[: 2 * P.N], ref.reshape(-1)[: 2 * P.N]), name
 
 
-@pytest.mark.parametrize("fmt", [1, 0])
+@pytest.mark.parametrize("fmt", [1, 0, 2])
 def test_process_query_on_sparse_database_matches_sparse_server(fmt):
     S, P, cl, pp, db, G, gdb, gpp = setup_case("T")
     sdb = db.reshape(P.slices, P.N, P.num_per, P.dim0).copy()

@@ -87,39 +87,3 @@ def test_tc5_long_k_many_tiles_worst_case():
         tdb.close()
         G.close()
 
-
-def test_tc5_sparse_database_skips_absent_tiles():
-    """lib/server's SparseDb semantics as cost (db/sparse_db.rs:5-47, compute/dot_product.rs:35): an item exists once written;
-    tiles (32 rows x 32 values of j) without a present item are neither fetched nor multiplied.  512 x 64 geometry = 16 k-steps
-    in two 8-step ring stages x 2 row tiles: patterns with a completely empty database, an empty row tile, an empty ring
-    stage, single k-steps inside a stage; the product must equal the oracle's on the zero-filled database every time."""
-    S, _, _, _, _, _, _, _ = setup_case("T")
-    kw = dict(O.PARAM_SETS["T"])
-    kw.update(nu_1=9, nu_2=6, n=1, db_item_size=2048)
-    P = O.Params(**kw)
-    G = S.Params(**kw)
-    rng = np.random.default_rng(77)
-    v = rng.integers(0, Q0, P.dim0 * 2 * P.N, dtype=np.uint64) | (rng.integers(0, Q1, P.dim0 * 2 * P.N, dtype=np.uint64) << np.uint64(32))
-    tdb = S.Database(G, fmt=2)
-    info = tdb.info()
-    assert info["format"] == 2 and info["present_items"] == 0 and info["capacity"] == P.dim0 * P.num_per
-    dense = np.zeros((P.N, P.num_per, P.dim0), dtype=np.uint64)             # reference layout [z][ii][j] of the one slice
-    assert not S.multiply_reg_by_database(G, tdb, 0, v).any()              # nothing present: all-zero product, no tile touched
-    placed = 0
-    # (j, ii): one k-step of stage 0 in row tile 0; then stage 1 only in row tile 1; then neighbours inside present tiles
-    for j, ii in [(37, 3), (300, 40), (301, 63), (37, 4), (0, 0), (511, 63), (255, 31), (256, 32)]:
-        poly = rng.integers(0, Q0, P.N, dtype=np.uint64) | (rng.integers(0, Q1, P.N, dtype=np.uint64) << np.uint64(32))
-        tdb.upsert_item(0, j * P.num_per + ii, poly)
-        dense[:, ii, j] = poly
-        placed += 1
-        assert tdb.info()["present_items"] == placed
-        assert np.array_equal(S.multiply_reg_by_database(G, tdb, 0, v), P.multiply_reg_by_database(dense.reshape(-1), v)), (j, ii)
-    tdb.upsert_item(0, 37 * P.num_per + 3, dense[:, 3, 37].copy())          # rewriting an item does not count twice
-    assert tdb.info()["present_items"] == placed
-    # bulk upload marks everything present
-    full = S.Database.from_words(G, dense.reshape(-1), fmt=2)
-    assert full.info()["present_items"] == P.dim0 * P.num_per
-    assert np.array_equal(S.multiply_reg_by_database(G, full, 0, v), P.multiply_reg_by_database(dense.reshape(-1), v))
-    full.close()
-    tdb.close()
-    G.close()
