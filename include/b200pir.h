@@ -54,13 +54,12 @@ int b200pir_ctx_synchronize(b200pir_ctx* ctx);
 /* knobs: "mul_variant" (kernel tiling), "batch" (max queries per database pass: 1, 2, 4, 8 or 16;
  * the IMAD layout uses at most 4), "db_format" (layout of databases created afterwards: -1 = automatic (default): 2 wherever the
  * wgmma kernel supports the geometry, else 1; 0 = IMAD, 1 = mma.sync INT8 fragments, 2 = wgmma tile images, tc5_kernels.cu), "profile" (0 off, 1 per call,
- * 2 accumulate over calls until set again); A/B switches for kernel variants: "intt_variant", "imma_variant",
- * "expand_variant" (0 = default everywhere); "fold_variant" (accepted, no effect: there is one fold kernel); "coalesce" (1 = default: concurrent single-query callers
+ * 2 accumulate over calls until set again); "fold_variant", "intt_variant", "imma_variant", "expand_variant",
+ * "expand_pair_min_ctas" (accepted, no effect: one kernel or schedule each remains); "coalesce" (1 = default: concurrent single-query callers
  * share database passes, see b200pir_coalesce_stats), "coalesce_window_us" (default 200: how long a batch that directly
  * follows a multi-query batch is held open for the callers of that batch to return; 0 = never), "sparse_fold" (1 = fold like lib/server's sparse server,
  * compute/fold.rs:15-65: an all-zero ciphertext short-cuts the external product; 0 = spiral-rs's dense fold, default; version-1
- * servers set 1: with t_gsw = 7 the dense fold does not decode items whose row is folded against an empty one); "expand_pair_min_ctas" (expansion rounds with at least this many active
- * ciphertexts use the paired kernel, default 1: every round);
+ * servers set 1: with t_gsw = 7 the dense fold does not decode items whose row is folded against an empty one);
  * unknown keys -> B200PIR_E_BADARG */
 int b200pir_ctx_set_option(b200pir_ctx* ctx, const char* key, int64_t value);
 /* Size the context's workspace once, up front, for `queries` concurrent queries against a database with `rows_local`

@@ -97,11 +97,7 @@ struct b200pir_ctx {
   DevBuf<uint32_t> d_neg1;   // [11][2][2048] ntt32 (params.rs:98-107)
   // options
   int mul_variant = 0, max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
-  int intt_variant = 0;
-  int expand_variant = 0;        // wide rounds: 0 paired + residue pipeline (2 CTAs/SM), 2 paired single kernel; 1: never paired
-  long pair_min_ctas = 1;        // every round paired: on H100 (S8, 16 queries) narrow rounds cost more at any width
   int sparse_fold = 0;           // 1: lib/server's fold (all-zero ciphertext shortcut, compute/fold.rs:37-43); 0: spiral-rs dense fold
-  int imma_variant = 0;          // 0: cp.async-pipelined kernel for 5..8 queries per pass, 1: load-then-use kernel
   int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the wgmma kernel
                                  // supports the geometry, else 1), 0 = IMAD layout, 1 = mma.sync fragments, 2 = wgmma tile images
   DevBuf<uint2> w_qf;            // B operand of the IMMA path (one group of <= 16 queries)
@@ -112,7 +108,7 @@ struct b200pir_ctx {
   DevBuf<uint64_t> w_query;      // [Q][2][2048] raw
   DevBuf<uint32_t> w_v;          // [Q][2^g][2][2][2048]
   DevBuf<uint32_t> w_zflags;     // all-zero flags of the current fold round's ciphertexts ("sparse_fold")
-  DevBuf<uint32_t> w_xr;         // [Q][num_in][2][2048] residues of row 0 (paired expansion rounds)
+  DevBuf<uint32_t> w_xr;         // [Q][num_in][2][2048] residues of row 0 (expansion rounds)
   DevBuf<uint4> w_qdev;          // [Q][dim0][2048]
   DevBuf<uint32_t> w_vfold, w_vfold_neg;   // [Q][nu_2][2][2t][2][2048]
   DevBuf<uint32_t> w_mult;       // [Q][slices][rows][2][2][2048]  NTT form, then residue form in place
@@ -384,11 +380,6 @@ void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size
   const PpTable T = c->pp_table(pp, (size_t)nq);
   for (int r = 0; r < g; r++) {
     const int num_in = 1 << r;
-    // wide rounds: one CTA per input ciphertext produces both outputs (no scalar-multiply pass, one inverse transform);
-    // narrow rounds keep one CTA per output, which halves their latency
-    const long active = (long)((stop_round > 0 && r > stop_round) ? num_in / 2 : num_in) * nq;
-    const bool pair = c->expand_variant != 1 && active >= c->pair_min_ctas;
-    if (!pair) launch_expand_scalar(c->dp, v, v_stride, nq, num_in, c->d_neg1.p + (size_t)r * 2 * POLY, s);
     ExpandRound R;
     R.r = r; R.num_in = num_in; R.stop_round = stop_round; R.max_bits_to_gen_right = max_right;
     R.fill_skipped = all_slots ? 1 : 0;
@@ -404,12 +395,9 @@ void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size
     } else {
       R.t_right = R.t_left; R.bits_right = R.bits_left; R.live_right = R.live_left; R.tab_right = T.left; R.off_right = R.off_left;   // unwrap_or(v_w_left), server.rs:549
     }
-    if (pair && c->expand_variant == 0) {
-      const size_t xr_stride = (size_t)num_in * 2 * POLY;
-      c->w_xr.ensure((size_t)nq * xr_stride);
-      launch_expand_round_res(c->dp, v, v_stride, c->w_xr.p, xr_stride, nq, R, c->d_neg1.p + (size_t)r * 2 * POLY, s);
-    } else if (pair) launch_expand_round_pair(c->dp, v, v_stride, nq, R, c->d_neg1.p + (size_t)r * 2 * POLY, s);
-    else launch_expand_round(c->dp, v, v_stride, nq, R, s);
+    const size_t xr_stride = (size_t)num_in * 2 * POLY;
+    c->w_xr.ensure((size_t)nq * xr_stride);
+    launch_expand_round_res(c->dp, v, v_stride, c->w_xr.p, xr_stride, nq, R, c->d_neg1.p + (size_t)r * 2 * POLY, s);
   }
 }
 
@@ -525,7 +513,7 @@ void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const 
     }
     {
       b200pir_ctx::Scope sc(c, ST_FROMNTT);
-      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->intt_variant, c->stream);
+      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
     }
   } else {
     // INT8 tensor-core path: z-major product in w_cts (free until the fold starts), then inverse NTT into w_mult
@@ -540,13 +528,13 @@ void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const 
       {
         b200pir_ctx::Scope sc(c, ST_MUL);
         launch_multiply_imma(c->dp, db->F, db->f.p, c->w_qf.p, c->w_cts.p + qi * out_stride, out_stride, nq, 0, c->slices,
-                             c->imma_variant, c->stream);
+                             c->stream);
         c->mul_launches++;
       }
     }
     {
       b200pir_ctx::Scope sc(c, ST_FROMNTT);
-      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->intt_variant, c->stream);
+      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
     }
   }
   {
@@ -759,14 +747,12 @@ int b200pir_ctx_set_option(b200pir_ctx* c, const char* key, int64_t value) {
   std::string k(key);
   if (k == "mul_variant") c->mul_variant = (int)value;
   else if (k == "batch") { if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) throw Error(B200PIR_E_BADARG, "batch must be 1, 2, 4, 8 or 16"); c->max_group = (int)value; }
-  else if (k == "fold_variant") {}   // one fold kernel now; the key stays accepted so existing callers keep working
-  else if (k == "intt_variant") c->intt_variant = (int)value;
-  else if (k == "imma_variant") c->imma_variant = (int)value;
+  // one kernel each now; the keys stay accepted so existing callers keep working
+  else if (k == "fold_variant" || k == "intt_variant" || k == "imma_variant" || k == "expand_variant" ||
+           k == "expand_pair_min_ctas") {}
   else if (k == "sparse_fold") c->sparse_fold = value != 0;
   else if (k == "coalesce") c->coalesce = value != 0;
   else if (k == "coalesce_window_us") { if (value < 0 || value > 100000) throw Error(B200PIR_E_BADARG, "coalesce_window_us must be 0..100000"); c->coalesce_window_us = (int)value; }
-  else if (k == "expand_variant") c->expand_variant = (int)value;
-  else if (k == "expand_pair_min_ctas") c->pair_min_ctas = (long)value;
   else if (k == "db_format") { if (value < -1 || value > 2) throw Error(B200PIR_E_BADARG, "db_format must be -1 (automatic), 0, 1 or 2"); c->db_format = (int)value; }
   else if (k == "profile") {
     if (value < 0 || value > 2) throw Error(B200PIR_E_BADARG, "profile must be 0, 1 or 2");
@@ -1462,7 +1448,7 @@ int b200pir_multiply_reg_by_database(b200pir_ctx* c, b200pir_db* db, uint64_t sl
     DevBuf<uint2> qf(imma_query_cells(db->F));
     DevBuf<uint32_t> zm((size_t)c->slices * rows * 4 * POLY);
     launch_query_to_frag(db->F, qd.p, 0, 1, qf.p, c->stream);
-    launch_multiply_imma(c->dp, db->F, db->f.p, qf.p, zm.p, 0, 1, (int)slice, 1, c->imma_variant, c->stream);
+    launch_multiply_imma(c->dp, db->F, db->f.p, qf.p, zm.p, 0, 1, (int)slice, 1, c->stream);
     launch_zmajor_to_ntt32(db->F, zm.p, o.p + (size_t)slice * rows * 4 * POLY, (int)slice, c->stream);
     B200_CUDA(cudaStreamSynchronize(c->stream));
   }

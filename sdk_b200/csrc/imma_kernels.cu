@@ -357,28 +357,9 @@ struct SyncI {
 
 // inverse NTT of every (ciphertext row, modulus) of the z-major product -> residue-form ciphertexts
 //   out[((query*slices + slice)*rows + ii)][ct_row][n][z]     (server.rs:707-709 without the CRT lift)
-// grid = (rows*2 polys, 2 moduli, nq*slices), 256 threads
-__global__ void __launch_bounds__(256)
-k_intt_from_zmajor(DevParams P, ImmaGeom F, const uint32_t* __restrict__ in_zm, size_t in_stride, uint32_t* __restrict__ out,
-                   int slices) {
-  __shared__ __align__(16) uint32_t sm[NTT_SMEM_WORDS];
-  const int tid = threadIdx.x, n = blockIdx.y;
-  const int ii = blockIdx.x >> 1, r = blockIdx.x & 1;
-  const int qs = blockIdx.z, qi = qs / slices, slice = qs % slices;
-  const uint32_t q = n ? P.q[1] : P.q[0];
-  const uint32_t* src = in_zm + (size_t)qi * in_stride + (((size_t)slice * 2 + n) * POLY) * F.rows * 2 + (size_t)ii * 2 + r;
-  uint32_t x[8];
-#pragma unroll
-  for (int k = 0; k < 8; k++) x[k] = __ldg(src + (size_t)(tid * 8 + k) * F.rows * 2);
-  ntt_inverse_group_nh(tid, x, sm, TwConstI{n, 2}, TwGlobalI{n ? P.inv_lz[1] : P.inv_lz[0]}, q, SyncI());
-  uint32_t* dst = out + ((((size_t)qs * F.rows + ii) * 2 + r) * 2 + n) * POLY;
-#pragma unroll
-  for (int a = 0; a < 8; a++) dst[a * 256 + tid] = x[a];
-}
-
-// Tiled variant: one CTA handles PP (= 2, 4 or 8) polynomials that are adjacent in the z-major product, so every
-// 32-byte sector it fetches is fully used (the simple kernel above uses 4 of every 32 bytes).  The PP polynomials are
-// transposed through shared memory, then inverse-transformed two at a time.
+// One CTA handles PP (= 2, 4 or 8) polynomials that are adjacent in the z-major product, so every 32-byte sector it fetches
+// is fully used (one CTA per polynomial would use 4 of every 32 bytes: its z-stride is rows*2 words).  The PP polynomials
+// are transposed through shared memory, then inverse-transformed two at a time.  rows*2 is even, so PP = 2 always fits.
 // grid = (rows*2 / PP, 2 moduli, nq*slices), 256 threads, dynamic smem = PP*2048*4 + 2*NTT_SMEM_WORDS*4
 template <int PP>
 __global__ void __launch_bounds__(256)
@@ -475,7 +456,7 @@ void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride
   k_query_to_frag<<<grid1d(warps * 32, 256), 256, 0, s>>>(F, q_dev, q_stride, nq, ntiles, qf);
 }
 void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* dbf, const uint2* qf, uint32_t* out_zm,
-                          size_t out_stride, int nq, int slice_begin, int slice_count, int variant, cudaStream_t s) {
+                          size_t out_stride, int nq, int slice_begin, int slice_count, cudaStream_t s) {
   if (nq < 1 || nq > 16) throw Error(-2, "imma multiply: 1..16 queries per pass");
   const int ntiles = imma_query_tiles(nq);
   const size_t smem = (size_t)ntiles * F.ks * 128 * sizeof(uint2);
@@ -493,7 +474,7 @@ void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* db
     return;
   }
   if (smem > 96 * 1024) throw Error(-2, "imma multiply: dim0 too large");
-  if (ntiles == 2 && variant == 0 && smem8 <= 112 * 1024)
+  if (ntiles == 2 && smem8 <= 112 * 1024)
     k_multiply_imma8<2, IMMA_STAGES><<<dim3(POLY, 2), 256, smem8, s>>>(P, F, dbf, qf, out_zm, out_stride, nq, slice_begin,
                                                                        slice_count);
   else if (ntiles == 1)
@@ -509,12 +490,10 @@ static void launch_intt_tiled(const DevParams& P, const ImmaGeom& F, const uint3
   k_intt_from_zmajor_tiled<PP><<<dim3(F.rows * 2 / PP, 2, nq * slices), 256, smem, s>>>(P, F, in_zm, in_stride, out, slices);
 }
 void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
-                             int nq, int slices, int variant, cudaStream_t s) {
+                             int nq, int slices, cudaStream_t s) {
   ++g_kernel_launches;
   const int polys = F.rows * 2;
-  if (variant == 1)
-    k_intt_from_zmajor<<<dim3(F.rows * 2, 2, nq * slices), 256, 0, s>>>(P, F, in_zm, in_stride, out, slices);
-  else if (polys % 8 == 0) launch_intt_tiled<8>(P, F, in_zm, in_stride, out, nq, slices, s);
+  if (polys % 8 == 0) launch_intt_tiled<8>(P, F, in_zm, in_stride, out, nq, slices, s);
   else if (polys % 4 == 0) launch_intt_tiled<4>(P, F, in_zm, in_stride, out, nq, slices, s);
   else launch_intt_tiled<2>(P, F, in_zm, in_stride, out, nq, slices, s);
 }

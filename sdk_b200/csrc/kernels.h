@@ -86,11 +86,10 @@ void launch_db_upsert_frag(const ImmaGeom& F, uint4* dbf, int slice, int il, int
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s);
 // out_zm: u32 [query][slice][n][z][row][ct_row]  (queries out_stride words apart)
 void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* dbf, const uint2* qf, uint32_t* out_zm,
-                          size_t out_stride, int nq, int slice_begin, int slice_count, int variant, cudaStream_t s);
+                          size_t out_stride, int nq, int slice_begin, int slice_count, cudaStream_t s);
 // inverse NTT of the z-major product -> residue-form ciphertexts [query*slices + slice][row][ct_row][n][z]
-// variant 0: tiled (sector-efficient) kernel, 1: simple gather kernel
 void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
-                             int nq, int slices, int variant, cudaStream_t s);
+                             int nq, int slices, cudaStream_t s);
 // z-major product of one slice -> ntt32 [row][ct_row][n][z]
 void launch_zmajor_to_ntt32(const ImmaGeom& F, const uint32_t* in_zm, uint32_t* out, int slice, cudaStream_t s);
 
@@ -148,10 +147,7 @@ void launch_folding_neg(const DevParams& P, uint32_t* out, const uint32_t* v_fol
                         cudaStream_t s);
 
 // ---- query expansion (server.rs:19-151, 525-591)
-// v: ntt32 [nq][2^g][2][n][z] (queries v_stride words apart).  One round = scalar-multiply launch + expand
-// launch, each covering all nq queries (grid.y).
-void launch_expand_scalar(const DevParams& P, uint32_t* v, size_t v_stride, int nq, int num_in, const uint32_t* neg1_r,
-                          cudaStream_t s);
+// v: ntt32 [nq][2^g][2][n][z] (queries v_stride words apart).
 // Public parameters are per QUERY: device arrays of base pointers (the ntt32 matrices of the client that sent query i), so one
 // launch serves concurrent queries of different clients — lib/server looks the parameters up per request (bin/server.rs:113-117).
 struct PpTable { const uint32_t* const* pack; const uint32_t* const* left; const uint32_t* const* right; const uint32_t* const* conv; };
@@ -162,13 +158,10 @@ struct ExpandRound {
   size_t off_left, off_right;
   int t_left, t_right, bits_left, bits_right;
   int live_left, live_right;   // live_digits(t_left / t_right): the automorphed coefficients are <= q
-  int fill_skipped;         // paired kernel: also write v[i + num_in] = v[i] (.) neg1 for skipped i (stage-level parity)
+  int fill_skipped;         // also write v[i + num_in] = v[i] (.) neg1 for skipped i (stage-level parity)
 };
-void launch_expand_round(const DevParams& P, uint32_t* v, size_t v_stride, int nq, const ExpandRound& R, cudaStream_t s);
-// both outputs of every input ciphertext in one CTA; replaces launch_expand_scalar + launch_expand_round for that round
-void launch_expand_round_pair(const DevParams& P, uint32_t* v, size_t v_stride, int nq, const ExpandRound& R,
-                              const uint32_t* neg1_r, cudaStream_t s);
-// the paired round split into an inverse-transform kernel (residues -> xr) and single-modulus CTAs at 3 per SM
+// One expansion round: both outputs of every input ciphertext are made together, by an inverse-transform kernel (residues ->
+// xr) and single-modulus CTAs at 3 per SM, each launch covering all nq queries
 void launch_expand_round_res(const DevParams& P, uint32_t* v, size_t v_stride, uint32_t* xr, size_t xr_stride, int nq,
                              const ExpandRound& R, const uint32_t* neg1_r, cudaStream_t s);
 // util.rs:323-355 reorient: v[idx_factor*j] -> q_dev   (per query: q_stride uint4 apart)

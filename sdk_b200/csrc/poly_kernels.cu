@@ -603,229 +603,18 @@ __global__ void k_folding_neg(DevParams P, uint32_t* out, const uint32_t* vf, si
 }
 
 // ------------------------------------------------------------------ query expansion
-// server.rs:105-110: v[num_in + i] = v[i] (.) neg1
-__global__ void k_expand_scalar(DevParams P, uint32_t* v, size_t v_stride, int num_in, const uint32_t* neg1) {
-  v += (size_t)blockIdx.y * v_stride;
-  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;     // over num_in * 2 rows * 2 mod * 2048
-  size_t total = (size_t)num_in * 4 * POLY;
-  if (idx >= total) return;
-  int z = (int)(idx % POLY);
-  int n = (int)((idx / POLY) & 1);
-  uint32_t a = v[idx], b = neg1[n * POLY + z];
-  v[total + idx] = barrett64((uint64_t)a * b, P.cr1[n], P.q[n]);
-}
-
-// server.rs:39-103 action_expand for ciphertext index blockIdx.x of round R.r (in place on v).
-__global__ void __launch_bounds__(CTA, 1) k_expand_round(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R) {
-  v += (size_t)blockIdx.y * v_stride;
-  extern __shared__ __align__(16) uint8_t dyn_smem[];
-  uint32_t* ntt_smem = reinterpret_cast<uint32_t*>(dyn_smem);
-  uint32_t* res = ntt_smem + 4 * NTT_SMEM_WORDS;
-  uint64_t* autom = reinterpret_cast<uint64_t*>(res + 2 * POLY);      // [2][2048]
-  Twiddle* tw = reinterpret_cast<Twiddle*>(autom + 2 * POLY);         // [2][HI_TW]
-  Grp g = make_grp(P, ntt_smem);
-  g.smem2 = ntt_smem + (2 + g.n) * NTT_SMEM_WORDS;
-
-  const int i = blockIdx.x;
-  const int ih = i < R.num_in ? i : i - R.num_in;       // index within its half (server.rs:112-119)
-  if ((R.stop_round > 0 && R.r > R.stop_round && (ih & 1)) ||
-      (R.stop_round > 0 && R.r == R.stop_round && (ih & 1) && (ih / 2) >= R.max_bits_to_gen_right))
-    return;
-  const bool left = (R.r != 0) && ((ih & 1) == 0);
-  const uint32_t* W = left ? R.tab_left[blockIdx.y] + R.off_left : R.tab_right[blockIdx.y] + R.off_right;
-  const int t_exp = left ? R.t_left : R.t_right;
-  const int bits = left ? R.bits_left : R.bits_right;
-  const int live = left ? R.live_left : R.live_right;
-
-  stage_fwd_twiddles(g, tw + g.n * HI_TW);
-  uint32_t* vi = v + (size_t)i * 4 * POLY;
-  // row 0: from_ntt + automorph (poly.rs:393-405), scattered into shared memory for the gadget digits
-  {
-    uint32_t x[8];
-    ld8(x, vi + (size_t)g.n * POLY + g.tid * 8);
-    grp_ntt_inv(g, x);
-    const int t_auto = R.t_auto;
-    const uint64_t Q = P.modulus;
-    crt_lift(x, res, g, P, [&](int z, uint64_t val) {
-      unsigned prod = (unsigned)z * (unsigned)t_auto;
-      unsigned num = prod >> NTT_LOG_N, rem = prod & (POLY - 1);
-      autom[rem] = (num & 1u) ? Q - val : val;           // zero maps to q, as in the reference
-    });
-  }
-  __syncthreads();
-  uint64_t acc[2][8];
-#pragma unroll
-  for (int r = 0; r < 2; r++)
-#pragma unroll
-    for (int e = 0; e < 8; e++) acc[r][e] = 0;
-  int cnt = 0;
-  // gadget_invert_rdim(.., rdim = 1): digit k -> key column k  (server.rs:82-89)
-  digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, live, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
-                      (size_t)t_exp * 2 * POLY, g);
-  // row 1: the reference computes to_ntt(automorph(from_ntt(row 1))) (server.rs:80-88).  X -> X^t permutes the
-  // roots of X^N + 1, so in the NTT domain the automorphism is a pure permutation of the evaluation slots:
-  // slot s holds the value at psi^(2 br(s) + 1), and tau_t(a) there equals a at psi^((2 br(s) + 1) t).  The
-  // values are canonical residues either way, so the gathered vector is bit-identical to the reference's.
-  // Gathered before any thread overwrites v[i].
-  uint32_t y[8];
-  {
-    const uint32_t* row1 = vi + ((size_t)2 + g.n) * POLY;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const unsigned sidx = (unsigned)(g.tid * 8 + k);
-      const unsigned e = 2u * (__brev(sidx) >> (32 - NTT_LOG_N)) + 1u;
-      const unsigned e2 = (e * (unsigned)R.t_auto) & (2u * POLY - 1u);
-      const unsigned src = __brev((e2 - 1u) >> 1) >> (32 - NTT_LOG_N);
-      y[k] = row1[src];
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int rho = 0; rho < 2; rho++) {
-    uint32_t o[8];
-    ld8(o, vi + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8);
-#pragma unroll
-    for (int e = 0; e < 8; e++) {
-      uint32_t s = addmod(o[e], barrett64(acc[rho][e], g.cr1, g.q), g.q);
-      o[e] = rho ? addmod(s, y[e], g.q) : s;
-    }
-    st8(vi + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8, o);
-  }
-}
-
-// Paired variant for the wide rounds: CTA i produces BOTH outputs that derive from v[i], i.e. index i and index
-// i + num_in (= action_expand on v[i] (.) neg1[r], server.rs:105-110).  neg1[r] is the NTT of -X^(N - 2^r) = X^(-2^r), so
+// server.rs:39-110, one round: CTA i produces BOTH outputs that derive from v[i], i.e. index i (action_expand on v[i]) and
+// index i + num_in (action_expand on v[i] (.) neg1[r], server.rs:105-110).  neg1[r] is the NTT of -X^(N - 2^r) = X^(-2^r), so
 //   * from_ntt(v[i] (.) neg1) is the negacyclic shift of from_ntt(v[i]) by 2^r places: coefficient k is residue k + 2^r
 //     of the first output, negated mod q_n (0 stays 0, the canonical residue the reference's inverse NTT returns) when
-//     k + 2^r wraps past N.  One inverse transform serves both outputs and the separate scalar-multiply pass
-//     (k_expand_scalar: 64 KiB of HBM traffic per ciphertext) disappears;
+//     k + 2^r wraps past N.  One inverse transform serves both outputs, and no separate scalar-multiply pass is needed;
 //   * the NTT-domain rows of the second output are pointwise products with neg1, formed in registers.
-// Only CTA i touches v[i] and v[i + num_in], so the round stays in place.  Used when the round has enough active
-// ciphertexts to fill the GPU; narrow rounds keep one CTA per output (half the latency).
-__global__ void __launch_bounds__(CTA, 1)
-k_expand_round_pair(DevParams P, uint32_t* v, size_t v_stride, ExpandRound R, const uint32_t* __restrict__ neg1) {
-  v += (size_t)blockIdx.y * v_stride;
-  extern __shared__ __align__(16) uint8_t dyn_smem[];
-  uint32_t* ntt_smem = reinterpret_cast<uint32_t*>(dyn_smem);
-  uint32_t* res = ntt_smem + 4 * NTT_SMEM_WORDS;
-  uint64_t* autom = reinterpret_cast<uint64_t*>(res + 2 * POLY);
-  Twiddle* tw = reinterpret_cast<Twiddle*>(autom + 2 * POLY);
-  Grp g = make_grp(P, ntt_smem);
-  g.smem2 = ntt_smem + (2 + g.n) * NTT_SMEM_WORDS;
-
-  const int i = blockIdx.x;                               // index within the half == i for both outputs
-  if ((R.stop_round > 0 && R.r > R.stop_round && (i & 1)) ||
-      (R.stop_round > 0 && R.r == R.stop_round && (i & 1) && (i / 2) >= R.max_bits_to_gen_right)) {
-    // never read again by the query path; the reference still leaves v[i + num_in] = v[i] (.) neg1 there
-    // (server.rs:105-110 runs before the skip test), which the stage-level entry point reproduces
-    if (R.fill_skipped) {
-      const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
-      const uint32_t qn = n ? P.q[1] : P.q[0];
-      const uint64_t cr1 = n ? P.cr1[1] : P.cr1[0];
-      uint32_t nn[8];
-      ld8_ro(nn, neg1 + (size_t)n * POLY + tid * 8);
-#pragma unroll
-      for (int rho = 0; rho < 2; rho++) {
-        uint32_t x[8];
-        ld8(x, v + ((size_t)i * 4 + rho * 2 + n) * POLY + tid * 8);
-#pragma unroll
-        for (int e = 0; e < 8; e++) x[e] = barrett64((uint64_t)x[e] * nn[e], cr1, qn);
-        st8(v + ((size_t)(i + R.num_in) * 4 + rho * 2 + n) * POLY + tid * 8, x);
-      }
-    }
-    return;
-  }
-  const bool left = (R.r != 0) && ((i & 1) == 0);
-  const uint32_t* W = left ? R.tab_left[blockIdx.y] + R.off_left : R.tab_right[blockIdx.y] + R.off_right;
-  const int t_exp = left ? R.t_left : R.t_right;
-  const int bits = left ? R.bits_left : R.bits_right;
-  const int live = left ? R.live_left : R.live_right;
-
-  stage_fwd_twiddles(g, tw + g.n * HI_TW);
-  uint32_t* vi = v + (size_t)i * 4 * POLY;
-  uint32_t* vo = v + (size_t)(i + R.num_in) * 4 * POLY;
-  const uint32_t* ng = neg1 + (size_t)g.n * POLY;
-  uint32_t keep[2][8], y[8];
-  {
-    uint32_t x[8];
-    ld8(x, vi + (size_t)g.n * POLY + g.tid * 8);
-#pragma unroll
-    for (int e = 0; e < 8; e++) keep[0][e] = x[e];
-    grp_ntt_inv(g, x);
-    __syncthreads();
-#pragma unroll
-    for (int a = 0; a < 8; a++) res[g.n * POLY + a * 256 + g.tid] = x[a];      // canonical residues, coefficient order
-  }
-  const uint32_t* row1 = vi + ((size_t)2 + g.n) * POLY;
-  ld8(keep[1], row1 + g.tid * 8);
-#pragma unroll
-  for (int k = 0; k < 8; k++) {
-    const unsigned sidx = (unsigned)(g.tid * 8 + k);
-    const unsigned e = 2u * (__brev(sidx) >> (32 - NTT_LOG_N)) + 1u;
-    const unsigned e2 = (e * (unsigned)R.t_auto) & (2u * POLY - 1u);
-    const unsigned src = __brev((e2 - 1u) >> 1) >> (32 - NTT_LOG_N);
-    y[k] = row1[src];
-  }
-  __syncthreads();
-  const uint64_t Q = P.modulus;
-  const uint32_t q0 = P.q[0], q1 = P.q[1];
-#pragma unroll 1
-  for (int half = 1; half >= 0; half--) {
-    const int shift = half ? R.num_in : 0;                // 2^r
-#pragma unroll
-    for (int a4 = 0; a4 < 4; a4++) {
-      const int k = (g.n * 4 + a4) * 256 + g.tid;
-      const int zs = (k + shift) & (POLY - 1);
-      uint32_t a0 = res[zs], a1 = res[POLY + zs];
-      if (k + shift >= POLY) {
-        a0 = a0 ? q0 - a0 : 0u;
-        a1 = a1 ? q1 - a1 : 0u;
-      }
-      const uint64_t val = crt_compose(a0, a1, P);
-      const unsigned prod = (unsigned)k * (unsigned)R.t_auto;
-      const unsigned num = prod >> NTT_LOG_N, rem = prod & (POLY - 1);
-      autom[rem] = (num & 1u) ? Q - val : val;            // zero maps to q, as in the reference
-    }
-    __syncthreads();
-    uint64_t acc[2][8];
-#pragma unroll
-    for (int r = 0; r < 2; r++)
-#pragma unroll
-      for (int e = 0; e < 8; e++) acc[r][e] = 0;
-    int cnt = 0;
-    digits_mac<2, true>(acc, cnt, SmemCoef{autom + g.tid}, live, bits, W + (size_t)g.n * POLY + g.tid * 8, (size_t)2 * POLY,
-                        (size_t)t_exp * 2 * POLY, g);
-    uint32_t* dst = half ? vo : vi;
-#pragma unroll
-    for (int rho = 0; rho < 2; rho++) {
-      uint32_t o[8], nn[8];
-      if (half) ld8_ro(nn, ng + g.tid * 8);
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        uint32_t base = keep[rho][e];
-        if (half) base = barrett64((uint64_t)base * nn[e], g.cr1, g.q);
-        uint32_t s = addmod(base, barrett64(acc[rho][e], g.cr1, g.q), g.q);
-        if (rho) {
-          uint32_t yy = y[e];
-          if (half) {
-            const unsigned sidx = (unsigned)(g.tid * 8 + e);
-            const unsigned ee = 2u * (__brev(sidx) >> (32 - NTT_LOG_N)) + 1u;
-            const unsigned e2 = (ee * (unsigned)R.t_auto) & (2u * POLY - 1u);
-            const unsigned src = __brev((e2 - 1u) >> 1) >> (32 - NTT_LOG_N);
-            yy = barrett64((uint64_t)yy * __ldg(ng + src), g.cr1, g.q);
-          }
-          s = addmod(s, yy, g.q);
-        }
-        o[e] = s;
-      }
-      st8(dst + ((size_t)rho * 2 + g.n) * POLY + g.tid * 8, o);
-    }
-    __syncthreads();
-  }
-}
-
-// ---- paired rounds, residue pipeline: the same arithmetic as k_expand_round_pair split the way k_fold_res is, so that
-// the transforms run in 256-thread single-modulus CTAs at 2 CTAs per SM instead of one 512-thread CTA per SM.
+// Row 1: the reference computes to_ntt(automorph(from_ntt(row 1))) (server.rs:80-88).  X -> X^t permutes the roots of
+// X^N + 1, so in the NTT domain the automorphism is a pure permutation of the evaluation slots: slot s holds the value at
+// psi^(2 br(s) + 1), and tau_t(a) there equals a at psi^((2 br(s) + 1) t).  The values are canonical residues either way,
+// so the gathered vector is bit-identical to the reference's.
+// Only CTA i touches v[i] and v[i + num_in], so the round stays in place.  The round runs as two kernels, the way k_fold_res
+// is split, so that the transforms run in 256-thread single-modulus CTAs at 2 CTAs per SM:
 //   k_expand_intt:       inverse transform of row 0 of every processed v[i], residues in coefficient order -> xr
 //   k_expand_round_res:  CTA (i, n): CRT lift (+ negacyclic shift for the second output) + automorphism + gadget digits
 //                        + forward transforms and key products modulo q_n; writes rows (., n) of v[i] and v[i + num_in].
@@ -871,7 +660,9 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
   uint32_t* vo = v + (size_t)(i + R.num_in) * 4 * POLY;
   if ((R.stop_round > 0 && R.r > R.stop_round && (i & 1)) ||
       (R.stop_round > 0 && R.r == R.stop_round && (i & 1) && (i / 2) >= R.max_bits_to_gen_right)) {
-    if (R.fill_skipped) {                                  // see k_expand_round_pair
+    // never read again by the query path; the reference still leaves v[i + num_in] = v[i] (.) neg1 there
+    // (server.rs:105-110 runs before the skip test), which the stage-level entry point reproduces
+    if (R.fill_skipped) {
       uint32_t nn[8];
       ld8_ro(nn, ng + g.tid * 8);
 #pragma unroll
@@ -944,7 +735,7 @@ k_expand_round_res(DevParams P, uint32_t* v, size_t v_stride, const uint32_t* __
       acc_room<2>(acc, cnt, 1, g);
       mac_digit<2>(acc, x, Wn + (size_t)kl * 2 * POLY, row_step);
     }
-    // row 1 automorphism = slot permutation (see k_expand_round); gather before any thread overwrites v[i]
+    // row 1 automorphism = slot permutation (see above); gather before any thread overwrites v[i]
     uint32_t yy[8];
 #pragma unroll
     for (int e = 0; e < 8; e++) {
@@ -1290,23 +1081,6 @@ void launch_folding_neg(const DevParams& P, uint32_t* out, const uint32_t* v_fol
                         cudaStream_t s) {
   size_t total = (size_t)count * 2 * 2 * t_gsw * 2 * POLY;
   if (total) ++g_kernel_launches, k_folding_neg<<<grid1d(total, 256), 256, 0, s>>>(P, out, v_folding, total, t_gsw, bits);
-}
-void launch_expand_scalar(const DevParams& P, uint32_t* v, size_t v_stride, int nq, int num_in, const uint32_t* neg1_r,
-                          cudaStream_t s) {
-  size_t total = (size_t)num_in * 4 * POLY;
-  ++g_kernel_launches;
-  k_expand_scalar<<<dim3(grid1d(total, 256), nq), 256, 0, s>>>(P, v, v_stride, num_in, neg1_r);
-}
-void launch_expand_round(const DevParams& P, uint32_t* v, size_t v_stride, int nq, const ExpandRound& R, cudaStream_t s) {
-  opt_in_smem(k_expand_round, (int)kDynSmemBig);
-  ++g_kernel_launches;
-  k_expand_round<<<dim3((unsigned)(2 * R.num_in), nq), CTA, kDynSmemBig, s>>>(P, v, v_stride, R);
-}
-void launch_expand_round_pair(const DevParams& P, uint32_t* v, size_t v_stride, int nq, const ExpandRound& R,
-                              const uint32_t* neg1_r, cudaStream_t s) {
-  opt_in_smem(k_expand_round_pair, (int)kDynSmemBig);
-  ++g_kernel_launches;
-  k_expand_round_pair<<<dim3((unsigned)R.num_in, nq), CTA, kDynSmemBig, s>>>(P, v, v_stride, R, neg1_r);
 }
 void launch_expand_round_res(const DevParams& P, uint32_t* v, size_t v_stride, uint32_t* xr, size_t xr_stride, int nq,
                              const ExpandRound& R, const uint32_t* neg1_r, cudaStream_t s) {

@@ -291,17 +291,9 @@ def test_worst_case_operands(t, version):
                 v = np.zeros((1 << P.g) * 2 * P.W, dtype=np.uint64)
                 v[: first.size] = first
                 ref = P.coefficient_expansion(v, pp)
-                for variant in (0, 2):
-                    for pair_min in (1, 1 << 30):
-                        G.set_option("expand_variant", variant)
-                        G.set_option("expand_pair_min_ctas", pair_min)
-                        got = v.copy()
-                        try:
-                            S.coefficient_expansion(G, gpp, got)
-                        finally:
-                            G.set_option("expand_variant", 0)
-                            G.set_option("expand_pair_min_ctas", 1)
-                        assert np.array_equal(got, ref), (t, version, pattern, variant, pair_min)
+                got = v.copy()
+                S.coefficient_expansion(G, gpp, got)
+                assert np.array_equal(got, ref), (t, version, pattern)
             # expand_query on raw ciphertexts of every coefficient q - 1, and of the non-canonical q
             for value in (q - 1, q):
                 ct = _raw(P, 2, value)

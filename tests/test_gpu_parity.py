@@ -207,8 +207,8 @@ def test_fold_and_folding_neg_match_oracle(name):
 
 
 # ------------------------------------------------------------------ expansion
-# expand_pair_min_ctas: rounds with at least that many active ciphertexts use the paired kernel (one CTA = both outputs
-# of an input, inverse transform shared through the negacyclic shift); 1 = every round, 1 << 30 = never, 8 = mixed
+# Every round is paired (one CTA = both outputs of an input, inverse transform shared through the negacyclic shift).
+# "expand_pair_min_ctas" and "expand_variant" once selected other schedules; they stay accepted and change nothing.
 @pytest.mark.parametrize("pair_min", [1, 8, 1 << 30])
 @pytest.mark.parametrize("name", CASES)
 def test_expand_query_matches_oracle(name, pair_min):
@@ -219,7 +219,7 @@ def test_expand_query_matches_oracle(name, pair_min):
     try:
         vreg, vf = S.expand_query(G, gpp, S.Query(ct=q["ct"]))
     finally:
-        G.set_option("expand_pair_min_ctas", 528)
+        G.set_option("expand_pair_min_ctas", 1)
     assert np.array_equal(vreg, vreg_ref)
     assert np.array_equal(vf, vf_ref)
 
@@ -227,7 +227,7 @@ def test_expand_query_matches_oracle(name, pair_min):
 @pytest.mark.parametrize("pair_min,variant", [(1, 0), (4, 0), (1, 2), (4, 2), (1 << 30, 0)])
 @pytest.mark.parametrize("name", ["T0", "T"])
 def test_coefficient_expansion_matches_oracle_all_slots(name, pair_min, variant):
-    # expand_variant 0: paired rounds as inverse-transform kernel + single-modulus CTAs; 2: paired rounds in one kernel
+    # every slot, including those the query path skips (fill_skipped)
     S, P, cl, pp, db, G, gdb, gpp = setup_case(name)
     q = cl.generate_query(9)
     v = np.zeros((1 << P.g) * 2 * P.W, dtype=np.uint64)
@@ -239,20 +239,24 @@ def test_coefficient_expansion_matches_oracle_all_slots(name, pair_min, variant)
     try:
         S.coefficient_expansion(G, gpp, got)
     finally:
-        G.set_option("expand_pair_min_ctas", 528)
+        G.set_option("expand_pair_min_ctas", 1)
         G.set_option("expand_variant", 0)
     assert np.array_equal(got, ref)
 
 
 def test_process_query_with_paired_expansion_everywhere():
+    # the retired kernel switches stay accepted and select nothing: every round is still paired, one kernel each
     S, P, cl, pp, db, G, gdb, gpp = setup_case("T")
     idxs = [1, 200, 33, 255, 128]
     qs = np.concatenate([cl.generate_query(i)["ct"] for i in idxs])
-    G.set_option("expand_pair_min_ctas", 1)
+    retired = {"expand_pair_min_ctas": (1 << 30, 1), "expand_variant": (1, 0), "intt_variant": (1, 0), "imma_variant": (1, 0)}
+    for k, (value, _) in retired.items():
+        G.set_option(k, value)
     try:
         out = S.process_query_batch(G, gpp, qs, gdb)
     finally:
-        G.set_option("expand_pair_min_ctas", 528)
+        for k, (_, default) in retired.items():
+            G.set_option(k, default)
     for k, i in enumerate(idxs):
         assert np.array_equal(out[k], P.process_query(pp, dict(ct=qs[k * 2 * P.N:(k + 1) * 2 * P.N]), db)), k
         assert np.array_equal(cl.decode_response(out[k]), P.db_plain_item(SEED_DB, i))
@@ -502,14 +506,13 @@ def test_imma_multiply_and_process_query_match_oracle(name):
     idxs = [0, 3, P.dim0 * P.num_per - 1, 17, 5, 9, 2, 11, 1, 30, 6]
     qs = np.concatenate([cl.generate_query(i)["ct"] for i in idxs])
     refs = [P.process_query(pp, dict(ct=qs[k * 2 * P.N:(k + 1) * 2 * P.N]), db) for k in range(len(idxs))]
-    # imma_variant 0 = cp.async-pipelined 8-query kernel (default), 1 = load-then-use kernel
+    # batch 8: the cp.async-pipelined 8-query kernel
     # batch 16: one pass of 11 queries on the four-column-tile kernel (third tile partly, fourth tile entirely padding)
-    for group, variant in ((4, 0), (8, 0), (8, 1), (16, 0)):
+    for group in (4, 8, 16):
         G.set_option("batch", group)
-        G.set_option("imma_variant", variant)
         out = S.process_query_batch(G, gpp, qs, fdb)
         for k in range(len(idxs)):
-            assert np.array_equal(out[k], refs[k]), (name, group, variant, k)
+            assert np.array_equal(out[k], refs[k]), (name, group, k)
     # 19 queries at batch 16: a full 16-query pass followed by a 3-query pass
     if name == "T":
         more = [7, 64, 100, 250, 12, 99, 180, 201]
@@ -521,7 +524,6 @@ def test_imma_multiply_and_process_query_match_oracle(name):
             kk = len(idxs) + k
             assert np.array_equal(out[kk], P.process_query(pp, dict(ct=qs2[kk * 2 * P.N:(kk + 1) * 2 * P.N]), db)), (name, "19", kk)
     G.set_option("batch", 16)
-    G.set_option("imma_variant", 0)
     # synthetic generator and item upsert in fragment order
     f2 = S.Database(G, fmt=1)
     f2.fill_synthetic(SEED_DB)
