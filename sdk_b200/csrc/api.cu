@@ -2180,7 +2180,7 @@ int b200pir_dpir_matvec_packed_dev(b200pir_dpir* m, const uint32_t* b_dev, uint3
 int b200pir_dpir_matvec_packed_rows(b200pir_dpir* m, uint64_t row_begin, uint64_t row_count, const uint32_t* b, uint32_t* out) {
   API_BEGIN
   if (!m || !b || !out) throw Error(B200PIR_E_BADARG, "null argument");
-  if (row_begin + row_count > m->rows) throw Error(B200PIR_E_SHAPE, "row range out of bounds");
+  if (row_begin > m->rows || row_count > m->rows - row_begin) throw Error(B200PIR_E_SHAPE, "row range out of bounds");
   if (row_count == 0) return 0;
   std::lock_guard<std::mutex> lk(m->mu);
   cudaSetDevice(m->device);

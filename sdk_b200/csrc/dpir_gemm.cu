@@ -76,14 +76,14 @@ struct GemmSmem {
   uint64_t full[G_STAGES], empty[G_STAGES];
 };
 
-// c[m][n] = sum_k a[m][k] b[k][n] mod 2^32 for one 128 x 32 tile per CTA (grid = (4 nt, mt))
+// c[m][n] = sum_k a[m][k] b[k][n] mod 2^32 for one 128 x 32 tile per CTA (grid = (4 nt, row tiles m_t0 .. m_t0 + gridDim.y - 1))
 __global__ void __launch_bounds__(G_THREADS, 1)
 k_dpir_gemm(const uint8_t* __restrict__ a_img, const uint8_t* __restrict__ b_img, uint32_t* __restrict__ c, size_t rows, size_t n_cols,
-            int mt, int nt, int ks) {
+            int mt, int nt, int ks, int m_t0) {
   extern __shared__ __align__(1024) uint8_t gsm[];
   GemmSmem* S = reinterpret_cast<GemmSmem*>(gsm + (size_t)G_STAGES * G_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_t = blockIdx.x >> 2, n_q = blockIdx.x & 3, m_t = blockIdx.y;
+  const int n_t = blockIdx.x >> 2, n_q = blockIdx.x & 3, m_t = m_t0 + (int)blockIdx.y;
   const size_t a_plane = (size_t)mt * ks * TC5_TILE, b_plane = (size_t)nt * ks * TC5_TILE;
   if (threadIdx.x == 0) {
     for (int s = 0; s < G_STAGES; s++) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 2); }
@@ -200,13 +200,19 @@ void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t 
   uint8_t *a_img = nullptr, *b_img = nullptr;
   B200_CUDA(cudaMalloc(&a_img, (size_t)2 * mt * ks * TC5_TILE));
   B200_CUDA(cudaMalloc(&b_img, (size_t)4 * nt * ks * TC5_TILE));
-  g_kernel_launches += 3;
+  g_kernel_launches += 2;
   k_gemm_a_image<<<blocks((size_t)mt * ks * 1024, 256), 256, 0, s>>>(a_img, a, rows, k_dim, mt, ks);
   k_gemm_b_image<<<blocks((size_t)nt * ks * 1024, 256), 256, 0, s>>>(b_img, b, k_dim, n_cols, nt, ks);
   const size_t smem = (size_t)G_STAGES * G_STAGE_BYTES + sizeof(GemmSmem) + 16;
   opt_in_smem(k_dpir_gemm, (int)smem);
-  k_dpir_gemm<<<dim3(4 * nt, mt), G_THREADS, smem, s>>>(a_img, b_img, c, rows, n_cols, mt, nt, ks);
-  cudaError_t e = cudaStreamSynchronize(s);
+  // gridDim.y is capped at 65535: more than 128 * 65535 rows take several launches
+  for (int m_t0 = 0; m_t0 < mt; m_t0 += 65535) {
+    ++g_kernel_launches;
+    k_dpir_gemm<<<dim3(4 * nt, std::min(mt - m_t0, 65535)), G_THREADS, smem, s>>>(a_img, b_img, c, rows, n_cols, mt, nt, ks, m_t0);
+  }
+  cudaError_t e = cudaGetLastError();
+  const cudaError_t se = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = se;
   cudaFree(a_img);
   cudaFree(b_img);
   if (e != cudaSuccess) throw Error(-3, std::string("dpir gemm: ") + cudaGetErrorString(e));

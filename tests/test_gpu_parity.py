@@ -654,7 +654,11 @@ def test_three_phase_multi_gpu_flow_equals_oracle(name, world, fmt):
 
 
 # ------------------------------------------------------------------ DoublePIR offline setup (doublepir.rs:76-108)
-@pytest.mark.parametrize("rows,kdim,cols", [(128, 32, 128), (45, 70, 33), (300, 257, 1024), (129, 1, 5)])
+@pytest.mark.parametrize("rows,kdim,cols", [(128, 32, 128), (45, 70, 33), (300, 257, 1024), (129, 1, 5),
+                                            # setup()'s GEMMs on real databases: h_1 = db a_1 (2048 k-steps through the
+                                            # 8-stage ring), h_2 = h_1' a_2 with K = l / x = 29 and 1
+                                            (29, 65536, 1024), (4096, 29, 1024), (16384, 1, 1024),
+                                            (257, 291, 389)])          # 3 x 4 tiles, 10 k-steps, every dimension ragged
 def test_dpir_matmul_limb_gemm_matches_oracle(rows, kdim, cols):
     """`&Matrix * &Matrix` (matrix/ops.rs:169-191) on the wgmma limb GEMM: small signed left operand (centred mod p, and the
     extremes -2^15 / 2^15 - 1), full 32-bit right operand including 0xffffffff; ragged shapes (zero padded tiles)."""
@@ -666,13 +670,17 @@ def test_dpir_matmul_limb_gemm_matches_oracle(rows, kdim, cols):
     b = rng.integers(0, 2**32, (kdim, cols), dtype=np.uint64).astype(np.uint32)
     b[0, 0] = 0xFFFFFFFF
     assert np.array_equal(D.matmul(a, b), O.dpir_mul(a, b, rows, kdim, cols))
-    with pytest.raises(D.B200PirError):
-        bad = a.copy()
-        bad[0, 0] = 40000
-        D.matmul(bad, b)
+    for v in (40000, 32768, -32769):
+        with pytest.raises(D.B200PirError):
+            bad = a.copy()
+            bad[0, 0] = np.int64(v).astype(np.uint32)
+            D.matmul(bad, b)
 
 
-@pytest.mark.parametrize("l,m,n,p,delta,x", [(24, 20, 8, 929, 4, 2), (256, 192, 64, 552, 4, 1), (96, 130, 1024, 1024, 4, 3)])
+@pytest.mark.parametrize("l,m,n,p,delta,x", [(24, 20, 8, 929, 4, 2), (256, 192, 64, 552, 4, 1), (96, 130, 1024, 1024, 4, 3),
+                                             # p = 2 (32 binary digits) and p = 1024; l / x mod 3 = 0, 1, 2; x = 8
+                                             (48, 50, 16, 2, 32, 8), (56, 33, 24, 2, 32, 8), (40, 70, 16, 1024, 4, 8),
+                                             (28, 40, 32, 1024, 4, 4)])
 def test_dpir_setup_matches_oracle(l, m, n, p, delta, x):
     """setup(): hint h_2 and the three server-state matrices (squished database, squished expanded h_1, padded transposed a_2)
     == the oracle's restatement, word for word."""

@@ -98,6 +98,36 @@ def mat_vec(a, v):                                                            # 
     return (a.astype(np.uint64) @ v.astype(np.uint64)).astype(np.uint32)      # wraps mod 2^64, then the low 32 bits
 
 
+# ---- the server's packed kernels, defined in numpy (uint64 sums masked to 32 bits) ---------------------------------------
+def unpack_fields(a, rows, cols):                                            # kernels.rs:9-12: 3 x 10 bits a word, bits 30-31 unused
+    w = np.asarray(a, dtype=np.uint64).reshape(rows, cols, 1)
+    return ((w >> (np.uint64(10) * np.arange(3, dtype=np.uint64))) & np.uint64(1023)).reshape(rows, 3 * cols)
+
+
+def np_matvec_packed(a, b, rows, cols):                                       # kernels.rs:14-178 matrix_mul_vec_packed
+    return ((unpack_fields(a, rows, cols) @ b.astype(np.uint64)) & np.uint64(0xFFFFFFFF)).astype(U32)
+
+
+def np_matrix_mul_transposed_packed(a, b, a_rows, a_cols, b_rows, b_cols):     # kernels.rs:180-278, both branches
+    bm = b.astype(np.uint64).reshape(b_rows, b_cols)[:, : 3 * a_cols]
+    return ((unpack_fields(a, a_rows, a_cols) @ bm.T) & np.uint64(0xFFFFFFFF)).astype(U32).reshape(-1)
+
+
+def np_transpose_expand_concat_cols_squish(a, rows, cols, modulus, delta, concat):   # matrix/indexing.rs:117-143, basis 10, d 3
+    out_rows, out_cols = cols * delta * concat, (rows // concat + 2) // 3
+    out = np.zeros((out_rows, out_cols), dtype=np.uint64)
+    val = np.asarray(a, dtype=np.uint64).reshape(rows, cols)
+    j = np.arange(rows, dtype=np.uint64)[:, None]
+    i = np.arange(cols, dtype=np.uint64)[None, :]
+    c = j // np.uint64(concat)
+    for f in range(delta):
+        r = (i * np.uint64(delta) + np.uint64(f)) + np.uint64(cols * delta) * (j % np.uint64(concat))
+        r, cd = np.broadcast_arrays(r, c // np.uint64(3))
+        np.add.at(out, (r.astype(np.int64), cd.astype(np.int64)), (val % np.uint64(modulus)) << (np.uint64(10) * (c % np.uint64(3))))
+        val //= np.uint64(modulus)
+    return (out & np.uint64(0xFFFFFFFF)).astype(U32).reshape(-1), out_rows, out_cols
+
+
 def query(i, a_1, a_2, prm, info, rng):                                       # doublepir.rs:111-160
     idx = i // info["packing"] if info["packing"] > 0 else i
     i1 = (idx // prm["m"]) * (info["ne"] // info["x"])
@@ -166,13 +196,18 @@ def recover(i, offline_h2, qmsg, answer, a_2, client, prm, info, batch_index=0):
 _prepared = {}
 
 
-def prepare(num_entries, bits, seed):
-    """pick_params, Db::with_data, init, setup (cached: the 2^24-entry setup is shared by two tests)"""
-    key = (num_entries, bits, seed)
+def prepare(num_entries, bits, seed, full_width=False):
+    """pick_params, Db::with_data, init, setup (cached: the 2^24-entry setup is shared by several tests).  full_width plants
+    values of all `bits` bits instead of bytes, so that entries wider than 8 bits have non-zero high base-p digits."""
+    full_width = full_width and bits > 8
+    key = (num_entries, bits, seed, full_width)
     if key not in _prepared:
         rng = np.random.default_rng(seed)
         prm = pick_params(num_entries, bits, SEC_PARAM, LOGQ)
-        data = rng.integers(0, min(1 << bits, 256), num_entries, dtype=np.uint8)   # the reference's iterator yields u8 items
+        if full_width:
+            data = rng.integers(0, 1 << bits, num_entries, dtype=np.uint64)
+        else:
+            data = rng.integers(0, min(1 << bits, 256), num_entries, dtype=np.uint8)   # the reference's iterator yields u8 items
         info, db = db_with_data(num_entries, bits, prm, data)
         n, l, m, p, x = prm["n"], prm["l"], prm["m"], prm["p"], info["x"]
         delta = math.ceil(LOGQ / math.log2(p))

@@ -166,6 +166,33 @@ def test_dpir_setup_restatement_against_its_definition():
     assert np.array_equal(O.dpir_mul(db, a1, l, m, n), ((db.astype(np.uint64) @ a1.astype(np.uint64)) & 0xFFFFFFFF).astype(np.uint32))
 
 
+def test_dpir_answer_tail_restatement_against_its_definition():
+    # answer()'s tail in the oracle (matrix_mul_transposed_packed, kernels.rs:180-278; transpose_expand_concat_cols_squish,
+    # indexing.rs:117-143) against the numpy definitions the GPU sweeps also use; words with bits 30 and 31 set, 0xffffffff
+    import test_oracle_doublepir_e2e as E
+    rng = np.random.default_rng(2)
+    for a_rows, a_cols, b_rows in [(24, 5, 8), (3, 40, 16), (1, 1, 8), (8, 150, 24)]:     # both of the reference's branches
+        a = rng.integers(0, 2**32, a_rows * a_cols, dtype=np.uint64).astype(np.uint32)
+        a[:a_cols] = 0xFFFFFFFF
+        b = rng.integers(0, 2**32, b_rows * 3 * a_cols, dtype=np.uint64).astype(np.uint32)
+        b[0] = 0xFFFFFFFF
+        assert np.array_equal(O.dpir_matrix_mul_transposed_packed(a, b, a_rows, a_cols, b_rows, 3 * a_cols),
+                              E.np_matrix_mul_transposed_packed(a, b, a_rows, a_cols, b_rows, 3 * a_cols)), (a_rows, a_cols)
+    for concat in (1, 2, 3, 4, 8):
+        for delta in (1, 2, 4, 5):
+            for modulus in (2, 3, 512, 991, 1024):
+                for rem in (0, 1, 2):
+                    rows, cols = concat * (6 + rem), 1 + rem
+                    a = rng.integers(0, 2**32, rows * cols, dtype=np.uint64).astype(np.uint32)
+                    a[: rows * cols // 2] = 0xFFFFFFFF
+                    o, orows, ocols = O.dpir_transpose_expand_concat_cols_squish(a, rows, cols, modulus, delta, concat)
+                    r, rr, rc = E.np_transpose_expand_concat_cols_squish(a, rows, cols, modulus, delta, concat)
+                    assert (orows, ocols) == (rr, rc) and np.array_equal(o, r), (concat, delta, modulus, rem)
+    a = rng.integers(0, 2**32, 9 * 4, dtype=np.uint64).astype(np.uint32)
+    b = rng.integers(0, 2**32, 12, dtype=np.uint64).astype(np.uint32)
+    assert np.array_equal(O.dpir_matvec_packed(a, b, 9, 4), E.np_matvec_packed(a, b, 9, 4))
+
+
 def test_oracle_reproduces_golden_fixtures():
     # tests/golden/spiral_golden.json was frozen from this oracle after the KAT pinning; any drift shows up here
     import json
