@@ -302,6 +302,49 @@ int b200pir_dpir_transpose_expand_concat_cols_squish(int device, const uint32_t*
                                                      uint64_t delta, uint64_t concat, uint32_t* out, uint64_t* out_rows,
                                                      uint64_t* out_cols);
 
+/* ---- DoublePIR offline load: raw entries -> database layout -> init() -> setup(), all in HBM ----------------------------- */
+/* Params {n, l, m, logq, p} as pick_params returned them (lib/doublepir/src/params/params.rs:5-15; sigma is not used here). */
+typedef struct {
+  uint64_t n, l, m, logq, p;
+} b200pir_dpir_params;
+/* DbInfo fields the layout depends on, plus Params::delta() (params.rs:21-23): packing = entries per Z_p element (0 when an
+ * entry takes several), ne = Z_p elements per entry, x (= ne: DbInfo::new's search starts at ne), delta = base-p digits of a
+ * 32-bit value. */
+typedef struct {
+  uint64_t packing, ne, x, delta;
+} b200pir_dpir_info;
+/* Keys of the two shared matrices (lib/doublepir/src/util/consts.rs:23-33): the first 16 bytes of SHA-256("blyss1") and of
+ * SHA-256("blyss2").  A_1 = derive(m x n, key 1), A_2 = derive((l/x) x n, key 2) (init(), doublepir.rs:46-51). */
+#define B200PIR_DPIR_SEED_A1 {0x9c, 0x22, 0x77, 0x85, 0x45, 0xac, 0x22, 0x97, 0x41, 0x90, 0x8e, 0x65, 0x2d, 0x33, 0x3a, 0x0f}
+#define B200PIR_DPIR_SEED_A2 {0x5f, 0xff, 0xc4, 0x82, 0xc7, 0x2a, 0x85, 0x4a, 0x10, 0x35, 0x9e, 0x9f, 0xa2, 0xf5, 0xe0, 0x7f}
+/* Entry formats of b200pir_dpir_load: one entry per byte (Db::load_data's Iterator<Item = u8>, database.rs:168-205), or eight
+ * entries per byte, least significant bit first (Db::load_data_fast's bits_from_byte, database.rs:1-19, :207-247). */
+#define B200PIR_DPIR_ENTRY_BYTES 0
+#define B200PIR_DPIR_ENTRY_BITS 1
+/* DbInfo::new (lib/doublepir/src/database/database.rs:58-90, num_db_entries :352-372, with f64 log2 / ceil as written) plus
+ * Params::delta().  Host only.  Zero entries or bits_per_entry outside [1, 63], null pointers or a zero n / l / m ->
+ * B200PIR_E_BADARG; logq != 32 or p outside [2, 1024] (the squish basis is 10 bits, database.rs:274) -> B200PIR_E_UNSUPPORTED;
+ * more Z_p elements than l * m (the reference's `assert!(db_elems <= params.l * params.m)`) -> B200PIR_E_SHAPE. */
+int b200pir_dpir_db_info(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, b200pir_dpir_info* out);
+/* Matrix::derive_from_seed(rows, cols, key) (matrix/matrix.rs:125-135, derive_with_aes matrix/derivation.rs:11-22) on the GPU,
+ * into the host buffer out (rows * cols u32): the AES-128 keystream in Ctr64BE mode, restarted every 64 KiB with
+ * IV = BE64(chunk index) || 0^8, read as little-endian u32 words. */
+int b200pir_dpir_derive_from_seed(int device, const uint8_t key[16], uint64_t rows, uint64_t cols, uint32_t* out);
+/* DoublePirServer::new + load_data / load_data_fast (doublepir/server.rs:160-165, 201-229): db_info as above, A_1 and A_2 derived
+ * on the device from the two keys above, the `len` bytes of `data` laid out as the l x m matrix (database.rs:168-247; BITS gives
+ * 8 len entries, including the trailing bits of the last byte), then setup() (doublepir.rs:76-108) as b200pir_dpir_setup.  The
+ * squished database stays in HBM: *db_out is a new handle of l x ceil(m/3) packed words for the matvec entry points.
+ * h1_squished, a2_t and h2 are host buffers shaped as b200pir_dpir_setup's.  Synchronous, on a stream of its own.
+ * Errors (no handle is returned and no device memory stays allocated): those of b200pir_dpir_db_info; null pointers, a bad
+ * device or an unknown entry_format -> B200PIR_E_BADARG; entries that would index past the l x m matrix (where the reference
+ * panics), or l not a multiple of x -> B200PIR_E_SHAPE; a laid-out word outside [-2^15, 2^15) (bytes far wider than
+ * bits_per_entry packed together; the setup GEMM's operand range) -> B200PIR_E_UNSUPPORTED. */
+int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                      const uint8_t* data, uint64_t len, int entry_format, b200pir_dpir** db_out, uint32_t* h1_squished,
+                      uint32_t* a2_t, uint32_t* h2);
+/* Reads a packed matrix back (rows * cols u32): the squished database server.rs:147-153 writes as `.dbp`. */
+int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out);
+
 #ifdef __cplusplus
 }
 #endif

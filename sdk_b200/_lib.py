@@ -19,6 +19,14 @@ class CParams(C.Structure):
                [("expand_queries", C.c_int32)]
 
 
+class DpirParams(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ("n", "l", "m", "logq", "p")]
+
+
+class DpirInfo(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ("packing", "ne", "x", "delta")]
+
+
 def _load():
     if not os.path.exists(SO_PATH):
         raise ImportError("sdk_b200: %s not found — build it with `python -m sdk_b200.build` "
@@ -104,6 +112,11 @@ def _load():
         "b200pir_dpir_transpose_expand_concat_cols_squish": (C.c_int, [C.c_int, u32p, C.c_uint64, C.c_uint64, C.c_uint64,
                                                                         C.c_uint64, C.c_uint64, u32p, C.POINTER(C.c_uint64),
                                                                         C.POINTER(C.c_uint64)]),
+        "b200pir_dpir_db_info": (C.c_int, [C.POINTER(DpirParams), C.c_uint64, C.c_uint64, C.POINTER(DpirInfo)]),
+        "b200pir_dpir_derive_from_seed": (C.c_int, [C.c_int, u8p, C.c_uint64, C.c_uint64, u32p]),
+        "b200pir_dpir_load": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, u8p, C.c_uint64, C.c_int,
+                                        C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_download": (C.c_int, [vp, u32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # raises AttributeError if the .so does not export a declared symbol

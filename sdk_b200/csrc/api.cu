@@ -2094,6 +2094,28 @@ int b200pir_dpir_create_synthetic(int device, uint64_t rows, uint64_t cols, uint
   *out = m;
   API_END
 }
+namespace {
+// doublepir.rs:76-108 setup() on device-resident inputs: db (l x m, centred), a1 (m x n), a2 (l/x x n).  db_squished is a device
+// buffer of l x ceil(m/3) words; h1_squished, a2_t and h2 are host buffers.  Synchronises s.
+void dpir_setup_dev(const uint32_t* d_db, const uint32_t* d_a1, const uint32_t* d_a2, uint64_t l, uint64_t m, uint64_t n, uint32_t p,
+                    uint64_t delta, uint64_t x, uint32_t* d_dbsq, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2, cudaStream_t s) {
+  const size_t lx = l / x, rows1 = n * delta * x, lx3 = lx + (3 - lx % 3) % 3;
+  DevBuf<uint32_t> d_h(l * n), d_hc(rows1 * lx), d_h2(rows1 * n);
+  DevBuf<uint32_t> d_h1sq(rows1 * ((lx + 2) / 3)), d_a2t(n * lx3);
+  launch_dpir_gemm(d_h.p, d_db, d_a1, l, m, n, s);                                       // h_1 = db.data * a_1
+  launch_dpir_transpose_expand_concat(d_hc.p, d_h.p, l, n, p, (int)delta, x, s);        // transpose, expand, concat_cols
+  launch_dpir_gemm(d_h2.p, d_hc.p, d_a2, rows1, lx, n, s);                               // h_2 = h_1 * a_2
+  launch_dpir_add_squish(d_dbsq, d_db, l, m, p / 2, s);                                  // db.data += p/2; db.squish()
+  launch_dpir_add_squish(d_h1sq.p, d_hc.p, rows1, lx, p / 2, s);                         // h_1 += p/2; squish
+  launch_dpir_pad_transpose(d_a2t.p, d_a2, lx, n, lx3, s);                               // a_2_copy
+  B200_CUDA(cudaMemcpyAsync(h1_squished, d_h1sq.p, d_h1sq.n * 4, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaMemcpyAsync(a2_t, d_a2t.p, d_a2t.n * 4, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaMemcpyAsync(h2, d_h2.p, d_h2.n * 4, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  B200_CUDA(cudaGetLastError());
+}
+}  // namespace
+
 // doublepir.rs:76-108 setup(): both matrix products on the tensor cores (dpir_gemm.cu), the rest as small kernels.  Host pointers.
 int b200pir_dpir_setup(int device, const uint32_t* db, uint64_t l, uint64_t m, const uint32_t* a1, uint64_t n, const uint32_t* a2,
                        uint32_t p, uint64_t delta, uint64_t x, uint32_t* db_squished, uint32_t* h1_squished, uint32_t* a2_t,
@@ -2109,22 +2131,13 @@ int b200pir_dpir_setup(int device, const uint32_t* db, uint64_t l, uint64_t m, c
   cudaStream_t s = nullptr;
   B200_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   try {
-    const size_t lx = l / x, rows1 = n * delta * x, lx3 = lx + (3 - lx % 3) % 3;
-    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n), d_h(l * n), d_hc(rows1 * lx), d_h2(rows1 * n);
-    DevBuf<uint32_t> d_dbsq(l * ((m + 2) / 3)), d_h1sq(rows1 * ((lx + 2) / 3)), d_a2t(n * lx3);
+    const size_t lx = l / x;
+    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n), d_dbsq(l * ((m + 2) / 3));
     B200_CUDA(cudaMemcpyAsync(d_db.p, db, l * m * 4, cudaMemcpyHostToDevice, s));
     B200_CUDA(cudaMemcpyAsync(d_a1.p, a1, m * n * 4, cudaMemcpyHostToDevice, s));
     B200_CUDA(cudaMemcpyAsync(d_a2.p, a2, lx * n * 4, cudaMemcpyHostToDevice, s));
-    launch_dpir_gemm(d_h.p, d_db.p, d_a1.p, l, m, n, s);                                   // h_1 = db.data * a_1
-    launch_dpir_transpose_expand_concat(d_hc.p, d_h.p, l, n, p, (int)delta, x, s);        // transpose, expand, concat_cols
-    launch_dpir_gemm(d_h2.p, d_hc.p, d_a2.p, rows1, lx, n, s);                             // h_2 = h_1 * a_2
-    launch_dpir_add_squish(d_dbsq.p, d_db.p, l, m, p / 2, s);                              // db.data += p/2; db.squish()
-    launch_dpir_add_squish(d_h1sq.p, d_hc.p, rows1, lx, p / 2, s);                         // h_1 += p/2; squish
-    launch_dpir_pad_transpose(d_a2t.p, d_a2.p, lx, n, lx3, s);                             // a_2_copy
+    dpir_setup_dev(d_db.p, d_a1.p, d_a2.p, l, m, n, p, delta, x, d_dbsq.p, h1_squished, a2_t, h2, s);
     B200_CUDA(cudaMemcpyAsync(db_squished, d_dbsq.p, d_dbsq.n * 4, cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaMemcpyAsync(h1_squished, d_h1sq.p, d_h1sq.n * 4, cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaMemcpyAsync(a2_t, d_a2t.p, d_a2t.n * 4, cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaMemcpyAsync(h2, d_h2.p, d_h2.n * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
     B200_CUDA(cudaGetLastError());
   } catch (...) { cudaStreamDestroy(s); throw; }
@@ -2232,6 +2245,128 @@ int b200pir_dpir_matvec_packed(b200pir_dpir* m, const uint32_t* b, uint32_t* out
   B200_CUDA(cudaMemcpyAsync(m->b.p, b, 3 * m->cols * 4, cudaMemcpyHostToDevice, m->stream));
   launch_dpir_matvec(m->out.p, m->a.p, m->b.p, m->rows, m->cols, 0, m->stream);
   B200_CUDA(cudaMemcpyAsync(out, m->out.p, m->rows * 4, cudaMemcpyDeviceToHost, m->stream));
+  B200_CUDA(cudaStreamSynchronize(m->stream));
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+// ---------------------------------------------------------------- DoublePIR offline load (dpir_load.cu)
+namespace {
+const uint8_t kDpirSeedA1[16] = B200PIR_DPIR_SEED_A1;
+const uint8_t kDpirSeedA2[16] = B200PIR_DPIR_SEED_A2;
+
+// DbInfo::new (database.rs:58-90) with num_db_entries (:352-372) and compute_num_entries_base_p (:345-350); Params::delta().
+// db_elems is num_db_entries' first value.
+b200pir_dpir_info dpir_info(const b200pir_dpir_params* prm, uint64_t num_entries, uint64_t bits, uint64_t* db_elems) {
+  if (!prm) throw Error(B200PIR_E_BADARG, "null argument");
+  if (num_entries == 0 || bits < 1 || bits > 63) throw Error(B200PIR_E_BADARG, "DbInfo: need entries > 0 and 1 <= bits_per_entry < 64");
+  if (!prm->n || !prm->l || !prm->m) throw Error(B200PIR_E_BADARG, "params: n, l and m must be positive");
+  if (prm->logq != 32) throw Error(B200PIR_E_UNSUPPORTED, "params: logq must be 32 (doublepir.rs:9)");
+  if (prm->p < 2 || prm->p > 1024) throw Error(B200PIR_E_UNSUPPORTED, "params: p must lie in [2, 2^10] (squish basis, database.rs:274)");
+  b200pir_dpir_info o;
+  const double log_p = std::log2((double)prm->p);
+  uint64_t elems;
+  if ((double)bits <= log_p) {                                   // pack several entries into one Z_p element
+    o.packing = (uint64_t)log_p / bits;
+    elems = (uint64_t)std::ceil((double)num_entries / (double)o.packing);
+    o.ne = 1;
+  } else {                                                       // several Z_p elements per entry
+    o.packing = 0;
+    o.ne = (uint64_t)std::ceil((double)bits / log_p);
+    if (num_entries > UINT64_MAX / o.ne) throw Error(B200PIR_E_SHAPE, "DbInfo: more Z_p elements than the database holds");
+    elems = num_entries * o.ne;
+  }
+  o.x = o.ne;                                                    // `while info.ne % info.x != 0 { info.x += 1 }` from x = ne
+  o.delta = (uint64_t)std::ceil((double)prm->logq / log_p);
+  if (prm->l > UINT64_MAX / prm->m || elems > prm->l * prm->m) throw Error(B200PIR_E_SHAPE, "DbInfo: more Z_p elements than l * m");
+  if (db_elems) *db_elems = elems;
+  return o;
+}
+int dpir_device(int device) {
+  int ndev = 0;
+  B200_CUDA(cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) throw Error(B200PIR_E_BADARG, "no such CUDA device (this library has no CPU path)");
+  B200_CUDA(cudaSetDevice(device));
+  return device;
+}
+struct DpirDeleter { void operator()(b200pir_dpir* m) const { b200pir_dpir_destroy(m); } };
+}  // namespace
+
+int b200pir_dpir_db_info(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, b200pir_dpir_info* out) {
+  API_BEGIN
+  if (!out) throw Error(B200PIR_E_BADARG, "null argument");
+  *out = dpir_info(params, num_entries, bits_per_entry, nullptr);
+  API_END
+}
+
+int b200pir_dpir_derive_from_seed(int device, const uint8_t key[16], uint64_t rows, uint64_t cols, uint32_t* out) {
+  API_BEGIN
+  if (!key || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  if (rows && cols > SIZE_MAX / 4 / rows) throw Error(B200PIR_E_SHAPE, "derive: matrix too large");
+  if (rows * cols == 0) return 0;
+  dpir_device(device);
+  cudaStream_t s = nullptr;
+  B200_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  try {
+    DevBuf<uint32_t> d(rows * cols);
+    launch_dpir_derive(d.p, d.n, dpir_aes_key(key), s);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(out, d.p, d.n * 4, cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));
+  } catch (...) { cudaStreamDestroy(s); throw; }
+  cudaStreamDestroy(s);
+  API_END
+}
+
+int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                      const uint8_t* data, uint64_t len, int entry_format, b200pir_dpir** db_out, uint32_t* h1_squished,
+                      uint32_t* a2_t, uint32_t* h2) {
+  API_BEGIN
+  if (!params || !data || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+  if (entry_format != B200PIR_DPIR_ENTRY_BYTES && entry_format != B200PIR_DPIR_ENTRY_BITS)
+    throw Error(B200PIR_E_BADARG, "unknown entry format");
+  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, nullptr);
+  const bool bits_format = entry_format == B200PIR_DPIR_ENTRY_BITS;
+  const uint64_t l = params->l, m = params->m, n = params->n, x = info.x;
+  const uint32_t p = (uint32_t)params->p;
+  if (bits_format && len > UINT64_MAX / 8) throw Error(B200PIR_E_SHAPE, "too many entries");
+  const uint64_t count = bits_format ? 8 * len : len;           // the number of items the reference's iterator yields
+  // where load_data would index past the matrix (and panic): the last packed element, or the last digit row of the last entry
+  if (info.packing ? (count + info.packing - 1) / info.packing > l * m : (count && ((count - 1) / m + 1) > l / info.ne))
+    throw Error(B200PIR_E_SHAPE, "the entries do not fit the l x m database");
+  if (l % x) throw Error(B200PIR_E_SHAPE, "l must be a multiple of x (concat_cols)");
+  dpir_device(device);
+  std::unique_ptr<b200pir_dpir, DpirDeleter> h(dpir_new(device, l, (m + 2) / 3));
+  cudaStream_t s = h->stream;
+  {
+    const size_t lx = l / x;
+    DevBuf<uint8_t> d_raw(len);
+    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n);
+    DevBuf<int> d_flag(1);
+    B200_CUDA(cudaMemsetAsync(d_flag.p, 0, sizeof(int), s));
+    if (len) B200_CUDA(cudaMemcpyAsync(d_raw.p, data, len, cudaMemcpyHostToDevice, s));
+    launch_dpir_derive(d_a1.p, d_a1.n, dpir_aes_key(kDpirSeedA1), s);              // init(): A_1 = derive(m x n, SEEDS_SHORT[0])
+    launch_dpir_derive(d_a2.p, d_a2.n, dpir_aes_key(kDpirSeedA2), s);              //         A_2 = derive(l/x x n, SEEDS_SHORT[1])
+    launch_dpir_layout(d_db.p, d_raw.p, count, bits_format, l, m, (uint32_t)info.packing, (uint32_t)bits_per_entry,
+                       (uint32_t)info.ne, p, d_flag.p, s);
+    B200_CUDA(cudaGetLastError());
+    int flag = 0;
+    B200_CUDA(cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));
+    if (flag) throw Error(B200PIR_E_UNSUPPORTED, "load: a packed database word lies outside [-2^15, 2^15) (entries far wider than bits_per_entry)");
+    d_raw.release();
+    dpir_setup_dev(d_db.p, d_a1.p, d_a2.p, l, m, n, p, info.delta, x, h->a.p, h1_squished, a2_t, h2, s);
+  }
+  *db_out = h.release();
+  API_END
+}
+
+int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out) {
+  API_BEGIN
+  if (!m || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  std::lock_guard<std::mutex> lk(m->mu);
+  cudaSetDevice(m->device);
+  B200_CUDA(cudaMemcpyAsync(out, m->a.p, m->rows * m->cols * 4, cudaMemcpyDeviceToHost, m->stream));
   B200_CUDA(cudaStreamSynchronize(m->stream));
   B200_CUDA(cudaGetLastError());
   API_END

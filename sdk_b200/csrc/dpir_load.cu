@@ -1,0 +1,177 @@
+// DoublePIR offline load on the GPU: the shared matrices derived from their seeds, and raw entries laid out as the database
+// matrix, both straight into HBM (DoublePirServer::new + load_data / load_data_fast, lib/doublepir/src/doublepir/server.rs:160-165,
+// 201-229).  setup() then runs on these device buffers (dpir_gemm.cu), so nothing the load produces crosses PCIe but the hint.
+//
+// k_dpir_derive: Matrix::derive_from_seed (matrix/matrix.rs:125-135) = derive_with_aes (matrix/derivation.rs:11-22): the
+// matrix's bytes are the AES-128 keystream in Ctr64BE mode, restarted every 64 KiB chunk with IV = BE64(chunk) || 0^8, i.e.
+// block b of the matrix encrypts BE64(b / 4096) || BE64(b % 4096).  u32 words are read little-endian from the keystream.
+// One thread per 16-byte block; T-tables (FIPS-197 section 5.2.1's round as four 32-bit table lookups per column) in shared
+// memory.  The lookups are data-dependent, so this is NOT constant-time: that is fine here, because the key and the output are
+// public (the reference derives public matrices only, matrix.rs:120-124) and nothing secret ever passes through this kernel.
+//
+// k_dpir_layout: Db::load_data / load_data_fast (database/database.rs:168-247) as a gather, one thread per word of the l x m
+// matrix, then "Map DB elems to [-p/2; p/2]" (the wrapping subtraction of p/2 from every word, touched or not).
+#include "kernels.h"
+
+namespace b200pir {
+
+namespace {
+
+// ---- AES-128 (FIPS-197) on the host: the S-box from its definition (section 5.1.1: multiplicative inverse in GF(2^8), then
+// the affine map), the key expansion (section 5.2) and the encryption T-table Te0 (Te1..Te3 are its byte rotations)
+uint8_t gf_mul(uint8_t a, uint8_t b) {
+  uint8_t r = 0;
+  while (b) {
+    if (b & 1) r ^= a;
+    a = (uint8_t)((a << 1) ^ ((a & 0x80) ? 0x1b : 0));
+    b >>= 1;
+  }
+  return r;
+}
+void aes_sbox(uint8_t s[256]) {
+  for (int x = 0; x < 256; x++) {
+    uint8_t inv = 0;
+    for (int y = 1; y < 256 && x; y++)
+      if (gf_mul((uint8_t)x, (uint8_t)y) == 1) { inv = (uint8_t)y; break; }
+    uint8_t v = inv, r = inv;
+    for (int i = 0; i < 4; i++) { r = (uint8_t)((r << 1) | (r >> 7)); v ^= r; }
+    s[x] = (uint8_t)(v ^ 0x63);
+  }
+}
+
+__device__ __forceinline__ uint32_t ror8(uint32_t v, int n) { return __funnelshift_r(v, v, n); }
+
+// grid-stride over the 16-byte blocks of an out_words-word matrix
+__global__ void __launch_bounds__(256) k_dpir_derive(uint32_t* __restrict__ out, size_t out_words, const __grid_constant__ DpirAesKey key) {
+  __shared__ uint32_t te[4][256];
+  __shared__ uint32_t sb[256];
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+    const uint32_t t = key.te0[i];
+    te[0][i] = t; te[1][i] = ror8(t, 8); te[2][i] = ror8(t, 16); te[3][i] = ror8(t, 24);
+    sb[i] = key.sbox[i];
+  }
+  __syncthreads();
+  const size_t blocks = (out_words + 3) / 4;
+  for (size_t b = (size_t)blockIdx.x * blockDim.x + threadIdx.x; b < blocks; b += (size_t)gridDim.x * blockDim.x) {
+    // derive_with_aes_at(key, i as u32, chunk): the chunk index is cast to u32 before it is widened into the IV
+    const uint64_t chunk = (uint32_t)(b >> 12), ctr = b & 4095;
+    // state columns as big-endian words (FIPS-197 section 3.4), round key 0 added
+    uint32_t s0 = (uint32_t)(chunk >> 32) ^ key.rk[0], s1 = (uint32_t)chunk ^ key.rk[1];
+    uint32_t s2 = (uint32_t)(ctr >> 32) ^ key.rk[2], s3 = (uint32_t)ctr ^ key.rk[3];
+#pragma unroll
+    for (int r = 1; r < 10; r++) {
+      const uint32_t t0 = te[0][s0 >> 24] ^ te[1][(s1 >> 16) & 255] ^ te[2][(s2 >> 8) & 255] ^ te[3][s3 & 255] ^ key.rk[4 * r];
+      const uint32_t t1 = te[0][s1 >> 24] ^ te[1][(s2 >> 16) & 255] ^ te[2][(s3 >> 8) & 255] ^ te[3][s0 & 255] ^ key.rk[4 * r + 1];
+      const uint32_t t2 = te[0][s2 >> 24] ^ te[1][(s3 >> 16) & 255] ^ te[2][(s0 >> 8) & 255] ^ te[3][s1 & 255] ^ key.rk[4 * r + 2];
+      const uint32_t t3 = te[0][s3 >> 24] ^ te[1][(s0 >> 16) & 255] ^ te[2][(s1 >> 8) & 255] ^ te[3][s2 & 255] ^ key.rk[4 * r + 3];
+      s0 = t0; s1 = t1; s2 = t2; s3 = t3;
+    }
+    uint32_t o[4];
+    // last round: SubBytes, ShiftRows, AddRoundKey (no MixColumns)
+    o[0] = (sb[s0 >> 24] << 24 | sb[(s1 >> 16) & 255] << 16 | sb[(s2 >> 8) & 255] << 8 | sb[s3 & 255]) ^ key.rk[40];
+    o[1] = (sb[s1 >> 24] << 24 | sb[(s2 >> 16) & 255] << 16 | sb[(s3 >> 8) & 255] << 8 | sb[s0 & 255]) ^ key.rk[41];
+    o[2] = (sb[s2 >> 24] << 24 | sb[(s3 >> 16) & 255] << 16 | sb[(s0 >> 8) & 255] << 8 | sb[s1 & 255]) ^ key.rk[42];
+    o[3] = (sb[s3 >> 24] << 24 | sb[(s0 >> 16) & 255] << 16 | sb[(s1 >> 8) & 255] << 8 | sb[s2 & 255]) ^ key.rk[43];
+    // keystream bytes 4w..4w+3 are big-endian column w; the matrix reads them as a little-endian u32.  The last block may
+    // be partial (rows * cols * 4 is a multiple of 4 only): its words past the end are not written.
+    if (4 * b + 4 <= out_words) {
+      *reinterpret_cast<uint4*>(out + 4 * b) = make_uint4(__byte_perm(o[0], 0, 0x0123), __byte_perm(o[1], 0, 0x0123),
+                                                          __byte_perm(o[2], 0, 0x0123), __byte_perm(o[3], 0, 0x0123));
+    } else {
+      for (int w = 0; w < 4 && 4 * b + w < out_words; w++) out[4 * b + w] = __byte_perm(o[w], 0, 0x0123);
+    }
+  }
+}
+
+// entry i of the input: a byte (load_data's Iterator<Item = u8>) or bit i % 8 of byte i / 8 (load_data_fast's bits_from_byte,
+// least significant bit first)
+template <bool BITS>
+__device__ __forceinline__ uint32_t entry(const uint8_t* __restrict__ data, size_t i) {
+  if (BITS) return (data[i >> 3] >> (i & 7)) & 1u;
+  return data[i];
+}
+
+// word k of the l x m matrix (row-major, k = row * m + col), then minus p/2.  `count` = number of entries the iterator yields.
+//   packing > 0: element k = sum_t e_{k packing + t} * coeff_t, coeff_0 = 1, coeff_{t+1} = coeff_t * 2^bits (wrapping u32, no
+//                masking: an entry wider than `bits` spills into the next field); the last group may be partial
+//                (the `iter.peek().is_none()` flush).
+//   packing = 0: data[(i / m) ne + j][i % m] = base_p(p, e_i, j), so word (row, col) holds digit row % ne of entry
+//                (row / ne) m + col.
+// Sets *out_of_range when a centred word lies outside [-2^15, 2^15), the operand range of the setup GEMM (dpir_gemm.cu).
+template <bool BITS>
+__global__ void k_dpir_layout(uint32_t* __restrict__ db, const uint8_t* __restrict__ data, size_t count, size_t l, size_t m,
+                              uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p, int* __restrict__ out_of_range) {
+  const size_t words = l * m;
+  bool bad = false;
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < words; k += (size_t)gridDim.x * blockDim.x) {
+    uint32_t v = 0;
+    if (packing) {
+      const size_t first = k * packing;
+      if (first < count) {
+        uint32_t coeff = 1;
+        const size_t last = first + packing < count ? first + packing : count;
+        for (size_t i = first; i < last; i++) {
+          v += entry<BITS>(data, i) * coeff;
+          coeff *= 1u << bits;
+        }
+      }
+    } else {
+      const size_t row = k / m, col = k - row * m;
+      const size_t i = (row / ne) * m + col;
+      if (i < count) {
+        uint32_t e = entry<BITS>(data, i);
+        for (uint32_t j = row % ne; j; j--) e /= p;                   // base_p (arith.rs:16-22)
+        v = e % p;
+      }
+    }
+    v -= p / 2;
+    db[k] = v;
+    bad |= (int32_t)v < -32768 || (int32_t)v > 32767;
+  }
+  if (bad) atomicOr(out_of_range, 1);
+}
+
+unsigned grid_for(size_t items, int block) {
+  const size_t need = (items + block - 1) / block;
+  return (unsigned)std::min<size_t>(need ? need : 1, 132 * 32);
+}
+
+}  // namespace
+
+DpirAesKey dpir_aes_key(const uint8_t key[16]) {
+  DpirAesKey k;
+  aes_sbox(k.sbox);
+  for (int i = 0; i < 4; i++) k.rk[i] = (uint32_t)key[4 * i] << 24 | (uint32_t)key[4 * i + 1] << 16 | (uint32_t)key[4 * i + 2] << 8 | key[4 * i + 3];
+  uint8_t rcon = 1;
+  for (int i = 4; i < 44; i++) {                          // FIPS-197 section 5.2 KeyExpansion, Nk = 4
+    uint32_t t = k.rk[i - 1];
+    if (i % 4 == 0) {
+      t = (t << 8) | (t >> 24);                           // RotWord
+      t = (uint32_t)k.sbox[t >> 24] << 24 | (uint32_t)k.sbox[(t >> 16) & 255] << 16 | (uint32_t)k.sbox[(t >> 8) & 255] << 8 |
+          k.sbox[t & 255];                                // SubWord
+      t ^= (uint32_t)rcon << 24;
+      rcon = gf_mul(rcon, 2);
+    }
+    k.rk[i] = k.rk[i - 4] ^ t;
+  }
+  for (int x = 0; x < 256; x++) {                         // column (2s, s, s, 3s) of MixColumns applied to S-box output s
+    const uint8_t s = k.sbox[x];
+    k.te0[x] = (uint32_t)gf_mul(s, 2) << 24 | (uint32_t)s << 16 | (uint32_t)s << 8 | gf_mul(s, 3);
+  }
+  return k;
+}
+
+void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cudaStream_t s) {
+  ++g_kernel_launches;
+  k_dpir_derive<<<grid_for((words + 3) / 4, 256), 256, 0, s>>>(out, words, key);
+}
+
+void launch_dpir_layout(uint32_t* db, const uint8_t* data, size_t count, bool bits_format, size_t l, size_t m, uint32_t packing,
+                        uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range, cudaStream_t s) {
+  ++g_kernel_launches;
+  const unsigned g = grid_for(l * m, 256);
+  if (bits_format) k_dpir_layout<true><<<g, 256, 0, s>>>(db, data, count, l, m, packing, bits, ne, p, out_of_range);
+  else k_dpir_layout<false><<<g, 256, 0, s>>>(db, data, count, l, m, packing, bits, ne, p, out_of_range);
+}
+
+}  // namespace b200pir

@@ -209,4 +209,15 @@ void launch_dpir_add_squish(uint32_t* out, const uint32_t* m, size_t rows, size_
 // rows padded with zeros to rows3, then transposed (doublepir.rs:96-100)
 void launch_dpir_pad_transpose(uint32_t* out, const uint32_t* a, size_t rows, size_t cols, size_t rows3, cudaStream_t s);
 
+// ---- DoublePIR offline load (dpir_load.cu)
+// AES-128 expanded on the host (FIPS-197): round keys as big-endian column words, the S-box and the T-table Te0
+struct DpirAesKey { uint32_t rk[44]; uint32_t te0[256]; uint8_t sbox[256]; };
+DpirAesKey dpir_aes_key(const uint8_t key[16]);
+// Matrix::derive_from_seed (matrix.rs:125-135, derivation.rs:11-22): out[0 .. words) = the AES-128-Ctr64BE keystream, 64 KiB chunks
+void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cudaStream_t s);
+// Db::load_data (bits_format false) / load_data_fast (true), database.rs:168-247: `count` entries of `data` -> the l x m matrix
+// minus p/2 (every word written); *out_of_range |= 1 when a word lies outside the setup GEMM's [-2^15, 2^15)
+void launch_dpir_layout(uint32_t* db, const uint8_t* data, size_t count, bool bits_format, size_t l, size_t m, uint32_t packing,
+                        uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range, cudaStream_t s);
+
 }  // namespace b200pir

@@ -3,7 +3,12 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import LIB, check, B200PirError  # noqa: F401
+from ._lib import LIB, check, B200PirError, DpirParams, DpirInfo  # noqa: F401
+
+# init()'s keys (util/consts.rs:23-33): the first 16 bytes of SHA-256("blyss1") and of SHA-256("blyss2")
+SEED_A1 = bytes.fromhex("9c22778545ac229741908e652d333a0f")
+SEED_A2 = bytes.fromhex("5fffc482c72a854a10359e9fa2f5e07f")
+ENTRY_BYTES, ENTRY_BITS = 0, 1          # load_data's one entry a byte / load_data_fast's eight a byte, LSB first
 
 
 class PackedMatrix:
@@ -18,6 +23,18 @@ class PackedMatrix:
         else:
             check(LIB.b200pir_dpir_create_synthetic(device, rows, cols, int(synthetic_seed), C.byref(h)))
         self._h, self.rows, self.cols = h, rows, cols
+
+    @classmethod
+    def _adopt(cls, h, rows, cols):
+        m = cls.__new__(cls)
+        m._h, m.rows, m.cols = h, rows, cols
+        return m
+
+    def download(self):
+        """The packed words back from HBM (rows x cols u32): what server.rs:147-153 saves as `.dbp`."""
+        out = np.zeros((self.rows, self.cols), dtype=np.uint32)
+        check(LIB.b200pir_dpir_download(self._h, out.ctypes.data))
+        return out
 
     def close(self):
         if getattr(self, "_h", None):
@@ -124,3 +141,44 @@ def setup(db, a1, a2, p, delta, x, device=0):
                                  out["db_squished"].ctypes.data, out["h1_squished"].ctypes.data, out["a2_t"].ctypes.data,
                                  out["h2"].ctypes.data))
     return out
+
+
+def _params(params):
+    return DpirParams(*(int(params[k]) for k in ("n", "l", "m", "logq", "p")))
+
+
+def db_info(params, num_entries, bits_per_entry):
+    """DbInfo::new (database.rs:58-90) + Params::delta(): dict(packing, ne, x, delta).  params: dict with n, l, m, logq, p
+    (pick_params' values)."""
+    out = DpirInfo()
+    check(LIB.b200pir_dpir_db_info(C.byref(_params(params)), num_entries, bits_per_entry, C.byref(out)))
+    return dict(packing=out.packing, ne=out.ne, x=out.x, delta=out.delta)
+
+
+def derive_from_seed(rows, cols, key, device=0):
+    """Matrix::derive_from_seed (matrix.rs:125-135) computed on the GPU: rows x cols u32."""
+    key = bytes(key)
+    if len(key) != 16:
+        raise ValueError("key must be 16 bytes")
+    out = np.zeros((rows, cols), dtype=np.uint32)
+    check(LIB.b200pir_dpir_derive_from_seed(device, key, rows, cols, out.ctypes.data))
+    return out
+
+
+def load(params, num_entries, bits_per_entry, data, entry_format=ENTRY_BYTES, device=0):
+    """DoublePirServer::new + load_data (ENTRY_BYTES) / load_data_fast (ENTRY_BITS) + setup() on the GPU (server.rs:160-165,
+    201-229): A_1 and A_2 are derived from SEED_A1 / SEED_A2 on the device.  data: the raw bytes.  Returns
+    (PackedMatrix of the squished database, resident in HBM; dict(h1_squished, a2_t, h2); db_info dict)."""
+    info = db_info(params, num_entries, bits_per_entry)
+    data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
+    n, l, m = int(params["n"]), int(params["l"]), int(params["m"])
+    x, delta = info["x"], info["delta"]
+    lx = l // x
+    rows1 = n * delta * x
+    out = dict(h1_squished=np.zeros((rows1, (lx + 2) // 3), dtype=np.uint32), a2_t=np.zeros((n, lx + (3 - lx % 3) % 3), dtype=np.uint32),
+               h2=np.zeros((rows1, n), dtype=np.uint32))
+    h = C.c_void_p()
+    check(LIB.b200pir_dpir_load(device, C.byref(_params(params)), num_entries, bits_per_entry, data.ctypes.data, data.size,
+                                entry_format, C.byref(h), out["h1_squished"].ctypes.data, out["a2_t"].ctypes.data,
+                                out["h2"].ctypes.data))
+    return PackedMatrix._adopt(h, l, (m + 2) // 3), out, info
