@@ -345,6 +345,46 @@ int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t nu
 /* Reads a packed matrix back (rows * cols u32): the squished database server.rs:147-153 writes as `.dbp`. */
 int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out);
 
+/* ---- DoublePIR online: answer() served from HBM ---------------------------------------------------------------------------- */
+typedef struct b200pir_dpir_server b200pir_dpir_server;
+/* matrix_mul_vec_packed (kernels.rs:118-178) for `count` vectors in one pass over the matrix: b = count x 3*cols u32, out =
+ * count x rows u32, host buffers, on the handle's stream.  Null pointers -> B200PIR_E_BADARG. */
+int b200pir_dpir_matvec_packed_many(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out);
+/* The state DoublePirServer::answer reads (doublepir/server.rs:201-247): `db` (borrowed: the handle of b200pir_dpir_load, or
+ * b200pir_dpir_create of a `.dbp`, or of one chunk's rows for a chunked server; it must outlive the server) plus server_state =
+ * [h_1, a_2^T] (doublepir.rs:104-106) as b200pir_dpir_load / b200pir_dpir_setup return them, uploaded once: h1_squished
+ * (n delta x) x ceil((l/x)/3), a2_t n x 3 ceil((l/x)/3).  p, delta, x and ne come from b200pir_dpir_db_info(params, num_entries,
+ * bits_per_entry).  The server owns a non-blocking stream, a mutex that serialises its calls, and a workspace for max_queries
+ * queries per call (the total over all requests of an answer_many).  Errors: those of b200pir_dpir_db_info (which here also takes
+ * bits_per_entry = 64: the server lays out no entries); null pointers, a bad
+ * device or max_queries == 0 -> B200PIR_E_BADARG; db with cols != ceil(m/3) or more than l rows, or l not a multiple of x ->
+ * B200PIR_E_SHAPE. */
+int b200pir_dpir_server_create(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                               b200pir_dpir* db, const uint32_t* h1_squished, const uint32_t* a2_t, size_t max_queries,
+                               b200pir_dpir_server** out);
+void b200pir_dpir_server_destroy(b200pir_dpir_server* s);
+/* The response length of `request` (Vec<State>::serialize(), serializer.rs): 4 + 8 + 4 delta x n + queries * ne/x * (16 +
+ * 4 (n delta x) + 4 delta x).  Checks the framing and the q_2 shapes (the checks that do not depend on the chunk). */
+int b200pir_dpir_answer_size(b200pir_dpir_server* s, const uint8_t* request, size_t len, size_t* out_len);
+/* DoublePirServer::answer (server.rs:235-247) when chunk_idx < 0; answer_inline(request, data, Some(chunk_idx))
+ * (server.rs:167-180) when chunk_idx >= 0, the server's matrix being `data`: batch chunk_idx's rows are rows [0, batch size) of
+ * it (doublepir.rs:270-279) and the other batches contribute zero rows.  out receives msg.serialize(); *out_len is its capacity
+ * on entry and the response length on return.  Row batches, message order and byte order are answer()'s and serializer.rs's.
+ * Where the reference panics, B200PIR_E_SHAPE and nothing is written: a header or data word past the end, a count, rows or
+ * cols >= 2^28, zero queries, a query with fewer than 1 + ne/x matrices, a q_1 / q_2 whose rows are not 3 x the packed columns
+ * or whose cols != 1, a chunk index >= the query count, a batch needing more rows than the server holds (an unchunked answer
+ * needs all l).  More than max_queries queries -> B200PIR_E_SHAPE (the limit in b200pir_last_error()); null pointers or
+ * *out_len below the response length -> B200PIR_E_BADARG.  Matrices past the first 1 + ne/x of a query and trailing bytes are
+ * ignored, as deserialize_iter ignores them.  The server stays usable after any error. */
+int b200pir_dpir_answer(b200pir_dpir_server* s, const uint8_t* request, size_t len, int64_t chunk_idx, uint8_t* out,
+                        size_t* out_len);
+/* `count` independent requests of different clients, unchunked, in one call: response i is byte for byte answer(requests[i]);
+ * the database is read once per pass of up to 16 requests and h_1 once per 16 q_2 vectors of the call.  out_lens[i]: capacity
+ * of outs[i] on entry, response length on return.  Errors as b200pir_dpir_answer (the query limit counts every request); on an
+ * error nothing is written to any output. */
+int b200pir_dpir_answer_many(b200pir_dpir_server* s, const uint8_t* const* requests, const size_t* lens, size_t count,
+                             uint8_t* const* outs, size_t* out_lens);
+
 #ifdef __cplusplus
 }
 #endif

@@ -117,6 +117,14 @@ def _load():
         "b200pir_dpir_load": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, u8p, C.c_uint64, C.c_int,
                                         C.POINTER(vp), u32p, u32p, u32p]),
         "b200pir_dpir_download": (C.c_int, [vp, u32p]),
+        "b200pir_dpir_matvec_packed_many": (C.c_int, [vp, u32p, C.c_size_t, u32p]),
+        "b200pir_dpir_server_create": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, vp, u32p, u32p, C.c_size_t,
+                                                 C.POINTER(vp)]),
+        "b200pir_dpir_server_destroy": (None, [vp]),
+        "b200pir_dpir_answer_size": (C.c_int, [vp, u8p, C.c_size_t, szp]),
+        "b200pir_dpir_answer": (C.c_int, [vp, u8p, C.c_size_t, C.c_int64, u8p, szp]),
+        "b200pir_dpir_answer_many": (C.c_int, [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_void_p),
+                                               C.POINTER(C.c_size_t)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # raises AttributeError if the .so does not export a declared symbol

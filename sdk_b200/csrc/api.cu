@@ -6,6 +6,7 @@
 #include "kernels.h"
 #include "ntt_tables.hpp"
 #include "update_body.hpp"
+#include "dpir_wire.hpp"
 #include "gadget.hpp"
 #include <cstdio>
 #include <cerrno>
@@ -2256,10 +2257,13 @@ const uint8_t kDpirSeedA1[16] = B200PIR_DPIR_SEED_A1;
 const uint8_t kDpirSeedA2[16] = B200PIR_DPIR_SEED_A2;
 
 // DbInfo::new (database.rs:58-90) with num_db_entries (:352-372) and compute_num_entries_base_p (:345-350); Params::delta().
-// db_elems is num_db_entries' first value.
-b200pir_dpir_info dpir_info(const b200pir_dpir_params* prm, uint64_t num_entries, uint64_t bits, uint64_t* db_elems) {
+// db_elems is num_db_entries' first value.  max_bits: 63 where entries are laid out; the server, which only needs the shape,
+// takes full 64-bit entries too.
+b200pir_dpir_info dpir_info(const b200pir_dpir_params* prm, uint64_t num_entries, uint64_t bits, uint64_t* db_elems,
+                            uint64_t max_bits = 63) {
   if (!prm) throw Error(B200PIR_E_BADARG, "null argument");
-  if (num_entries == 0 || bits < 1 || bits > 63) throw Error(B200PIR_E_BADARG, "DbInfo: need entries > 0 and 1 <= bits_per_entry < 64");
+  if (num_entries == 0 || bits < 1 || bits > max_bits)
+    throw Error(B200PIR_E_BADARG, "DbInfo: need entries > 0 and 1 <= bits_per_entry <= " + std::to_string(max_bits));
   if (!prm->n || !prm->l || !prm->m) throw Error(B200PIR_E_BADARG, "params: n, l and m must be positive");
   if (prm->logq != 32) throw Error(B200PIR_E_UNSUPPORTED, "params: logq must be 32 (doublepir.rs:9)");
   if (prm->p < 2 || prm->p > 1024) throw Error(B200PIR_E_UNSUPPORTED, "params: p must lie in [2, 2^10] (squish basis, database.rs:274)");
@@ -2367,6 +2371,323 @@ int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out) {
   std::lock_guard<std::mutex> lk(m->mu);
   cudaSetDevice(m->device);
   B200_CUDA(cudaMemcpyAsync(out, m->a.p, m->rows * m->cols * 4, cudaMemcpyDeviceToHost, m->stream));
+  B200_CUDA(cudaStreamSynchronize(m->stream));
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+// ---------------------------------------------------------------- DoublePIR online: answer() from HBM (dpir_serve.cu)
+struct b200pir_dpir_server {
+  int device = 0, sm_count = 0;
+  std::mutex mu;                 // calls stage through one workspace: serialised
+  cudaStream_t stream = nullptr;
+  b200pir_dpir* db = nullptr;    // borrowed
+  uint64_t n = 0, l = 0, p = 0, delta = 0, x = 0, e = 0;       // e = ne / x: q_2 vectors a query
+  uint64_t dx = 0, rows1 = 0, c1 = 0, lx3 = 0, dcols = 0;      // delta x; n delta x; packed cols of h_1 and a_1'; 3 c1; db cols
+  size_t max_queries = 0;
+  DevBuf<uint32_t> h1, a2t;      // server_state, resident
+  // workspace for max_queries queries (and as many requests): staged vectors + task tables (one upload), a_1 / a_1' / msg[0]
+  // per request, the responses in wire layout (one download)
+  size_t stage_cap = 0, resp_cap = 0, task_cap = 0, vec_cap = 0;
+  uint8_t* h_stage = nullptr;
+  uint8_t* h_resp = nullptr;
+  DevBuf<uint8_t> d_stage, d_resp;
+  DevBuf<uint32_t> d_a1, d_a1sq, d_msg0;
+  ~b200pir_dpir_server() {
+    if (h_stage) cudaFreeHost(h_stage);
+    if (h_resp) cudaFreeHost(h_resp);
+  }
+};
+
+namespace {
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+uint64_t ceil_div(uint64_t a, uint64_t b) { return (a + b - 1) / b; }
+
+struct DpirCall {               // one request of a call
+  const uint8_t* req;
+  DpirWireRequest w;
+  DpirResponseLayout L;
+  size_t resp_off = 0;          // byte offset of its response in d_resp
+  std::vector<const uint32_t*> q1, q2;   // device addresses of its staged vectors ([k], [k * e + j]); q1[k] null when not read
+};
+
+// Parse + the checks of doublepir.rs:246-350 for one request; chunk < 0: unchunked.
+int dpir_prepare_call(b200pir_dpir_server* S, const uint8_t* req, size_t len, int64_t chunk, DpirCall& c, std::string& err) {
+  c.req = req;
+  int rc = parse_dpir_request(req, len, S->e, S->c1, c.w, err);
+  if (!rc) rc = check_dpir_batches(c.w, S->l, S->db->rows, S->dcols, chunk, err);
+  c.L = DpirResponseLayout{c.w.queries, S->e, S->dx, S->n, S->rows1};
+  return rc;
+}
+
+// The passes of answer() for every request of `calls` on the server's stream; responses to outs[i].  Everything has been
+// checked; no allocation, no device-wide synchronisation, one upload and one download.
+void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t chunk, uint8_t* const* outs, size_t* out_lens) {
+  const size_t R = calls.size();
+  cudaStream_t s = S->stream;
+  // ---- stage the vectors the passes read (the request's bytes as they are: big-endian words, swapped by the kernels)
+  size_t off = 0;
+  auto stage = [&](const DpirCall& c, const DpirWireMat& m) {
+    const size_t bytes = (size_t)m.rows * 4;
+    if (off + bytes > S->stage_cap) throw Error(B200PIR_E_SHAPE, "dpir: staging overflow");
+    std::memcpy(S->h_stage + off, c.req + m.data_pos(), bytes);
+    const uint32_t* dev = reinterpret_cast<const uint32_t*>(S->d_stage.p + off);
+    off = align_up(off + bytes, 16);
+    return dev;
+  };
+  size_t resp_total = 0;
+  for (auto& c : calls) {
+    c.q1.assign(c.w.queries, nullptr);
+    c.q2.assign(c.w.queries * S->e, nullptr);
+    for (size_t k = 0; k < c.w.queries; k++) {
+      if (chunk < 0 || (uint64_t)chunk == k) c.q1[k] = stage(c, c.w.q1(k));
+      for (size_t j = 0; j < S->e; j++) c.q2[k * S->e + j] = stage(c, c.w.q2(k, j));
+    }
+    c.resp_off = resp_total;
+    resp_total += c.L.bytes();
+  }
+  if (resp_total > S->resp_cap) throw Error(B200PIR_E_SHAPE, "dpir: response workspace overflow");
+  // ---- task tables: database pass, h_1 pass, a_1' * q_2
+  std::vector<DpirMvTask> tasks;
+  std::vector<DpirMvVec> vecs;
+  uint8_t* resp = S->d_resp.p;
+  auto add_tiles = [&](const uint32_t* a, uint64_t rows, uint64_t cols, uint32_t vec0, uint32_t nv) {
+    for (uint64_t t0 = 0; t0 < rows; t0 += kDpirMvRows)
+      tasks.push_back(DpirMvTask{a + t0 * cols, (uint32_t)std::min<uint64_t>(kDpirMvRows, rows - t0), vec0, nv, (uint32_t)t0});
+  };
+  int vmax_db = 1, vmax_h1 = 1, vmax_a1 = 1;
+  if (chunk >= 0) {             // one request: batch `chunk` from rows [0, its size) of the server's matrix
+    const DpirCall& c = calls[0];
+    const uint64_t nq = c.w.queries, rows = dpir_batch_rows(S->l, nq, chunk);
+    vecs.push_back(DpirMvVec{c.q1[chunk], S->d_a1.p + dpir_batch_begin(S->l, nq, chunk)});
+    add_tiles(S->db->a.p, rows, S->dcols, 0, 1);
+  } else {                      // the rows cut at every request's batch boundaries: one q_1 per request in each segment
+    std::vector<uint64_t> cuts{0, S->l};
+    for (const auto& c : calls)
+      for (uint64_t k = 1; k < c.w.queries; k++) cuts.push_back(dpir_batch_begin(S->l, c.w.queries, k));
+    std::sort(cuts.begin(), cuts.end());
+    cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
+    for (size_t g = 0; g + 1 < cuts.size(); g++) {
+      const uint64_t s0 = cuts[g], s1 = cuts[g + 1];
+      for (size_t i0 = 0; i0 < R; i0 += kDpirMvMaxVecs) {
+        const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, R - i0);
+        for (size_t i = i0; i < i0 + nv; i++) {
+          const uint64_t nq = calls[i].w.queries, bs = S->l / nq;
+          const uint64_t k = bs ? std::min(s0 / bs, nq - 1) : nq - 1;
+          vecs.push_back(DpirMvVec{calls[i].q1[k], S->d_a1.p + i * S->l + s0});
+        }
+        vmax_db = std::max<int>(vmax_db, nv);
+        add_tiles(S->db->a.p + s0 * S->dcols, s1 - s0, S->dcols, vec0, nv);
+      }
+    }
+  }
+  const size_t t_h1 = tasks.size();
+  {
+    std::vector<DpirMvVec> all;
+    for (const auto& c : calls)
+      for (size_t k = 0; k < c.w.queries; k++)
+        for (size_t j = 0; j < S->e; j++)
+          all.push_back(DpirMvVec{c.q2[k * S->e + j], reinterpret_cast<uint32_t*>(resp + c.resp_off + c.L.a2_data(k, j))});
+    for (size_t v0 = 0; v0 < all.size(); v0 += kDpirMvMaxVecs) {
+      const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, all.size() - v0);
+      vecs.insert(vecs.end(), all.begin() + v0, all.begin() + v0 + nv);
+      vmax_h1 = std::max<int>(vmax_h1, nv);
+      add_tiles(S->h1.p, S->rows1, S->c1, vec0, nv);
+    }
+  }
+  const size_t t_a1 = tasks.size();
+  for (size_t i = 0; i < R; i++) {
+    const DpirCall& c = calls[i];
+    std::vector<DpirMvVec> mine;
+    for (size_t k = 0; k < c.w.queries; k++)
+      for (size_t j = 0; j < S->e; j++)
+        mine.push_back(DpirMvVec{c.q2[k * S->e + j], reinterpret_cast<uint32_t*>(resp + c.resp_off + c.L.h2_data(k, j))});
+    for (size_t v0 = 0; v0 < mine.size(); v0 += kDpirMvMaxVecs) {
+      const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, mine.size() - v0);
+      vecs.insert(vecs.end(), mine.begin() + v0, mine.begin() + v0 + nv);
+      vmax_a1 = std::max<int>(vmax_a1, nv);
+      add_tiles(S->d_a1sq.p + i * S->dx * S->c1, S->dx, S->c1, vec0, nv);
+    }
+  }
+  if (tasks.size() > S->task_cap || vecs.size() > S->vec_cap) throw Error(B200PIR_E_SHAPE, "dpir: task table overflow");
+  const size_t off_tasks = off, off_vecs = align_up(off_tasks + tasks.size() * sizeof(DpirMvTask), 16);
+  const size_t used = off_vecs + vecs.size() * sizeof(DpirMvVec);
+  if (used > S->stage_cap) throw Error(B200PIR_E_SHAPE, "dpir: staging overflow");
+  std::memcpy(S->h_stage + off_tasks, tasks.data(), tasks.size() * sizeof(DpirMvTask));
+  std::memcpy(S->h_stage + off_vecs, vecs.data(), vecs.size() * sizeof(DpirMvVec));
+  const DpirMvTask* d_tasks = reinterpret_cast<const DpirMvTask*>(S->d_stage.p + off_tasks);
+  const DpirMvVec* d_vecs = reinterpret_cast<const DpirMvVec*>(S->d_stage.p + off_vecs);
+  // ---- the passes
+  B200_CUDA(cudaMemcpyAsync(S->d_stage.p, S->h_stage, used, cudaMemcpyHostToDevice, s));
+  B200_CUDA(cudaMemsetAsync(S->d_a1.p, 0, R * S->l * 4, s));   // split-k partial sums add into it; unread batches stay zero
+  launch_dpir_matvec_multi(d_tasks, t_h1, d_vecs, S->dcols, vmax_db, dpir_mv_ksplit(t_h1, S->dcols, S->sm_count), DPIR_MV_B_BE, s);
+  for (size_t i = 0; i < R; i++)        // a_1.transpose_expand_concat_cols_squish(p, delta, x, 10, 3)
+    launch_dpir_transpose_expand(S->d_a1sq.p + i * S->dx * S->c1, S->d_a1.p + i * S->l, S->l, 1, S->p, S->delta, S->x, S->dx,
+                                 S->c1, s);
+  // msg[0] = matrix_mul_transposed_packed(a_1', a_2^T) of every request at once (their a_1' are stacked)
+  launch_dpir_mul_transposed(S->d_msg0.p, S->d_a1sq.p, S->a2t.p, R * S->dx, S->c1, S->n, S->lx3, s);
+  for (size_t i = 0; i < R; i++)
+    launch_dpir_bswap(reinterpret_cast<uint32_t*>(resp + calls[i].resp_off + calls[i].L.msg0_data()), S->d_msg0.p + i * S->dx * S->n,
+                      S->dx * S->n, s);
+  launch_dpir_matvec_multi(d_tasks + t_h1, t_a1 - t_h1, d_vecs, S->c1, vmax_h1, 1, DPIR_MV_B_BE | DPIR_MV_OUT_BE, s);
+  launch_dpir_matvec_multi(d_tasks + t_a1, tasks.size() - t_a1, d_vecs, S->c1, vmax_a1, 1, DPIR_MV_B_BE | DPIR_MV_OUT_BE, s);
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaMemcpyAsync(S->h_resp, S->d_resp.p, resp_total, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  B200_CUDA(cudaGetLastError());
+  for (size_t i = 0; i < R; i++) {
+    const DpirCall& c = calls[i];
+    std::memcpy(outs[i], S->h_resp + c.resp_off, c.L.bytes());
+    write_dpir_response_headers(c.L, outs[i]);
+    out_lens[i] = c.L.bytes();
+  }
+}
+}  // namespace
+
+int b200pir_dpir_server_create(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                               b200pir_dpir* db, const uint32_t* h1_squished, const uint32_t* a2_t, size_t max_queries,
+                               b200pir_dpir_server** out) {
+  API_BEGIN
+  if (!params || !db || !h1_squished || !a2_t || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  if (max_queries == 0 || max_queries >= kDpirWireMaxLen) throw Error(B200PIR_E_BADARG, "max_queries must lie in [1, 2^28)");
+  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, nullptr, 64);
+  if (device != db->device) throw Error(B200PIR_E_BADARG, "the database lives on another device");
+  const uint64_t l = params->l, x = info.x;
+  if (l % x) throw Error(B200PIR_E_SHAPE, "l must be a multiple of x (concat_cols)");
+  if (db->cols != (params->m + 2) / 3) throw Error(B200PIR_E_SHAPE, "the database's packed columns are not ceil(m / 3)");
+  if (db->rows > l) throw Error(B200PIR_E_SHAPE, "the database has more than l rows");
+  dpir_device(device);
+  std::unique_ptr<b200pir_dpir_server> S(new b200pir_dpir_server());
+  S->device = device;
+  S->db = db;
+  S->n = params->n; S->l = l; S->p = params->p; S->delta = info.delta; S->x = x; S->e = info.ne / x;
+  S->dx = info.delta * x; S->rows1 = S->n * S->dx; S->c1 = (l / x + 2) / 3; S->lx3 = 3 * S->c1; S->dcols = db->cols;
+  S->max_queries = max_queries;
+  B200_CUDA(cudaDeviceGetAttribute(&S->sm_count, cudaDevAttrMultiProcessorCount, device));
+  B200_CUDA(cudaStreamCreateWithFlags(&S->stream, cudaStreamNonBlocking));
+  struct StreamGuard {
+    b200pir_dpir_server* s;
+    ~StreamGuard() { if (s) cudaStreamDestroy(s->stream); }
+  } sg{S.get()};
+  const uint64_t Q = max_queries, e = S->e;
+  // bounds of one call: at most Q requests and Q queries; the database pass has at most Q row segments (each request of k
+  // queries adds k - 1 cuts), each tiled and repeated once per 16 requests
+  S->task_cap = (ceil_div(l, kDpirMvRows) + Q) * ceil_div(Q, kDpirMvMaxVecs)
+              + ceil_div(S->rows1, kDpirMvRows) * ceil_div(Q * e, kDpirMvMaxVecs)
+              + ceil_div(S->dx, kDpirMvRows) * Q * e;
+  S->vec_cap = Q * Q + 2 * Q * e;
+  S->stage_cap = Q * (align_up(3 * S->dcols * 4, 16) + e * align_up(3 * S->c1 * 4, 16)) + align_up(S->task_cap * sizeof(DpirMvTask), 16)
+               + S->vec_cap * sizeof(DpirMvVec);
+  S->resp_cap = Q * (12 + S->dx * S->n * 4) + Q * e * DpirResponseLayout{1, e, S->dx, S->n, S->rows1}.pair_bytes();
+  B200_CUDA(cudaMallocHost(&S->h_stage, S->stage_cap));
+  B200_CUDA(cudaMallocHost(&S->h_resp, S->resp_cap));
+  S->d_stage.alloc(S->stage_cap);
+  S->d_resp.alloc(S->resp_cap);
+  S->d_a1.alloc(Q * l);
+  S->d_a1sq.alloc(Q * S->dx * S->c1);
+  S->d_msg0.alloc(Q * S->dx * S->n);
+  S->h1.alloc(S->rows1 * S->c1);
+  S->a2t.alloc(S->n * S->lx3);
+  B200_CUDA(cudaMemcpyAsync(S->h1.p, h1_squished, S->h1.n * 4, cudaMemcpyHostToDevice, S->stream));
+  B200_CUDA(cudaMemcpyAsync(S->a2t.p, a2_t, S->a2t.n * 4, cudaMemcpyHostToDevice, S->stream));
+  B200_CUDA(cudaStreamSynchronize(S->stream));
+  sg.s = nullptr;
+  *out = S.release();
+  API_END
+}
+
+void b200pir_dpir_server_destroy(b200pir_dpir_server* S) {
+  if (!S) return;
+  cudaSetDevice(S->device);
+  if (S->stream) {
+    cudaStreamSynchronize(S->stream);
+    cudaStreamDestroy(S->stream);
+  }
+  delete S;
+}
+
+int b200pir_dpir_answer_size(b200pir_dpir_server* S, const uint8_t* request, size_t len, size_t* out_len) {
+  API_BEGIN
+  if (!S || !request || !out_len) throw Error(B200PIR_E_BADARG, "null argument");
+  DpirWireRequest w;
+  std::string err;
+  if (int rc = parse_dpir_request(request, len, S->e, S->c1, w, err)) throw Error(rc, err);
+  *out_len = DpirResponseLayout{w.queries, S->e, S->dx, S->n, S->rows1}.bytes();
+  API_END
+}
+
+int b200pir_dpir_answer(b200pir_dpir_server* S, const uint8_t* request, size_t len, int64_t chunk_idx, uint8_t* out,
+                        size_t* out_len) {
+  API_BEGIN
+  if (!S || !request || !out || !out_len) throw Error(B200PIR_E_BADARG, "null argument");
+  std::vector<DpirCall> calls(1);
+  std::string err;
+  if (int rc = dpir_prepare_call(S, request, len, chunk_idx < 0 ? -1 : chunk_idx, calls[0], err)) throw Error(rc, err);
+  if (calls[0].w.queries > S->max_queries)
+    throw Error(B200PIR_E_SHAPE, "the request has " + std::to_string(calls[0].w.queries) + " queries; this server answers at most " +
+                                     std::to_string(S->max_queries) + " a call (max_queries)");
+  if (*out_len < calls[0].L.bytes()) throw Error(B200PIR_E_BADARG, "the output holds fewer bytes than the response");
+  std::lock_guard<std::mutex> lk(S->mu);
+  cudaSetDevice(S->device);
+  dpir_serve(S, calls, chunk_idx < 0 ? -1 : chunk_idx, &out, out_len);
+  API_END
+}
+
+int b200pir_dpir_answer_many(b200pir_dpir_server* S, const uint8_t* const* requests, const size_t* lens, size_t count,
+                             uint8_t* const* outs, size_t* out_lens) {
+  API_BEGIN
+  if (!S || (count && (!requests || !lens || !outs || !out_lens))) throw Error(B200PIR_E_BADARG, "null argument");
+  for (size_t i = 0; i < count; i++)
+    if (!requests[i] || !outs[i]) throw Error(B200PIR_E_BADARG, "null request or output " + std::to_string(i));
+  if (count == 0) return 0;
+  std::vector<DpirCall> calls(count);
+  uint64_t total = 0;
+  for (size_t i = 0; i < count; i++) {
+    std::string err;
+    if (int rc = dpir_prepare_call(S, requests[i], lens[i], -1, calls[i], err)) throw Error(rc, "request " + std::to_string(i) + ": " + err);
+    total += calls[i].w.queries;
+  }
+  if (total > S->max_queries)
+    throw Error(B200PIR_E_SHAPE, "the call has " + std::to_string(total) + " queries; this server answers at most " +
+                                     std::to_string(S->max_queries) + " a call (max_queries)");
+  for (size_t i = 0; i < count; i++)
+    if (out_lens[i] < calls[i].L.bytes()) throw Error(B200PIR_E_BADARG, "output " + std::to_string(i) + " holds fewer bytes than its response");
+  std::lock_guard<std::mutex> lk(S->mu);
+  cudaSetDevice(S->device);
+  dpir_serve(S, calls, -1, outs, out_lens);
+  API_END
+}
+
+// matrix_mul_vec_packed for `count` vectors, one pass over the matrix per 16 (host buffers; the multi-vector kernel's test face)
+int b200pir_dpir_matvec_packed_many(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out) {
+  API_BEGIN
+  if (!m || !b || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  if (count == 0) return 0;
+  if (m->rows > 0xFFFFFFFFull || count > 0xFFFFFFFFull) throw Error(B200PIR_E_SHAPE, "too many rows or vectors");
+  std::lock_guard<std::mutex> lk(m->mu);
+  cudaSetDevice(m->device);
+  int sms = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
+  DevBuf<uint32_t> d_b(count * 3 * m->cols), d_out(count * m->rows);
+  std::vector<DpirMvTask> tasks;
+  std::vector<DpirMvVec> vecs;
+  int vmax = 1;
+  for (size_t v0 = 0; v0 < count; v0 += kDpirMvMaxVecs) {
+    const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, count - v0);
+    for (size_t v = v0; v < v0 + nv; v++) vecs.push_back(DpirMvVec{d_b.p + v * 3 * m->cols, d_out.p + v * m->rows});
+    vmax = std::max<int>(vmax, nv);
+    for (uint64_t t0 = 0; t0 < m->rows; t0 += kDpirMvRows)
+      tasks.push_back(DpirMvTask{m->a.p + t0 * m->cols, (uint32_t)std::min<uint64_t>(kDpirMvRows, m->rows - t0), vec0, nv, (uint32_t)t0});
+  }
+  DevBuf<DpirMvTask> d_tasks(tasks.size());
+  DevBuf<DpirMvVec> d_vecs(vecs.size());
+  B200_CUDA(cudaMemcpyAsync(d_tasks.p, tasks.data(), tasks.size() * sizeof(DpirMvTask), cudaMemcpyHostToDevice, m->stream));
+  B200_CUDA(cudaMemcpyAsync(d_vecs.p, vecs.data(), vecs.size() * sizeof(DpirMvVec), cudaMemcpyHostToDevice, m->stream));
+  B200_CUDA(cudaMemcpyAsync(d_b.p, b, d_b.n * 4, cudaMemcpyHostToDevice, m->stream));
+  B200_CUDA(cudaMemsetAsync(d_out.p, 0, d_out.n * 4, m->stream));
+  launch_dpir_matvec_multi(d_tasks.p, tasks.size(), d_vecs.p, m->cols, vmax, dpir_mv_ksplit(tasks.size(), m->cols, sms), 0, m->stream);
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaMemcpyAsync(out, d_out.p, d_out.n * 4, cudaMemcpyDeviceToHost, m->stream));
   B200_CUDA(cudaStreamSynchronize(m->stream));
   B200_CUDA(cudaGetLastError());
   API_END

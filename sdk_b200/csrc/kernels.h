@@ -197,6 +197,24 @@ void launch_dpir_mul_transposed(uint32_t* out, const uint32_t* a, const uint32_t
 void launch_dpir_transpose_expand(uint32_t* out, const uint32_t* a, size_t rows, size_t cols, uint64_t modulus, size_t delta,
                                   size_t concat, size_t out_rows, size_t out_cols, cudaStream_t s);
 
+// ---- DoublePIR packed matrix x many vectors (dpir_serve.cu): the passes of answer() over every request of a call
+// A task is one CTA: rows [0, rows) (rows <= kDpirMvRows) of the matrix at `a` (rows `cols` words apart) against the vectors
+// vecs[vec0, vec0 + nv) (nv <= kDpirMvMaxVecs); vector v's result for row r goes to vecs[vec0 + v].out[out_off + r].
+constexpr int kDpirMvRows = 32;
+constexpr int kDpirMvMaxVecs = 16;
+struct DpirMvTask { const uint32_t* a; uint32_t rows, vec0, nv, out_off; };
+struct DpirMvVec { const uint32_t* b; uint32_t* out; };          // b: 3 * cols words
+enum { DPIR_MV_B_BE = 1,        // vector words are big-endian (wire order): swapped as they are staged
+       DPIR_MV_OUT_BE = 2 };    // results are stored big-endian (wire order); needs ksplit == 1
+// ksplit > 1 splits every task's k range over that many CTAs whose partial sums are added with atomicAdd into outputs the
+// caller has zeroed.  vmax = the largest nv of any task.
+void launch_dpir_matvec_multi(const DpirMvTask* tasks, size_t ntasks, const DpirMvVec* vecs, size_t cols, int vmax, int ksplit,
+                              int flags, cudaStream_t s);
+// the k split that gives `ntasks` tasks about two CTAs an SM, each at least one 256-column chunk
+int dpir_mv_ksplit(size_t ntasks, size_t cols, int sm_count);
+// dst[i] = byte-swapped src[i]
+void launch_dpir_bswap(uint32_t* dst, const uint32_t* src, size_t words, cudaStream_t s);
+
 // ---- DoublePIR offline setup (dpir_gemm.cu): doublepir.rs:76-108
 // c (rows x n_cols) = a (rows x k_dim, entries in [-2^15, 2^15) as wrapping u32) * b (k_dim x n_cols) mod 2^32; device pointers;
 // 8-bit limb products on the tensor cores (wgmma) (exact); synchronises the stream

@@ -58,6 +58,14 @@ def matrix_mul_vec_packed(a, b, basis=10, compression=3):
     return out
 
 
+def matrix_mul_vec_packed_many(a, bs):
+    """matrix_mul_vec_packed(a, b) for every b of bs in one pass over a per 16 vectors: (len(bs), a.rows) uint32."""
+    bs = np.ascontiguousarray(np.asarray(bs, dtype=np.uint32).reshape(-1, 3 * a.cols))
+    out = np.zeros((bs.shape[0], a.rows), dtype=np.uint32)
+    check(LIB.b200pir_dpir_matvec_packed_many(a._h, bs.ctypes.data, bs.shape[0], out.ctypes.data))
+    return out
+
+
 def matrix_mul_vec_packed_rows(a, row_begin, row_count, b):
     """matrix_mul_vec_packed(db.rows(start, n), q) (doublepir.rs:301)."""
     out = np.zeros(row_count, dtype=np.uint32)
@@ -109,6 +117,94 @@ def answer(db, queries, h_1, a_2_transpose, p, delta, x, ne):
     hm.close()
     am.close()
     return msg
+
+
+def serialize_state(mats):
+    """State::serialize (serializer.rs:56-94): u32 BE count, then per matrix u32 BE rows, cols and data.  A 1-D array is a
+    column (len x 1), as answer()'s vectors are."""
+    out = [len(mats).to_bytes(4, "big")]
+    for a in mats:
+        a = np.asarray(a, dtype=np.uint32)
+        rows, cols = (a.shape[0], 1) if a.ndim == 1 else a.shape
+        out += [int(rows).to_bytes(4, "big"), int(cols).to_bytes(4, "big"), a.astype(">u4").tobytes()]
+    return b"".join(out)
+
+
+def serialize_request(queries):
+    """Vec<State>::serialize: what DoublePirServer::answer reads (queries: list of [q_1, q_2, ...])."""
+    return len(queries).to_bytes(4, "big") + b"".join(serialize_state(q) for q in queries)
+
+
+def deserialize_state(buf):
+    """Vec<Matrix>::deserialize: a list of (rows, cols) uint32 arrays; trailing bytes are ignored."""
+    buf = bytes(buf)
+    count, pos, out = int.from_bytes(buf[:4], "big"), 4, []
+    for _ in range(count):
+        rows, cols = int.from_bytes(buf[pos:pos + 4], "big"), int.from_bytes(buf[pos + 4:pos + 8], "big")
+        pos += 8
+        out.append(np.frombuffer(buf, dtype=">u4", count=rows * cols, offset=pos).astype(np.uint32).reshape(rows, cols))
+        pos += 4 * rows * cols
+    return out
+
+
+class Server:
+    """DoublePirServer::answer / answer_inline (doublepir/server.rs:167-180, 235-247) served from HBM.  db: the PackedMatrix
+    `load` returns (or one chunk's rows, for answer(.., chunk_idx)); borrowed, it must stay open while the server is.
+    h1_squished / a2_t: the host matrices `load` / `setup` return, uploaded once.  max_queries bounds the queries of one call."""
+
+    def __init__(self, db, h1_squished, a2_t, params, num_entries, bits_per_entry, max_queries=32, device=0):
+        self.db = db
+        self.max_queries = max_queries
+        h1 = np.ascontiguousarray(h1_squished, dtype=np.uint32)
+        a2 = np.ascontiguousarray(a2_t, dtype=np.uint32)
+        h = C.c_void_p()
+        check(LIB.b200pir_dpir_server_create(device, C.byref(_params(params)), num_entries, bits_per_entry, db._h, h1.ctypes.data,
+                                             a2.ctypes.data, max_queries, C.byref(h)))
+        self._h = h
+
+    def answer_size(self, request):
+        n = C.c_size_t()
+        check(LIB.b200pir_dpir_answer_size(self._h, bytes(request), len(request), C.byref(n)))
+        return n.value
+
+    def _size_or_zero(self, request):
+        # a malformed request gets no buffer; the answer call itself then reports why it is refused
+        try:
+            return self.answer_size(request)
+        except B200PirError:
+            return 0
+
+    def answer(self, request, chunk_idx=None):
+        """msg.serialize() of answer(); chunk_idx = k: answer_inline(.., Some(k)) with this server's matrix as the data."""
+        request = bytes(request)
+        n = C.c_size_t(self._size_or_zero(request))
+        out = C.create_string_buffer(max(n.value, 1))
+        check(LIB.b200pir_dpir_answer(self._h, request, len(request), -1 if chunk_idx is None else int(chunk_idx), out, C.byref(n)))
+        return out.raw[:n.value]
+
+    def answer_many(self, requests):
+        """answer() of every request (different clients, unchunked) in one call."""
+        requests = [bytes(r) for r in requests]
+        k = len(requests)
+        sizes = [self._size_or_zero(r) for r in requests]
+        outs = [C.create_string_buffer(max(s, 1)) for s in sizes]
+        reqs = (C.c_void_p * k)(*[C.cast(C.c_char_p(r), C.c_void_p) for r in requests])
+        lens = (C.c_size_t * k)(*[len(r) for r in requests])
+        optr = (C.c_void_p * k)(*[C.cast(o, C.c_void_p) for o in outs])
+        olen = (C.c_size_t * k)(*sizes)
+        check(LIB.b200pir_dpir_answer_many(self._h, reqs, lens, k, optr, olen))
+        return [o.raw[:olen[i]] for i, o in enumerate(outs)]
+
+    def close(self):
+        if getattr(self, "_h", None):
+            LIB.b200pir_dpir_server_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def matmul(a, b, device=0):
