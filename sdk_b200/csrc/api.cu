@@ -246,13 +246,26 @@ struct b200pir_db {
   b200pir_ctx* ctx;
   Shard shard;
   int rows;                 // local second-dimension rows
-  int format = 0;           // 0: d (IMAD layout)  1: f (INT8 MMA fragment order)  2: t (wgmma tile images)
-  DevBuf<uint4> d;          // [slice][row][dim0/2][2048]
-  DevBuf<uint4> f;          // [slice][n][z][mt][ks][limb][lane]
-  DevBuf<uint8_t> t;        // format 2: [slice][n][z][mt][ks][4096 B] tile images (tc5_kernels.cu)
-  Tc5Geom T;
-  ImmaGeom F;
-  size_t slice_cells() const { return (size_t)rows * (ctx->dim0 / 2) * POLY; }
+  DbLayout layout;          // format (0: IMAD cells, 1: mma.sync fragments, 2: wgmma tile images), geometries, store.p
+  DevBuf<uint8_t> store;    // db_bytes(layout, slices) bytes
+  // The first dimension's product is z-major (formats 1 and 2: u32 [query][slice][n][z][row][ct_row]) or ntt32 (format 0)
+  bool zmajor_product() const { return layout.format != 0; }
+  // The bulk loaders (upload, synthetic fill) build a slice in the format-0 layout and then place_slice0 it.  Where slice s is
+  // built: returned as the base pointer the format-0 kernels address slice s from (imad_cell).  For format 0 that is the
+  // store.  Otherwise the slice is built in `scratch`, one format-0 slice allocated on first use, and the base is `scratch`
+  // minus s format-0 slices: only slice s is ever addressed from it, and that slice is the scratch.
+  uint4* slice0_base(int s, DevBuf<uint8_t>& scratch) {
+    if (layout.format == 0) return reinterpret_cast<uint4*>(store.p);
+    const size_t slice0_bytes = imad_cell(layout.G, 1, 0, 0, 0) * sizeof(uint4);
+    if (!scratch.p) scratch.alloc(slice0_bytes);
+    return reinterpret_cast<uint4*>(reinterpret_cast<uintptr_t>(scratch.p) - (uintptr_t)s * slice0_bytes);
+  }
+  // slice s, built at slice0_base(s, scratch), into the store: nothing to do for format 0, a re-tiling for formats 1 and 2
+  void place_slice0(int s, const DevBuf<uint8_t>& scratch, cudaStream_t st) {
+    const uint4* src = reinterpret_cast<const uint4*>(scratch.p);
+    if (layout.format == 1) launch_db_to_frag(layout.F, src, reinterpret_cast<uint4*>(store.p), s, st);
+    else if (layout.format == 2) launch_db_to_tc5(layout.T, src, store.p, s, st);
+  }
   // Presence (lib/server's SparseDb, db/sparse_db.rs:5-47: an item exists once it has been written).  Storage stays dense in HBM
   // (absent = zero polynomial, so every sum is unchanged); what the map buys is COST: on the wgmma path whole 32-row x 32-j
   // tiles without a present item are neither fetched nor multiplied (tile_mask, one bit per tile, kept on the device).
@@ -264,7 +277,7 @@ struct b200pir_db {
   void presence_init() {
     present.assign((capacity() + 63) / 64, 0);
     present_count = 0;
-    h_tile_mask.assign((size_t)ctx->slices * T.mt, 0u);
+    h_tile_mask.assign((size_t)ctx->slices * layout.T.mt, 0u);
     tile_mask.alloc(h_tile_mask.size());
     B200_CUDA(cudaMemset(tile_mask.p, 0, h_tile_mask.size() * 4));
   }
@@ -272,7 +285,7 @@ struct b200pir_db {
   bool mark_host(int slice, int il, int j) {
     const uint64_t bit = ((uint64_t)slice * rows + il) * ctx->dim0 + j;
     if (!((present[bit >> 6] >> (bit & 63)) & 1)) { present[bit >> 6] |= 1ull << (bit & 63); present_count++; }
-    const size_t w = (size_t)slice * T.mt + (il >> 5);
+    const size_t w = (size_t)slice * layout.T.mt + (il >> 5);
     const uint32_t nv = h_tile_mask[w] | (1u << (j >> 5));
     if (nv == h_tile_mask[w]) return false;
     h_tile_mask[w] = nv;
@@ -281,7 +294,7 @@ struct b200pir_db {
   // one item written (stream-ordered update of the device mask word)
   void mark(int slice, int il, int j, cudaStream_t s) {
     if (mark_host(slice, il, j)) {
-      const size_t w = (size_t)slice * T.mt + (il >> 5);
+      const size_t w = (size_t)slice * layout.T.mt + (il >> 5);
       B200_CUDA(cudaMemcpyAsync(tile_mask.p + w, &h_tile_mask[w], 4, cudaMemcpyHostToDevice, s));
     }
   }
@@ -298,6 +311,7 @@ struct b200pir_db {
     const uint64_t lo = (uint64_t)slice * rows * ctx->dim0, hi = lo + (uint64_t)rows * ctx->dim0;
     for (uint64_t b = lo; b < hi; b++)
       if (!((present[b >> 6] >> (b & 63)) & 1)) { present[b >> 6] |= 1ull << (b & 63); present_count++; }
+    const Tc5Geom& T = layout.T;
     const uint32_t full = T.ks >= 32 ? 0xffffffffu : ((1u << T.ks) - 1u);
     for (int m = 0; m < T.mt; m++) h_tile_mask[(size_t)slice * T.mt + m] = full;
     B200_CUDA(cudaMemcpyAsync(tile_mask.p + (size_t)slice * T.mt, &h_tile_mask[(size_t)slice * T.mt], (size_t)T.mt * 4,
@@ -467,6 +481,63 @@ void run_prepare(b200pir_ctx* c, b200pir_pp* pp, size_t count, bool images = fal
   // v_folding_neg (server.rs:680) is not materialised: the fold fast path uses G - C_k implicitly.
 }
 
+// The first-dimension product of `count` queries (operands qdev + qi * dim0 * POLY) over slices [slice_begin, slice_begin +
+// slice_count), into `out` (queries slices * rows * 4 * POLY words apart) in the form db->zmajor_product() names.
+// `images`: the operand already sits as tile images (format 2; groups of `per_group` <= 16 queries, one image each).
+void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, uint32_t* out, int slice_begin,
+                   int slice_count, const uint8_t* images = nullptr, size_t per_group = 16) {
+  const DbLayout& L = db->layout;
+  const size_t q_stride = (size_t)c->dim0 * POLY;
+  const size_t out_stride = (size_t)c->slices * db->rows * 4 * POLY;
+  if (L.format == 0) {
+    // IMAD path: 4, 2 or 1 queries per database pass
+    b200pir_ctx::Scope sc(c, ST_MUL);
+    size_t qi = 0;
+    while (qi < count) {
+      int nq = 1;
+      if (count - qi >= 4 && c->max_group >= 4) nq = 4;
+      else if (count - qi >= 2 && c->max_group >= 2) nq = 2;
+      launch_multiply(c->dp, L.G, reinterpret_cast<const uint4*>(L.base), qdev + qi * q_stride, out + qi * out_stride,
+                      slice_begin, slice_count, nq, q_stride, out_stride, c->mul_variant, c->stream);
+      c->mul_launches++;
+      qi += nq;
+    }
+  } else if (L.format == 2) {
+    // wgmma path: same z-major product as the mma.sync path, 16 queries per database pass
+    if (!images) c->w_qt.ensure(tc5_query_bytes(L.T));
+    const size_t step = images ? per_group : 16;
+    for (size_t qi = 0, g = 0; qi < count; qi += step, g++) {
+      const int nq = (int)std::min<size_t>(step, count - qi);
+      const uint8_t* qt = images ? images + g * tc5_query_bytes(L.T) : c->w_qt.p;
+      if (!images) {
+        b200pir_ctx::Scope sq(c, ST_QIMG);
+        launch_query_to_tc5(L.T, qdev + qi * q_stride, q_stride, nq, c->w_qt.p, c->stream);
+      }
+      b200pir_ctx::Scope sc(c, ST_MUL);
+      launch_multiply_tc5(c->dp, L.T, L.base, db->tile_mask.p, qt, out + qi * out_stride, out_stride, nq, slice_begin,
+                          slice_count, c->sm_count, c->stream);
+      c->mul_launches++;
+    }
+  } else {
+    // INT8 tensor-core path
+    c->w_qf.ensure(imma_query_cells(L.F));
+    const size_t per_pass = (c->max_group >= 16 && imma_supports_16(L.F)) ? 16 : (c->max_group >= 8 ? 8 : 4);
+    for (size_t qi = 0; qi < count; qi += per_pass) {
+      const int nq = (int)std::min<size_t>(per_pass, count - qi);
+      {
+        b200pir_ctx::Scope sq(c, ST_QIMG);
+        launch_query_to_frag(L.F, qdev + qi * q_stride, q_stride, nq, c->w_qf.p, c->stream);
+      }
+      {
+        b200pir_ctx::Scope sc(c, ST_MUL);
+        launch_multiply_imma(c->dp, L.F, reinterpret_cast<const uint4*>(L.base), c->w_qf.p, out + qi * out_stride, out_stride,
+                             nq, slice_begin, slice_count, c->stream);
+        c->mul_launches++;
+      }
+    }
+  }
+}
+
 // first dimension + from_ntt + local fold.  Leaves survivors at w_cts[(qi*slices + slice)*rows*2*POLY].
 // `images`: the first-dimension operand already sits as tile images (groups of `per_group` <= 16 queries, one image each)
 void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev = nullptr,
@@ -474,69 +545,15 @@ void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const 
   if (!qdev) qdev = c->w_qdev.p;
   if (!vfold) vfold = c->w_vfold.p;
   const int rows = db->rows;
-  MulGeom G = c->geom(rows);
-  const size_t q_stride = (size_t)c->dim0 * POLY;
   const size_t out_stride = (size_t)c->slices * rows * 4 * POLY;
-  if (db->format == 0) {
-    {
-      b200pir_ctx::Scope sc(c, ST_MUL);
-      size_t qi = 0;
-      while (qi < count) {
-        int nq = 1;
-        if (count - qi >= 4 && c->max_group >= 4) nq = 4;
-        else if (count - qi >= 2 && c->max_group >= 2) nq = 2;
-        launch_multiply(c->dp, G, db->d.p, qdev + qi * q_stride, c->w_mult.p + qi * out_stride, 0, c->slices, nq,
-                        q_stride, out_stride, c->mul_variant, c->stream);
-        c->mul_launches++;
-        qi += nq;
-      }
-    }
-    {
-      // server.rs:707-709 from_ntt, minus the CRT lift: inverse NTT of every CRT half in place -> residue form
-      b200pir_ctx::Scope sc(c, ST_FROMNTT);
-      launch_ntt32(c->dp, c->w_mult.p, count * c->slices * rows * 2, true, c->stream);
-    }
-  } else if (db->format == 2) {
-    // wgmma path: same z-major product as the mma.sync path, 16 queries per database pass
-    if (!images) c->w_qt.ensure(tc5_query_bytes(db->T));
-    const size_t step = images ? per_group : 16;
-    for (size_t qi = 0, g = 0; qi < count; qi += step, g++) {
-      const int nq = (int)std::min<size_t>(step, count - qi);
-      const uint8_t* qt = images ? images + g * tc5_query_bytes(db->T) : c->w_qt.p;
-      if (!images) {
-        b200pir_ctx::Scope sq(c, ST_QIMG);
-        launch_query_to_tc5(db->T, qdev + qi * q_stride, q_stride, nq, c->w_qt.p, c->stream);
-      }
-      b200pir_ctx::Scope sc(c, ST_MUL);
-      launch_multiply_tc5(c->dp, db->T, db->t.p, db->tile_mask.p, qt, c->w_cts.p + qi * out_stride, out_stride, nq, 0, c->slices,
-                          c->sm_count, c->stream);
-      c->mul_launches++;
-    }
-    {
-      b200pir_ctx::Scope sc(c, ST_FROMNTT);
-      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
-    }
-  } else {
-    // INT8 tensor-core path: z-major product in w_cts (free until the fold starts), then inverse NTT into w_mult
-    c->w_qf.ensure(imma_query_cells(db->F));
-    const size_t per_pass = (c->max_group >= 16 && imma_supports_16(db->F)) ? 16 : (c->max_group >= 8 ? 8 : 4);
-    for (size_t qi = 0; qi < count; qi += per_pass) {
-      const int nq = (int)std::min<size_t>(per_pass, count - qi);
-      {
-        b200pir_ctx::Scope sq(c, ST_QIMG);
-        launch_query_to_frag(db->F, qdev + qi * q_stride, q_stride, nq, c->w_qf.p, c->stream);
-      }
-      {
-        b200pir_ctx::Scope sc(c, ST_MUL);
-        launch_multiply_imma(c->dp, db->F, db->f.p, c->w_qf.p, c->w_cts.p + qi * out_stride, out_stride, nq, 0, c->slices,
-                             c->stream);
-        c->mul_launches++;
-      }
-    }
-    {
-      b200pir_ctx::Scope sc(c, ST_FROMNTT);
-      launch_intt_from_zmajor(c->dp, db->F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
-    }
+  // server.rs:707-709 from_ntt, minus the CRT lift, into w_mult in residue form: a z-major product goes to w_cts (free until
+  // the fold starts) and is inverse-transformed from there; an ntt32 product is inverse-transformed in place
+  const bool zmajor = db->zmajor_product();
+  run_first_dim(c, db, count, qdev, zmajor ? c->w_cts.p : c->w_mult.p, 0, c->slices, images, per_group);
+  {
+    b200pir_ctx::Scope sc(c, ST_FROMNTT);
+    if (zmajor) launch_intt_from_zmajor(c->dp, db->layout.F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
+    else launch_ntt32(c->dp, c->w_mult.p, count * c->slices * rows * 2, true, c->stream);
   }
   {
     b200pir_ctx::Scope sc(c, ST_FOLD);
@@ -784,24 +801,16 @@ int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count
   db->ctx = c;
   db->shard = Shard{(int)shard_index, (int)shard_count};
   db->rows = c->num_per / (int)shard_count;
-  db->F = make_imma_geom(c->dim0, db->rows);
-  db->T = make_tc5_geom(c->dim0, db->rows);
-  db->format = c->db_format >= 0 ? c->db_format : (tc5_supported(db->T) ? 2 : 1);
+  DbLayout& L = db->layout;
+  L.G = c->geom(db->rows);
+  L.F = make_imma_geom(c->dim0, db->rows);
+  L.T = make_tc5_geom(c->dim0, db->rows);
+  L.format = c->db_format >= 0 ? c->db_format : (tc5_supported(L.T) ? 2 : 1);
   db->presence_init();
-  if (db->format == 0) {
-    size_t cells = (size_t)c->slices * db->slice_cells();
-    db->d.alloc(cells);
-    B200_CUDA(cudaMemsetAsync(db->d.p, 0, cells * sizeof(uint4), c->stream));
-  } else if (db->format == 2) {
-    if (!tc5_supported(db->T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
-    size_t bytes = tc5_db_bytes(db->T, c->slices);
-    db->t.alloc(bytes);
-    B200_CUDA(cudaMemsetAsync(db->t.p, 0, bytes, c->stream));
-  } else {
-    size_t cells = imma_db_cells(db->F, c->slices);
-    db->f.alloc(cells);
-    B200_CUDA(cudaMemsetAsync(db->f.p, 0, cells * sizeof(uint4), c->stream));
-  }
+  if (L.format == 2 && !tc5_supported(L.T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
+  db->store.alloc(db_bytes(L, c->slices));
+  L.base = db->store.p;
+  B200_CUDA(cudaMemsetAsync(db->store.p, 0, db->store.n, c->stream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
   *out = db.release();
   API_END
@@ -821,11 +830,9 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
   const size_t per_z = (size_t)c->dim0 * c->num_per;
   int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, ((size_t)64 << 20) / (per_z * 8)));
   DevBuf<uint64_t> stage(per_z * zc);
-  MulGeom G = c->geom(db->rows);
-  DevBuf<uint4> tmp;
-  uint4* dst;
-  if (db->format == 0) dst = db->d.p + (size_t)slice * db->slice_cells();
-  else { tmp.alloc(db->slice_cells()); dst = tmp.p; }
+  const MulGeom& G = db->layout.G;
+  DevBuf<uint8_t> scratch;
+  uint4* dst = db->slice0_base((int)slice, scratch) + imad_cell(G, (int)slice, 0, 0, 0);
   for (int z0 = 0; z0 < POLY; z0 += zc) {
     int cur = std::min(zc, POLY - z0);
     const uint64_t* src = fetch((size_t)z0 * per_z, per_z * cur);
@@ -833,13 +840,7 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
     launch_db_retile_chunk(G, db->shard, dst, stage.p, z0, cur, c->stream);
     B200_CUDA(cudaStreamSynchronize(c->stream));
   }
-  if (db->format == 1) {
-    launch_db_to_frag(db->F, tmp.p, db->f.p, (int)slice, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-  } else if (db->format == 2) {
-    launch_db_to_tc5(db->T, tmp.p, db->t.p, (int)slice, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-  }
+  db->place_slice0((int)slice, scratch, c->stream);
   db->mark_slice((int)slice, c->stream);
   B200_CUDA(cudaStreamSynchronize(c->stream));
   B200_CUDA(cudaGetLastError());
@@ -856,8 +857,7 @@ void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t spa
   B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
   const size_t chunks = (size_t)c->slices;
   const size_t bpc = (c->hp.db_item_size + chunks - 1) / chunks;             // params.bytes_per_chunk()
-  const DbDst dst{db->format, c->geom(db->rows), db->F, db->T, db->d.p, db->f.p, db->t.p};
-  launch_write_items(c->dp, dst, c->w_wbytes.p, c->w_witems.p, (int)count, (int)chunks, (int)bpc, c->hp.p, c->stream);
+  launch_write_items(c->dp, db->layout, c->w_wbytes.p, c->w_witems.p, (int)count, (int)chunks, (int)bpc, c->hp.p, c->stream);
 }
 
 // Database export, shared by b200pir_db_download(_slice) and b200pir_db_save_file.  A chunk is one slice and a range of z of
@@ -887,9 +887,8 @@ void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end,
     for (size_t k = 0; k < chunks.size(); k++) {
       {
         Guard gd(c);
-        const DbDst dst{db->format, c->geom(db->rows), db->F, db->T, db->d.p, db->f.p, db->t.p};
         uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
-        launch_db_export(dst, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
+        launch_db_export(db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
         B200_CUDA(cudaMemcpyAsync(c->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, c->stream));
         B200_CUDA(cudaEventRecord(c->export_done[k & 1], c->stream));
       }
@@ -1037,9 +1036,7 @@ int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint6
   if (ii % db->shard.count != db->shard.index) return 0;           // row lives on another GPU
   DevBuf<uint64_t> tmp(POLY);
   B200_CUDA(cudaMemcpyAsync(tmp.p, poly, POLY * 8, cudaMemcpyHostToDevice, c->stream));
-  if (db->format == 0) launch_db_upsert(c->geom(db->rows), db->d.p, (int)slice, ii / db->shard.count, j, tmp.p, c->stream);
-  else if (db->format == 2) launch_db_upsert_tc5(db->T, db->t.p, (int)slice, ii / db->shard.count, j, tmp.p, c->stream);
-  else launch_db_upsert_frag(db->F, db->f.p, (int)slice, ii / db->shard.count, j, tmp.p, c->stream);
+  launch_db_upsert(db->layout, (int)slice, ii / db->shard.count, j, tmp.p, c->stream);
   db->mark((int)slice, ii / db->shard.count, j, c->stream);
   // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
   B200_CUDA(cudaStreamSynchronize(c->stream));
@@ -1169,9 +1166,9 @@ int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity
 int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes) {
   API_BEGIN
   if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  if (format) *format = db->format;
+  if (format) *format = db->layout.format;
   if (local_rows) *local_rows = (uint64_t)db->rows;
-  if (hbm_bytes) *hbm_bytes = (uint64_t)(db->d.n * sizeof(uint4) + db->f.n * sizeof(uint4) + db->t.n);
+  if (hbm_bytes) *hbm_bytes = (uint64_t)db->store.n;
   API_END
 }
 int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
@@ -1179,21 +1176,15 @@ int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
   if (!c) throw Error(B200PIR_E_BADARG, "null ctx");
   Guard gd(c);
   check_db(c, db);
-  MulGeom G = c->geom(db->rows);
-  // keep each launch's grid below 2^31 CTAs
+  // keep each launch's grid below 2^31 CTAs; slices built in the scratch go one at a time
   size_t per_slice = (size_t)db->rows * (c->dim0 / 2);
   int step = (int)std::max<size_t>(1, std::min<size_t>(c->slices, ((size_t)1 << 30) / per_slice));
-  if (db->format == 0) {
-    for (int s0 = 0; s0 < c->slices; s0 += step)
-      launch_db_synth(c->dp, G, db->shard, db->d.p, seed, c->hp.p, s0, std::min(step, c->slices - s0), c->stream);
-  } else {
-    // build each slice in the IMAD layout in a scratch buffer, then re-tile it into fragment order
-    DevBuf<uint4> tmp(db->slice_cells());
-    for (int s0 = 0; s0 < c->slices; s0++) {
-      launch_db_synth(c->dp, G, db->shard, tmp.p - (size_t)s0 * db->slice_cells(), seed, c->hp.p, s0, 1, c->stream);
-      if (db->format == 2) launch_db_to_tc5(db->T, tmp.p, db->t.p, s0, c->stream);
-      else launch_db_to_frag(db->F, tmp.p, db->f.p, s0, c->stream);
-    }
+  if (db->layout.format != 0) step = 1;
+  DevBuf<uint8_t> scratch;
+  for (int s0 = 0; s0 < c->slices; s0 += step) {
+    launch_db_synth(c->dp, db->layout.G, db->shard, db->slice0_base(s0, scratch), seed, c->hp.p, s0,
+                    std::min(step, c->slices - s0), c->stream);
+    db->place_slice0(s0, scratch, c->stream);
   }
   for (int s0 = 0; s0 < c->slices; s0++) db->mark_slice(s0, c->stream);
   B200_CUDA(cudaStreamSynchronize(c->stream));
@@ -1429,31 +1420,17 @@ int b200pir_multiply_reg_by_database(b200pir_ctx* c, b200pir_db* db, uint64_t sl
   check_db(c, db);
   if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
   const int rows = db->rows;
-  MulGeom G = c->geom(rows);
+  const bool zmajor = db->zmajor_product();
   DevBuf<uint64_t> vq((size_t)c->dim0 * 2 * POLY);
   DevBuf<uint4> qd((size_t)c->dim0 * POLY);
-  DevBuf<uint32_t> o((size_t)c->slices * rows * 4 * POLY);
+  DevBuf<uint32_t> o((size_t)c->slices * rows * 4 * POLY), zm(zmajor ? o.n : 0);
   DevBuf<uint64_t> wide((size_t)rows * 4 * POLY);
   B200_CUDA(cudaMemcpyAsync(vq.p, v_firstdim, vq.n * 8, cudaMemcpyHostToDevice, c->stream));
-  launch_query_to_dev(G, qd.p, vq.p, c->stream);
-  if (db->format == 0) {
-    launch_multiply(c->dp, G, db->d.p, qd.p, o.p, (int)slice, 1, 1, 0, 0, c->mul_variant, c->stream);
-  } else if (db->format == 2) {
-    DevBuf<uint8_t> qt(tc5_query_bytes(db->T));
-    DevBuf<uint32_t> zm((size_t)c->slices * rows * 4 * POLY);
-    launch_query_to_tc5(db->T, qd.p, 0, 1, qt.p, c->stream);
-    launch_multiply_tc5(c->dp, db->T, db->t.p, db->tile_mask.p, qt.p, zm.p, 0, 1, (int)slice, 1, c->sm_count, c->stream);
-    launch_zmajor_to_ntt32(db->F, zm.p, o.p + (size_t)slice * rows * 4 * POLY, (int)slice, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-  } else {
-    DevBuf<uint2> qf(imma_query_cells(db->F));
-    DevBuf<uint32_t> zm((size_t)c->slices * rows * 4 * POLY);
-    launch_query_to_frag(db->F, qd.p, 0, 1, qf.p, c->stream);
-    launch_multiply_imma(c->dp, db->F, db->f.p, qf.p, zm.p, 0, 1, (int)slice, 1, c->stream);
-    launch_zmajor_to_ntt32(db->F, zm.p, o.p + (size_t)slice * rows * 4 * POLY, (int)slice, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  launch_widen(wide.p, o.p + (size_t)slice * rows * 4 * POLY, wide.n, c->stream);
+  launch_query_to_dev(db->layout.G, qd.p, vq.p, c->stream);
+  run_first_dim(c, db, 1, qd.p, zmajor ? zm.p : o.p, (int)slice, 1);
+  uint32_t* o_slice = o.p + (size_t)slice * rows * 4 * POLY;          // ntt32 [row][ct_row][n][z] of this slice
+  if (zmajor) launch_zmajor_to_ntt32(db->layout.F, zm.p, o_slice, (int)slice, c->stream);
+  launch_widen(wide.p, o_slice, wide.n, c->stream);
   B200_CUDA(cudaMemcpyAsync(out, wide.p, wide.n * 8, cudaMemcpyDeviceToHost, c->stream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
   B200_CUDA(cudaGetLastError());
@@ -1624,7 +1601,7 @@ int b200pir_encode(b200pir_ctx* c, const uint64_t* v_packed_raw, uint8_t* out, s
 // ---------------------------------------------------------------- process_query
 static void run_query_batch_resident(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, size_t count, uint8_t* out_dev) {
   // queries are already in c->w_query; format-2 databases get their operand as tile images straight from the expansion
-  const bool images = db->format == 2 && c->hp.expand_queries;
+  const bool images = db->layout.format == 2 && c->hp.expand_queries;
   run_prepare(c, pp, count, images);
   run_first_dim_and_fold(c, db, count, nullptr, nullptr, images ? c->w_qt.p : nullptr, 16);
   run_pack_encode(c, pp, c->folded, c->folded_stride, count, out_dev);
@@ -1902,7 +1879,7 @@ int b200pir_first_dim_fold_images_dev(b200pir_ctx* c, b200pir_db* db, const void
   if (!c || !images_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
-  if (db->format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
+  if (db->layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
   if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
   const size_t count = groups * per_group;
   if (count == 0) return 0;

@@ -77,18 +77,18 @@ k_db_export_limbs(const uint8_t* __restrict__ db, int mt_count, int ks_count, in
 
 }  // namespace
 
-void launch_db_export(const DbDst& D, int slice, int z0, int zc, uint64_t* out, cudaStream_t s) {
+void launch_db_export(const DbLayout& L, int slice, int z0, int zc, uint64_t* out, cudaStream_t s) {
   if (zc <= 0) return;
   ++g_kernel_launches;
-  if (D.format == 0) {
-    const dim3 grid((unsigned)D.G.num_per, (unsigned)((D.G.dim0 / 2 + 31) / 32), (unsigned)((zc + 31) / 32));
-    k_db_export_imad<<<grid, 256, 0, s>>>(D.G, D.d, slice, z0, zc, out);
-  } else if (D.format == 2) {
-    k_db_export_limbs<32><<<dim3((unsigned)zc, (unsigned)D.T.mt, (unsigned)D.T.ks), 256, 0, s>>>(
-        D.t, D.T.mt, D.T.ks, D.T.rows, D.T.dim0, slice, z0, out);
+  if (L.format == 0) {
+    const dim3 grid((unsigned)L.G.num_per, (unsigned)((L.G.dim0 / 2 + 31) / 32), (unsigned)((zc + 31) / 32));
+    k_db_export_imad<<<grid, 256, 0, s>>>(L.G, reinterpret_cast<const uint4*>(L.base), slice, z0, zc, out);
+  } else if (L.format == 2) {
+    k_db_export_limbs<32><<<dim3((unsigned)zc, (unsigned)L.T.mt, (unsigned)L.T.ks), 256, 0, s>>>(
+        L.base, L.T.mt, L.T.ks, L.T.rows, L.T.dim0, slice, z0, out);
   } else {
-    k_db_export_limbs<16><<<dim3((unsigned)zc, (unsigned)D.F.mt, (unsigned)D.F.ks), 128, 0, s>>>(
-        reinterpret_cast<const uint8_t*>(D.f), D.F.mt, D.F.ks, D.F.rows, D.F.dim0, slice, z0, out);
+    k_db_export_limbs<16><<<dim3((unsigned)zc, (unsigned)L.F.mt, (unsigned)L.F.ks), 128, 0, s>>>(
+        L.base, L.F.mt, L.F.ks, L.F.rows, L.F.dim0, slice, z0, out);
   }
 }
 

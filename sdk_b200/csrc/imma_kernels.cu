@@ -81,14 +81,6 @@ k_db_to_frag(ImmaGeom F, const uint4* __restrict__ db0_slice, uint4* __restrict_
   }
 }
 
-// one item polynomial (2048 packed words lo|hi<<32) into the fragment-order database (byte writes)
-__global__ void k_db_upsert_frag(ImmaGeom F, uint4* dbf, int slice, int il, int j, const uint64_t* poly) {
-  int z = blockIdx.x * blockDim.x + threadIdx.x;
-  if (z >= POLY) return;
-  const uint64_t w = poly[z];
-  place_frag(F, reinterpret_cast<uint8_t*>(dbf), slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
-}
-
 // expanded queries (format of mul_kernels.cu: uint4 [jp][jb][z]) -> B fragments
 //   qf[n][z][nt][ks][limb m][lane] = uint2{b0, b1};  column (nt*8 + g) = 2*query + ciphertext row
 __global__ void __launch_bounds__(256)
@@ -431,9 +423,6 @@ inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + blo
 void upload_imma_constants(const Twiddle* lo) {
   B200_CUDA(cudaMemcpyToSymbol(c_tw_lo_imma, lo, sizeof(Twiddle) * 2 * 3 * 64));
 }
-size_t imma_db_cells(const ImmaGeom& F, int slices) {
-  return (size_t)slices * 2 * POLY * F.mt * F.ks * 4 * 32;
-}
 size_t imma_query_cells(const ImmaGeom& F) { return (size_t)2 * POLY * 4 * F.ks * 4 * 32; }   // up to 4 column tiles
 // 16 queries per pass need the B operand (4 tiles) plus the A rings in one CTA's shared memory
 bool imma_supports_16(const ImmaGeom& F) {
@@ -444,10 +433,6 @@ void launch_db_to_frag(const ImmaGeom& F, const uint4* db0_slice, uint4* dbf, in
   size_t warps = (size_t)POLY * F.mt * F.ks;
   ++g_kernel_launches;
   k_db_to_frag<<<grid1d(warps * 32, 256), 256, 0, s>>>(F, db0_slice, dbf, slice);
-}
-void launch_db_upsert_frag(const ImmaGeom& F, uint4* dbf, int slice, int il, int j, const uint64_t* poly, cudaStream_t s) {
-  ++g_kernel_launches;
-  k_db_upsert_frag<<<POLY / 256, 256, 0, s>>>(F, dbf, slice, il, j, poly);
 }
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s) {
   const int ntiles = imma_query_tiles(nq);

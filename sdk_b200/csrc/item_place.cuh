@@ -1,9 +1,10 @@
 // Where one NTT coordinate z of one database item lives in each device layout, and how it is read back.  Item (slice, local
 // row il, column j) holds, at every z, the residue mod q0 (`lo`) and mod q1 (`hi`) of the packed word lo | hi << 32
-// (loading.rs:34-41 pack_ntt_poly).  The single-item upserts, the batched raw-byte writer (k_write_items) and the export
-// kernels (export_kernels.cu) all address the database through these maps, so every writer and reader agrees on the layouts.
-// The maps are __host__ __device__ and use no CUDA types: tests/cpp/db_layout_inverse.cpp checks on the CPU that place and
-// fetch are mutually inverse and that no two items share a byte.
+// (loading.rs:34-41 pack_ntt_poly).  The single-item upsert, the batched raw-byte writer (k_write_items) and the export
+// kernels (export_kernels.cu) all address the database through these maps, so every writer and reader agrees on the layouts;
+// the host sizes the store with db_bytes.  The maps are __host__ __device__ and use no CUDA types:
+// tests/cpp/db_layout_inverse.cpp checks on the CPU that place and fetch are mutually inverse, that no two items share a
+// byte and that every byte a writer touches lies inside db_bytes.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -115,6 +116,32 @@ TC5_HD uint64_t fetch_tc5(const Tc5Geom& T, const uint8_t* dbt, int slice, int i
     for (int l = 0; l < 4; l++) w |= (uint64_t)plane[tc5_in_plane(T, il, j, l)] << (32 * n + 7 * l);
   }
   return w;
+}
+
+// ---- one database as every writer and reader sees it: its layout, the geometries of the three layouts (local rows) and its
+// store, db_bytes(layout, slices) bytes at `base` (cudaMalloc's 256-byte alignment covers the uint4 view of format 0)
+struct DbLayout {
+  int format;               // 0: IMAD cells, 1: mma.sync fragments, 2: wgmma tile images
+  MulGeom G; ImmaGeom F; Tc5Geom T;
+  uint8_t* base;
+};
+// bytes of the first `slices` slices of the store; every size and slice offset of a store is counted here, in bytes
+TC5_HD size_t db_bytes(const DbLayout& L, int slices) {
+  if (L.format == 0) return imad_cell(L.G, slices, 0, 0, 0) * 16;
+  if (L.format == 2) return limb_plane(L.T.mt, L.T.ks, TC5_TILE, slices, 0, 0);
+  return limb_plane(L.F.mt, L.F.ks, FRAG_GROUP, slices, 0, 0);
+}
+TC5_HD size_t slice_bytes(const DbLayout& L) { return db_bytes(L, 1); }
+
+TC5_HD void place_item(const DbLayout& L, int slice, int il, int j, int z, uint32_t lo, uint32_t hi) {
+  if (L.format == 0) place_imad(L.G, reinterpret_cast<uint32_t*>(L.base), slice, il, j, z, lo, hi);
+  else if (L.format == 2) place_tc5(L.T, L.base, slice, il, j, z, lo, hi);
+  else place_frag(L.F, L.base, slice, il, j, z, lo, hi);
+}
+TC5_HD uint64_t fetch_item(const DbLayout& L, int slice, int il, int j, int z) {
+  if (L.format == 0) return fetch_imad(L.G, reinterpret_cast<const uint32_t*>(L.base), slice, il, j, z);
+  if (L.format == 2) return fetch_tc5(L.T, L.base, slice, il, j, z);
+  return fetch_frag(L.F, L.base, slice, il, j, z);
 }
 
 }  // namespace b200pir

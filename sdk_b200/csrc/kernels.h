@@ -8,7 +8,7 @@
 //   matrices   : row-major [row][col] of polys, as PolyMatrixRaw / PolyMatrixNTT (poly.rs:59-71)
 #pragma once
 #include "common.cuh"
-#include "item_place.cuh"    // POLY, MulGeom, ImmaGeom and where an item lives in each layout
+#include "item_place.cuh"    // POLY, MulGeom, ImmaGeom, DbLayout and where an item lives in each layout
 
 namespace b200pir {
 
@@ -67,22 +67,18 @@ struct Shard { int index, count; };
 // reference layout u64 [zc][num_per_global][dim0] (z in [z0,z0+zc))  ->  db_dev slice (local rows)
 void launch_db_retile_chunk(const MulGeom& G, Shard sh, uint4* db_dev_slice, const uint64_t* ref_chunk, int z0, int zc,
                             cudaStream_t s);
-// one item poly (2048 packed words, lo|hi<<32) -> its place in db_dev   (lib/server db/loading.rs:317-359)
-void launch_db_upsert(const MulGeom& G, uint4* db_dev, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
 // synthetic DB: plaintext coeff = splitmix64(seed, ((slice*items + item)*2048 + z)) % p, recentred, NTT'd, packed
 // (server.rs:223-275 with a counter PRNG; item = j*num_per_global + ii)
 void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_dev, uint64_t seed, uint64_t pt_modulus,
                      int slice_begin, int slice_count, cudaStream_t s);
 
 // ---- first dimension on INT8 tensor cores (imma_kernels.cu): database in MMA fragment order
-size_t imma_db_cells(const ImmaGeom& F, int slices);      // uint4 cells of the whole database
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
 bool imma_supports_16(const ImmaGeom& F);                 // 16 queries per database pass fit one CTA's shared memory
 inline int imma_query_tiles(int nq) { return nq > 8 ? 4 : (nq > 4 ? 2 : 1); }   // column tiles of 4 queries
 void upload_imma_constants(const Twiddle* lo);
 // one slice in the IMAD layout (uint4 [row][jp][z]) -> fragment order
 void launch_db_to_frag(const ImmaGeom& F, const uint4* db0_slice, uint4* dbf, int slice, cudaStream_t s);
-void launch_db_upsert_frag(const ImmaGeom& F, uint4* dbf, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s);
 // out_zm: u32 [query][slice][n][z][row][ct_row]  (queries out_stride words apart)
 void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* dbf, const uint2* qf, uint32_t* out_zm,
@@ -94,11 +90,9 @@ void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32
 void launch_zmajor_to_ntt32(const ImmaGeom& F, const uint32_t* in_zm, uint32_t* out, int slice, cudaStream_t s);
 
 // ---- first dimension on wgmma (tc5_kernels.cu): operands stored as shared-memory tile images (database format 2)
-size_t tc5_db_bytes(const Tc5Geom& T, int slices);
 size_t tc5_query_bytes(const Tc5Geom& T);                 // 16 queries
 bool tc5_supported(const Tc5Geom& T);
 void launch_db_to_tc5(const Tc5Geom& T, const uint4* db0_slice, uint8_t* dbt, int slice, cudaStream_t s);
-void launch_db_upsert_tc5(const Tc5Geom& T, uint8_t* dbt, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
 void launch_query_to_tc5(const Tc5Geom& T, const uint4* q_dev, size_t q_stride, int nq, uint8_t* qt, cudaStream_t s);
 // out_zm as launch_multiply_imma; up to 16 queries per pass; one persistent CTA per SM
 // reorient_reg_ciphertexts (util.rs:323-355) fused with the re-tiling: expansion workspace v (ntt32 [query][slot][row][n][z]) ->
@@ -109,22 +103,19 @@ void launch_reorient_to_tc5(const Tc5Geom& T, const uint32_t* v, size_t v_stride
 void launch_multiply_tc5(const DevParams& P, const Tc5Geom& T, const uint8_t* dbt, const uint32_t* tile_mask, const uint8_t* qt,
                          uint32_t* out_zm, size_t out_stride, int nq, int slice_begin, int slice_count, int sm_count, cudaStream_t s);
 
-// ---- raw item bytes -> database (lib/server db/loading.rs:317-359 update_item_raw, batched)
-// One database as the writer sees it: its layout and the geometry / storage of that layout (local rows).
-struct DbDst {
-  int format;               // 0: d (IMAD layout), 1: f (mma.sync fragments), 2: t (wgmma tile images)
-  MulGeom G; ImmaGeom F; Tc5Geom T;
-  uint4* d; uint4* f; uint8_t* t;
-};
+// ---- writes into a database, in any layout (DbLayout, item_place.cuh; mul_kernels.cu)
+// one item poly (2048 packed words, lo|hi<<32) -> its place at (slice, local row il, column j)   (lib/server db/loading.rs:317-359)
+void launch_db_upsert(const DbLayout& L, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
+// raw item bytes -> database (loading.rs:317-359 update_item_raw, batched)
 // item = the raw bytes [off, off + len) of the staged buffer, written to local row il, column j of every slice
 struct ItemWrite { uint32_t off, len, il, j; };
 // every (item, chunk c < chunks) pair: chunk c = bytes [c * bpc, (c + 1) * bpc) of the item, zero past its len, converted
 // (recenter_mod, NTT, pack: loading.rs:278-299, 34-41) and placed at the item's cell of slice c.  One launch.
-void launch_write_items(const DevParams& P, const DbDst& D, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
+void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
                         int bpc, uint64_t pt_modulus, cudaStream_t s);
 // ---- database export (export_kernels.cu), the inverse of the loaders: the local rows of slice `slice` at z in [z0, z0 + zc) ->
 // out u64 [zc][rows][dim0] (the reference layout [z][ii][j] restricted to this GPU's rows), words lo | hi << 32.  One launch.
-void launch_db_export(const DbDst& D, int slice, int z0, int zc, uint64_t* out, cudaStream_t s);
+void launch_db_export(const DbLayout& L, int slice, int z0, int zc, uint64_t* out, cudaStream_t s);
 
 // ---- second dimension
 // mult output ntt32 [cnt][r][n][z] -> raw ciphertexts u64 [cnt][r][z]   (server.rs:707-709)

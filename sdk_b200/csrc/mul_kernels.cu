@@ -155,13 +155,6 @@ __global__ void k_db_retile(MulGeom G, Shard sh, uint4* db_slice, const uint64_t
       make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
 }
 
-__global__ void k_db_upsert(MulGeom G, uint4* db, int slice, int ii, int j, const uint64_t* poly) {
-  int z = blockIdx.x * blockDim.x + threadIdx.x;
-  if (z >= POLY) return;
-  const uint64_t w = poly[z];
-  place_imad(G, reinterpret_cast<uint32_t*>(db), slice, ii, j, z, (uint32_t)w, (uint32_t)(w >> 32));
-}
-
 __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index) {
   uint64_t z = seed + (index + 1) * 0x9E3779B97F4A7C15ULL;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
@@ -211,7 +204,7 @@ k_db_synth(DevParams P, MulGeom G, Shard sh, uint4* db, uint64_t seed, uint64_t 
 // two residues go straight to the item's place in the database of slice c.  512 threads: one 256-thread group per modulus;
 // 2 CTAs per SM (64 registers, no spills on sm_90a).
 __global__ void __launch_bounds__(512, 2)
-k_write_items(DevParams P, DbDst D, const uint8_t* __restrict__ bytes, const ItemWrite* __restrict__ items, int bpc, uint64_t pt) {
+k_write_items(DevParams P, DbLayout L, const uint8_t* __restrict__ bytes, const ItemWrite* __restrict__ items, int bpc, uint64_t pt) {
   __shared__ __align__(16) uint32_t ntt_smem[2 * NTT_SMEM_WORDS];
   __shared__ uint32_t halves[2][POLY];
   const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
@@ -233,12 +226,15 @@ k_write_items(DevParams P, DbDst D, const uint8_t* __restrict__ bytes, const Ite
   for (int k = 0; k < 8; k++) halves[n][tid * 8 + k] = x[k];
   __syncthreads();
   const int il = (int)it.il, j = (int)it.j;
-  for (int z = threadIdx.x; z < POLY; z += 512) {
-    const uint32_t lo = halves[0][z], hi = halves[1][z];
-    if (D.format == 0) place_imad(D.G, reinterpret_cast<uint32_t*>(D.d), slice, il, j, z, lo, hi);
-    else if (D.format == 2) place_tc5(D.T, D.t, slice, il, j, z, lo, hi);
-    else place_frag(D.F, reinterpret_cast<uint8_t*>(D.f), slice, il, j, z, lo, hi);
-  }
+  for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, il, j, z, halves[0][z], halves[1][z]);
+}
+
+// one item polynomial (2048 packed words lo|hi<<32) into the database, in any layout
+__global__ void k_db_upsert(DbLayout L, int slice, int il, int j, const uint64_t* poly) {
+  const int z = blockIdx.x * blockDim.x + threadIdx.x;
+  if (z >= POLY) return;
+  const uint64_t w = poly[z];
+  place_item(L, slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
 }
 
 // ------------------------------------------------------------------ DoublePIR
@@ -462,16 +458,16 @@ void launch_db_retile_chunk(const MulGeom& G, Shard sh, uint4* db_dev_slice, con
   ++g_kernel_launches;
   k_db_retile<<<grid1d(total, 256), 256, 0, s>>>(G, sh, db_dev_slice, ref_chunk, z0, zc);
 }
-void launch_db_upsert(const MulGeom& G, uint4* db_dev, int slice, int il, int j, const uint64_t* poly, cudaStream_t s) {
+void launch_db_upsert(const DbLayout& L, int slice, int il, int j, const uint64_t* poly, cudaStream_t s) {
   ++g_kernel_launches;
-  k_db_upsert<<<POLY / 256, 256, 0, s>>>(G, db_dev, slice, il, j, poly);
+  k_db_upsert<<<POLY / 256, 256, 0, s>>>(L, slice, il, j, poly);
 }
-void launch_write_items(const DevParams& P, const DbDst& D, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
+void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
                         int bpc, uint64_t pt_modulus, cudaStream_t s) {
   if (count == 0) return;
   if (chunks > 65535) throw Error(-2, "write_items: more than 65535 slices");
   ++g_kernel_launches;
-  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, D, bytes, items, bpc, pt_modulus);
+  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, bytes, items, bpc, pt_modulus);
 }
 void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_dev, uint64_t seed, uint64_t pt_modulus,
                      int slice_begin, int slice_count, cudaStream_t s) {

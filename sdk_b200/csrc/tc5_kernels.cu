@@ -57,14 +57,6 @@ k_db_to_tc5(Tc5Geom T, const uint4* __restrict__ db0_slice, uint8_t* __restrict_
   for (int n = 0; n < 2; n++) tc5_db_store(dbt + tc5_db_tile(T, slice, n, z, mt, ks) * TC5_TILE, t, res[n]);
 }
 
-// one item polynomial (2048 packed words lo|hi<<32) into the tile images (byte writes)
-__global__ void k_db_upsert_tc5(Tc5Geom T, uint8_t* dbt, int slice, int il, int j, const uint64_t* poly) {
-  const int z = blockIdx.x * blockDim.x + threadIdx.x;
-  if (z >= POLY) return;
-  const uint64_t w = poly[z];
-  place_tc5(T, dbt, slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
-}
-
 // expanded queries (uint4 [j][z] per query, q_stride apart) -> qT.  CTA = (pair of z, ks): every 32-byte sector it reads is
 // fully used; the four 4 KiB tiles (2 z x 2 n) are assembled in shared memory and written out contiguously.
 __global__ void __launch_bounds__(256)
@@ -274,7 +266,6 @@ k_multiply_tc5(DevParams P, Tc5Geom T, const uint8_t* __restrict__ dbt, const ui
 
 }  // namespace
 
-size_t tc5_db_bytes(const Tc5Geom& T, int slices) { return (size_t)slices * 2 * POLY * T.mt * T.ks * TC5_TILE; }
 size_t tc5_query_bytes(const Tc5Geom& T) { return (size_t)2 * POLY * T.ks * TC5_TILE; }
 static size_t tc5_smem_bytes(const Tc5Geom& T, int ksps, int bbufs) {
   return (size_t)bbufs * T.ks * TC5_TILE + (size_t)tc5_ring_stages(T.ks, ksps, bbufs) * ksps * TC5_TILE + sizeof(Tc5Smem) + 16;
@@ -285,10 +276,6 @@ bool tc5_supported(const Tc5Geom& T) { return T.dim0 % 2 == 0 && tc5_ring_stages
 void launch_db_to_tc5(const Tc5Geom& T, const uint4* db0_slice, uint8_t* dbt, int slice, cudaStream_t s) {
   ++g_kernel_launches;
   k_db_to_tc5<<<dim3(POLY, T.mt, T.ks), 256, 0, s>>>(T, db0_slice, dbt, slice);
-}
-void launch_db_upsert_tc5(const Tc5Geom& T, uint8_t* dbt, int slice, int il, int j, const uint64_t* poly, cudaStream_t s) {
-  ++g_kernel_launches;
-  k_db_upsert_tc5<<<POLY / 256, 256, 0, s>>>(T, dbt, slice, il, j, poly);
 }
 void launch_query_to_tc5(const Tc5Geom& T, const uint4* q_dev, size_t q_stride, int nq, uint8_t* qt, cudaStream_t s) {
   if (nq < 1 || nq > 16) throw Error(-2, "wgmma multiply: 1..16 queries per pass");

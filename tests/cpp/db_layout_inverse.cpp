@@ -1,10 +1,12 @@
 // The item maps of sdk_b200/csrc/item_place.cuh, on the CPU: for every geometry, every (il, j) and several z,
+//   - db_bytes is each layout's store size in bytes, as restated here, and slice_bytes is its share of one slice;
+//   - every byte an item is placed at, and every byte the bulk slice writers address, lies inside db_bytes;
 //   - the bytes different items (and moduli, limbs, z) occupy never overlap, in all three layouts;
-//   - fetch(place(w)) == w for canonical residues, including the all-(q - 1) words, and an unwritten cell fetches as 0;
+//   - fetch_item(place_item(w)) == w for canonical residues, including the all-(q - 1) words, and an unwritten cell fetches as 0;
 //   - the four limb-l bytes of j = 4 kq .. 4 kq + 3 are one 4-byte word at frag_word / tc5_word (what the export kernels read),
 //     and join_limb_words recovers the residues from those words.
-// place/fetch run on whole buffers where a slice fits in 64 MiB; for the larger geometries the same checks run on the per-plane
-// maps they are built from (frag_in_plane / tc5_in_plane inside one (slice, n, z) plane, imad_word for format 0).
+// place_item/fetch_item run on whole stores where the database is small enough; for the larger geometries the same checks run on
+// the per-plane maps they are built from (frag_in_plane / tc5_in_plane inside one (slice, n, z) plane, imad_word for format 0).
 #include "../../sdk_b200/csrc/item_place.cuh"
 #include <algorithm>
 #include <cstdio>
@@ -39,6 +41,36 @@ static void check_geometry(int dim0, int rows) {
   const MulGeom G{dim0, rows, slices};
   const ImmaGeom F = make_imma_geom(dim0, rows);
   const Tc5Geom T = make_tc5_geom(dim0, rows);
+  DbLayout L[3] = {{0, G, F, T, nullptr}, {1, G, F, T, nullptr}, {2, G, F, T, nullptr}};
+  // ---- store sizes in bytes: format 0 is slices x rows x dim0/2 x 2048 16-byte cells, format 1 slices x 2 x 2048 x mt x ks
+  // groups of 4 x 32 16-byte fragments, format 2 slices x 2 x 2048 x mt x ks 4096-byte tile images
+  {
+    const size_t want[3] = {(size_t)slices * rows * (dim0 / 2) * POLY * 16, (size_t)slices * 2 * POLY * F.mt * F.ks * 4 * 32 * 16,
+                            (size_t)slices * 2 * POLY * T.mt * T.ks * 4096};
+    for (int f = 0; f < 3; f++) {
+      CHECK(db_bytes(L[f], slices) == want[f], "format %d: db_bytes %zu, want %zu (dim0 %d rows %d)", f, db_bytes(L[f], slices),
+            want[f], dim0, rows);
+      CHECK(slice_bytes(L[f]) * slices == want[f], "format %d: slice_bytes (dim0 %d rows %d)", f, dim0, rows);
+    }
+  }
+  // ---- the bulk writers stay inside the store: the format-0 slice builders (k_db_retile, k_db_synth) write the cells of
+  // imad_cell, ending at slices * slice_bytes; the re-tilers write slice s of formats 1 (k_db_to_frag's address, restated) and 2
+  // (tc5_db_tile) within [s, s + 1) * slice_bytes
+  CHECK((imad_cell(G, slices - 1, rows - 1, dim0 - 1, POLY - 1) + 1) * 16 <= slices * slice_bytes(L[0]) &&
+        slices * slice_bytes(L[0]) <= db_bytes(L[0], slices), "format 0 slice builders past the store (dim0 %d rows %d)", dim0, rows);
+  for (int s = 0; s < slices; s++) {
+    auto frag_cell = [&](int n, int z, int mt, int ks, int l, int lane) {
+      return (((((size_t)s * 2 + n) * POLY + z) * F.mt + mt) * F.ks + ks) * 4 * 32 + (size_t)l * 32 + lane;
+    };
+    const size_t lo[2] = {frag_cell(0, 0, 0, 0, 0, 0) * 16, tc5_db_tile(T, s, 0, 0, 0, 0) * TC5_TILE};
+    const size_t end[2] = {(frag_cell(1, POLY - 1, F.mt - 1, F.ks - 1, 3, 31) + 1) * 16,
+                           (tc5_db_tile(T, s, 1, POLY - 1, T.mt - 1, T.ks - 1) + 1) * TC5_TILE};
+    for (int f = 1; f < 3; f++)
+      CHECK(lo[f - 1] == s * slice_bytes(L[f]) && end[f - 1] <= (s + 1) * slice_bytes(L[f]) &&
+            (s + 1) * slice_bytes(L[f]) <= db_bytes(L[f], slices), "format %d re-tiler of slice %d past its slice (dim0 %d rows %d)",
+            f, s, dim0, rows);
+  }
+  if (failures) return;      // the stores below are db_bytes long: a wrong size would be written out of bounds
   // ---- disjointness of every byte of every item at the chosen z (both slices' planes of z, both moduli, all limbs)
   {
     std::vector<size_t> o0, o1, o2;
@@ -54,11 +86,10 @@ static void check_geometry(int dim0, int rows) {
                 o2.push_back(tc5_plane(T, s, n, z) + tc5_in_plane(T, il, j, l));
               }
           }
-    const size_t cells0 = (size_t)slices * rows * (dim0 / 2) * POLY * 4;
-    const size_t bytes12[2] = {(size_t)slices * 2 * POLY * F.mt * F.ks * FRAG_GROUP, (size_t)slices * 2 * POLY * T.mt * T.ks * TC5_TILE};
-    CHECK(*std::max_element(o0.begin(), o0.end()) < cells0, "format 0 word out of the allocation");
-    CHECK(*std::max_element(o1.begin(), o1.end()) < bytes12[0], "format 1 byte out of the allocation");
-    CHECK(*std::max_element(o2.begin(), o2.end()) < bytes12[1], "format 2 byte out of the allocation");
+    // the bytes place_item writes: o0 holds u32 words
+    CHECK((*std::max_element(o0.begin(), o0.end()) + 1) * 4 <= db_bytes(L[0], slices), "format 0 word out of the store");
+    CHECK(*std::max_element(o1.begin(), o1.end()) < db_bytes(L[1], slices), "format 1 byte out of the store");
+    CHECK(*std::max_element(o2.begin(), o2.end()) < db_bytes(L[2], slices), "format 2 byte out of the store");
     no_overlap(o0, "format 0", dim0, rows);
     no_overlap(o1, "format 1", dim0, rows);
     no_overlap(o2, "format 2", dim0, rows);
@@ -79,11 +110,17 @@ static void check_geometry(int dim0, int rows) {
     join_limb_words(w, back);
     for (int i = 0; i < 4; i++) CHECK(back[i] == r[i], "join_limb_words");
   }
-  // ---- fetch(place(w)) == w
+  // ---- fetch_item(place_item(w)) == w, on stores of exactly db_bytes followed by a guard no write may reach
   const size_t items = (size_t)rows * dim0;
   if (items * POLY * 8 * slices <= ((size_t)64 << 20)) {
-    std::vector<uint32_t> d0((size_t)slices * rows * (dim0 / 2) * POLY * 4, 0);
-    std::vector<uint8_t> d1((size_t)slices * 2 * POLY * F.mt * F.ks * FRAG_GROUP, 0), d2((size_t)slices * 2 * POLY * T.mt * T.ks * TC5_TILE, 0);
+    const size_t guard = 4096;
+    std::vector<uint32_t> store[3];
+    for (int f = 0; f < 3; f++) {
+      store[f].assign((db_bytes(L[f], slices) + guard) / 4, 0);
+      // a placed residue (< 2^28) or limb byte (< 2^7) never leaves a guard word all ones
+      std::fill(store[f].end() - guard / 4, store[f].end(), 0xFFFFFFFFu);
+      L[f].base = reinterpret_cast<uint8_t*>(store[f].data());
+    }
     // every second item stays unwritten
     rng_state = 0x9E3779B97F4A7C15ull;
     for (int z : zs)
@@ -91,21 +128,21 @@ static void check_geometry(int dim0, int rows) {
         for (int j = 0; j < dim0; j++) {
           if ((il + j) & 1) continue;
           const uint64_t w = word_for(il, j, z);
-          place_imad(G, d0.data(), slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
-          place_frag(F, d1.data(), slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
-          place_tc5(T, d2.data(), slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
+          for (int f = 0; f < 3; f++) place_item(L[f], slice, il, j, z, (uint32_t)w, (uint32_t)(w >> 32));
         }
+    for (int f = 0; f < 3; f++)
+      CHECK(std::all_of(store[f].end() - guard / 4, store[f].end(), [](uint32_t v) { return v == 0xFFFFFFFFu; }),
+            "format %d: place_item wrote past db_bytes (dim0 %d rows %d)", f, dim0, rows);
     rng_state = 0x9E3779B97F4A7C15ull;
     for (int z : zs)
       for (int il = 0; il < rows; il++)
         for (int j = 0; j < dim0; j++) {
           const bool written = !((il + j) & 1);
           const uint64_t w = written ? word_for(il, j, z) : 0;
-          CHECK(fetch_imad(G, d0.data(), slice, il, j, z) == w, "format 0 (%d,%d) il %d j %d z %d", dim0, rows, il, j, z);
-          CHECK(fetch_frag(F, d1.data(), slice, il, j, z) == w, "format 1 (%d,%d) il %d j %d z %d", dim0, rows, il, j, z);
-          CHECK(fetch_tc5(T, d2.data(), slice, il, j, z) == w, "format 2 (%d,%d) il %d j %d z %d", dim0, rows, il, j, z);
-          CHECK(fetch_imad(G, d0.data(), 0, il, j, z) == 0 && fetch_frag(F, d1.data(), 0, il, j, z) == 0 &&
-                fetch_tc5(T, d2.data(), 0, il, j, z) == 0, "slice 0 is unwritten");
+          for (int f = 0; f < 3; f++) {
+            CHECK(fetch_item(L[f], slice, il, j, z) == w, "format %d (%d,%d) il %d j %d z %d", f, dim0, rows, il, j, z);
+            CHECK(fetch_item(L[f], 0, il, j, z) == 0, "format %d: slice 0 is unwritten", f);
+          }
         }
   } else {
     // one (slice, n, z) plane of each limb layout at a time: the in-plane maps the whole-buffer functions add the plane base to
