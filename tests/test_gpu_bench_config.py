@@ -1,7 +1,8 @@
 """The bench configuration itself (BASELINE.json configs[1]: S8 = 2^17 items x 8 KiB = 1 GiB of plaintext, 8 GiB in HBM,
 nu_2 = 8: the 256-row fold tree, the 16-queries-per-pass first dimension) — size-independent property at full size: the
 decoded response equals the planted plaintext, recomputed from the counter PRNG the GPU database generator uses
-(the generator itself is checked against the oracle's at small size in test_gpu_parity.py).  Also DoublePIR config #4 and the
+(the generator itself is checked against the oracle's at small size in test_gpu_parity.py).  S8's bytes, stage by stage and
+end to end, are compared with the oracle's in test_gpu_deep_geometry_parity.py.  Also DoublePIR config #4 and the
 NTT sweep of config #5 at full size against oracle samples (DoublePIR at 2^23 rows: the 2^24-row matrix, 91.7 GB, does not
 fit an 80 GB H100)."""
 import numpy as np
