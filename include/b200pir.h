@@ -347,9 +347,17 @@ int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out);
 
 /* ---- DoublePIR online: answer() served from HBM ---------------------------------------------------------------------------- */
 typedef struct b200pir_dpir_server b200pir_dpir_server;
-/* matrix_mul_vec_packed (kernels.rs:118-178) for `count` vectors in one pass over the matrix: b = count x 3*cols u32, out =
- * count x rows u32, host buffers, on the handle's stream.  Null pointers -> B200PIR_E_BADARG. */
+/* matrix_mul_vec_packed (kernels.rs:118-178) for `count` vectors: b = count x 3*cols u32, out = count x rows u32, host buffers,
+ * on the handle's stream.  The matrix is read once per pass of up to 64 vectors on the tensor cores, or of up to 16 on the
+ * integer kernel; the kernel is chosen as the answer path chooses it.  Null pointers -> B200PIR_E_BADARG. */
 int b200pir_dpir_matvec_packed_many(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out);
+/* The same on a named kernel, for tests and measurements: B200PIR_DPIR_MV_AUTO (as above), B200PIR_DPIR_MV_MULTI (the integer
+ * kernel, 16 vectors a pass) or B200PIR_DPIR_MV_TC (the tensor cores, 64 vectors a pass).  Results do not depend on the kernel.
+ * Another value -> B200PIR_E_BADARG. */
+#define B200PIR_DPIR_MV_AUTO 0
+#define B200PIR_DPIR_MV_MULTI 1
+#define B200PIR_DPIR_MV_TC 2
+int b200pir_dpir_matvec_packed_many_on(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out, int kernel);
 /* The state DoublePirServer::answer reads (doublepir/server.rs:201-247): `db` (borrowed: the handle of b200pir_dpir_load, or
  * b200pir_dpir_create of a `.dbp`, or of one chunk's rows for a chunked server; it must outlive the server) plus server_state =
  * [h_1, a_2^T] (doublepir.rs:104-106) as b200pir_dpir_load / b200pir_dpir_setup return them, uploaded once: h1_squished
@@ -379,7 +387,8 @@ int b200pir_dpir_answer_size(b200pir_dpir_server* s, const uint8_t* request, siz
 int b200pir_dpir_answer(b200pir_dpir_server* s, const uint8_t* request, size_t len, int64_t chunk_idx, uint8_t* out,
                         size_t* out_len);
 /* `count` independent requests of different clients, unchunked, in one call: response i is byte for byte answer(requests[i]);
- * the database is read once per pass of up to 16 requests and h_1 once per 16 q_2 vectors of the call.  out_lens[i]: capacity
+ * the database is read once per pass of up to 64 requests and h_1 once per 64 q_2 vectors of the call, on the tensor cores;
+ * a pass of 8 or fewer vectors runs on the integer kernel, 16 a pass (DESIGN §4.5).  out_lens[i]: capacity
  * of outs[i] on entry, response length on return.  Errors as b200pir_dpir_answer (the query limit counts every request); on an
  * error nothing is written to any output. */
 int b200pir_dpir_answer_many(b200pir_dpir_server* s, const uint8_t* const* requests, const size_t* lens, size_t count,

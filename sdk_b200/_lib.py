@@ -118,6 +118,7 @@ def _load():
                                         C.POINTER(vp), u32p, u32p, u32p]),
         "b200pir_dpir_download": (C.c_int, [vp, u32p]),
         "b200pir_dpir_matvec_packed_many": (C.c_int, [vp, u32p, C.c_size_t, u32p]),
+        "b200pir_dpir_matvec_packed_many_on": (C.c_int, [vp, u32p, C.c_size_t, u32p, C.c_int]),
         "b200pir_dpir_server_create": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, vp, u32p, u32p, C.c_size_t,
                                                  C.POINTER(vp)]),
         "b200pir_dpir_server_destroy": (None, [vp]),

@@ -2370,6 +2370,8 @@ struct b200pir_dpir_server {
   uint8_t* h_resp = nullptr;
   DevBuf<uint8_t> d_stage, d_resp;
   DevBuf<uint32_t> d_a1, d_a1sq, d_msg0;
+  DevBuf<uint8_t> d_img;         // query images of the passes that run on the tensor cores (every q_1, then every q_2)
+  size_t img_q1 = 0, img_q2 = 0; // bytes of one q_1 / q_2 image
   ~b200pir_dpir_server() {
     if (h_stage) cudaFreeHost(h_stage);
     if (h_resp) cudaFreeHost(h_resp);
@@ -2386,6 +2388,7 @@ struct DpirCall {               // one request of a call
   DpirResponseLayout L;
   size_t resp_off = 0;          // byte offset of its response in d_resp
   std::vector<const uint32_t*> q1, q2;   // device addresses of its staged vectors ([k], [k * e + j]); q1[k] null when not read
+  std::vector<const uint32_t*> q1i, q2i; // the same vectors' query images, for passes on the tensor cores
 };
 
 // Parse + the checks of doublepir.rs:246-350 for one request; chunk < 0: unchunked.
@@ -2424,20 +2427,47 @@ void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t ch
     resp_total += c.L.bytes();
   }
   if (resp_total > S->resp_cap) throw Error(B200PIR_E_SHAPE, "dpir: response workspace overflow");
+  // ---- which kernel each pass runs, from the vectors it holds and the matrix rows; the tensor-core passes read query images
+  uint64_t total_q = 0;
+  for (const auto& c : calls) total_q += c.w.queries;
+  const bool tc_db = dpir_use_tc(chunk >= 0 ? 1 : R, chunk >= 0 ? dpir_batch_rows(S->l, calls[0].w.queries, chunk) : S->l);
+  const bool tc_h1 = dpir_use_tc(total_q * S->e, S->rows1);
+  const size_t cap_db = tc_db ? DTC_VECS : kDpirMvMaxVecs, cap_h1 = tc_h1 ? DTC_VECS : kDpirMvMaxVecs;
+  std::vector<DpirTcImage> jobs;
+  {
+    size_t n1 = 0, n2 = 0;
+    for (auto& c : calls) {
+      c.q1i.assign(c.q1.size(), nullptr);
+      c.q2i.assign(c.q2.size(), nullptr);
+      for (size_t k = 0; tc_db && k < c.q1.size(); k++)
+        if (c.q1[k]) {
+          uint8_t* img = S->d_img.p + n1++ * S->img_q1;
+          jobs.push_back(DpirTcImage{c.q1[k], img, (uint32_t)S->dcols});
+          c.q1i[k] = reinterpret_cast<const uint32_t*>(img);
+        }
+      for (size_t k = 0; tc_h1 && k < c.q2.size(); k++) {
+        uint8_t* img = S->d_img.p + S->max_queries * S->img_q1 + n2++ * S->img_q2;
+        jobs.push_back(DpirTcImage{c.q2[k], img, (uint32_t)S->c1});
+        c.q2i[k] = reinterpret_cast<const uint32_t*>(img);
+      }
+    }
+    if (n1 > S->max_queries || n2 > S->max_queries * S->e) throw Error(B200PIR_E_SHAPE, "dpir: query image workspace overflow");
+  }
   // ---- task tables: database pass, h_1 pass, a_1' * q_2
   std::vector<DpirMvTask> tasks;
   std::vector<DpirMvVec> vecs;
   uint8_t* resp = S->d_resp.p;
-  auto add_tiles = [&](const uint32_t* a, uint64_t rows, uint64_t cols, uint32_t vec0, uint32_t nv) {
-    for (uint64_t t0 = 0; t0 < rows; t0 += kDpirMvRows)
-      tasks.push_back(DpirMvTask{a + t0 * cols, (uint32_t)std::min<uint64_t>(kDpirMvRows, rows - t0), vec0, nv, (uint32_t)t0});
+  auto add_tiles = [&](const uint32_t* a, uint64_t rows, uint64_t cols, uint32_t vec0, uint32_t nv, bool tc) {
+    const uint64_t tr = tc ? DTC_ROWS : kDpirMvRows;
+    for (uint64_t t0 = 0; t0 < rows; t0 += tr)
+      tasks.push_back(DpirMvTask{a + t0 * cols, (uint32_t)std::min<uint64_t>(tr, rows - t0), vec0, nv, (uint32_t)t0});
   };
   int vmax_db = 1, vmax_h1 = 1, vmax_a1 = 1;
   if (chunk >= 0) {             // one request: batch `chunk` from rows [0, its size) of the server's matrix
     const DpirCall& c = calls[0];
     const uint64_t nq = c.w.queries, rows = dpir_batch_rows(S->l, nq, chunk);
-    vecs.push_back(DpirMvVec{c.q1[chunk], S->d_a1.p + dpir_batch_begin(S->l, nq, chunk)});
-    add_tiles(S->db->a.p, rows, S->dcols, 0, 1);
+    vecs.push_back(DpirMvVec{tc_db ? c.q1i[chunk] : c.q1[chunk], S->d_a1.p + dpir_batch_begin(S->l, nq, chunk)});
+    add_tiles(S->db->a.p, rows, S->dcols, 0, 1, tc_db);
   } else {                      // the rows cut at every request's batch boundaries: one q_1 per request in each segment
     std::vector<uint64_t> cuts{0, S->l};
     for (const auto& c : calls)
@@ -2446,15 +2476,15 @@ void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t ch
     cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
     for (size_t g = 0; g + 1 < cuts.size(); g++) {
       const uint64_t s0 = cuts[g], s1 = cuts[g + 1];
-      for (size_t i0 = 0; i0 < R; i0 += kDpirMvMaxVecs) {
-        const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, R - i0);
+      for (size_t i0 = 0; i0 < R; i0 += cap_db) {
+        const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(cap_db, R - i0);
         for (size_t i = i0; i < i0 + nv; i++) {
           const uint64_t nq = calls[i].w.queries, bs = S->l / nq;
           const uint64_t k = bs ? std::min(s0 / bs, nq - 1) : nq - 1;
-          vecs.push_back(DpirMvVec{calls[i].q1[k], S->d_a1.p + i * S->l + s0});
+          vecs.push_back(DpirMvVec{tc_db ? calls[i].q1i[k] : calls[i].q1[k], S->d_a1.p + i * S->l + s0});
         }
         vmax_db = std::max<int>(vmax_db, nv);
-        add_tiles(S->db->a.p + s0 * S->dcols, s1 - s0, S->dcols, vec0, nv);
+        add_tiles(S->db->a.p + s0 * S->dcols, s1 - s0, S->dcols, vec0, nv, tc_db);
       }
     }
   }
@@ -2464,12 +2494,13 @@ void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t ch
     for (const auto& c : calls)
       for (size_t k = 0; k < c.w.queries; k++)
         for (size_t j = 0; j < S->e; j++)
-          all.push_back(DpirMvVec{c.q2[k * S->e + j], reinterpret_cast<uint32_t*>(resp + c.resp_off + c.L.a2_data(k, j))});
-    for (size_t v0 = 0; v0 < all.size(); v0 += kDpirMvMaxVecs) {
-      const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, all.size() - v0);
+          all.push_back(DpirMvVec{tc_h1 ? c.q2i[k * S->e + j] : c.q2[k * S->e + j],
+                                  reinterpret_cast<uint32_t*>(resp + c.resp_off + c.L.a2_data(k, j))});
+    for (size_t v0 = 0; v0 < all.size(); v0 += cap_h1) {
+      const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(cap_h1, all.size() - v0);
       vecs.insert(vecs.end(), all.begin() + v0, all.begin() + v0 + nv);
       vmax_h1 = std::max<int>(vmax_h1, nv);
-      add_tiles(S->h1.p, S->rows1, S->c1, vec0, nv);
+      add_tiles(S->h1.p, S->rows1, S->c1, vec0, nv, tc_h1);
     }
   }
   const size_t t_a1 = tasks.size();
@@ -2483,21 +2514,30 @@ void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t ch
       const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, mine.size() - v0);
       vecs.insert(vecs.end(), mine.begin() + v0, mine.begin() + v0 + nv);
       vmax_a1 = std::max<int>(vmax_a1, nv);
-      add_tiles(S->d_a1sq.p + i * S->dx * S->c1, S->dx, S->c1, vec0, nv);
+      add_tiles(S->d_a1sq.p + i * S->dx * S->c1, S->dx, S->c1, vec0, nv, false);
     }
   }
   if (tasks.size() > S->task_cap || vecs.size() > S->vec_cap) throw Error(B200PIR_E_SHAPE, "dpir: task table overflow");
   const size_t off_tasks = off, off_vecs = align_up(off_tasks + tasks.size() * sizeof(DpirMvTask), 16);
-  const size_t used = off_vecs + vecs.size() * sizeof(DpirMvVec);
+  const size_t off_jobs = align_up(off_vecs + vecs.size() * sizeof(DpirMvVec), 16);
+  const size_t used = off_jobs + jobs.size() * sizeof(DpirTcImage);
   if (used > S->stage_cap) throw Error(B200PIR_E_SHAPE, "dpir: staging overflow");
   std::memcpy(S->h_stage + off_tasks, tasks.data(), tasks.size() * sizeof(DpirMvTask));
   std::memcpy(S->h_stage + off_vecs, vecs.data(), vecs.size() * sizeof(DpirMvVec));
+  std::memcpy(S->h_stage + off_jobs, jobs.data(), jobs.size() * sizeof(DpirTcImage));
   const DpirMvTask* d_tasks = reinterpret_cast<const DpirMvTask*>(S->d_stage.p + off_tasks);
   const DpirMvVec* d_vecs = reinterpret_cast<const DpirMvVec*>(S->d_stage.p + off_vecs);
+  // the h_1 and a_1' passes store big-endian results, so they never split k; the database pass adds into zeroed a_1
+  auto pass = [&](bool tc, size_t t0, size_t t1, uint64_t cols, int vmax, bool split, int flags) {
+    if (tc) launch_dpir_matvec_tc(d_tasks + t0, t1 - t0, d_vecs, cols, split ? dpir_tc_ksplit(t1 - t0, cols, S->sm_count) : 1, flags, s);
+    else launch_dpir_matvec_multi(d_tasks + t0, t1 - t0, d_vecs, cols, vmax, split ? dpir_mv_ksplit(t1 - t0, cols, S->sm_count) : 1, flags, s);
+  };
   // ---- the passes
   B200_CUDA(cudaMemcpyAsync(S->d_stage.p, S->h_stage, used, cudaMemcpyHostToDevice, s));
   B200_CUDA(cudaMemsetAsync(S->d_a1.p, 0, R * S->l * 4, s));   // split-k partial sums add into it; unread batches stay zero
-  launch_dpir_matvec_multi(d_tasks, t_h1, d_vecs, S->dcols, vmax_db, dpir_mv_ksplit(t_h1, S->dcols, S->sm_count), DPIR_MV_B_BE, s);
+  launch_dpir_tc_image(reinterpret_cast<const DpirTcImage*>(S->d_stage.p + off_jobs), jobs.size(), std::max(S->dcols, S->c1),
+                       DPIR_MV_B_BE, s);
+  pass(tc_db, 0, t_h1, S->dcols, vmax_db, true, DPIR_MV_B_BE);
   for (size_t i = 0; i < R; i++)        // a_1.transpose_expand_concat_cols_squish(p, delta, x, 10, 3)
     launch_dpir_transpose_expand(S->d_a1sq.p + i * S->dx * S->c1, S->d_a1.p + i * S->l, S->l, 1, S->p, S->delta, S->x, S->dx,
                                  S->c1, s);
@@ -2506,8 +2546,8 @@ void dpir_serve(b200pir_dpir_server* S, std::vector<DpirCall>& calls, int64_t ch
   for (size_t i = 0; i < R; i++)
     launch_dpir_bswap(reinterpret_cast<uint32_t*>(resp + calls[i].resp_off + calls[i].L.msg0_data()), S->d_msg0.p + i * S->dx * S->n,
                       S->dx * S->n, s);
-  launch_dpir_matvec_multi(d_tasks + t_h1, t_a1 - t_h1, d_vecs, S->c1, vmax_h1, 1, DPIR_MV_B_BE | DPIR_MV_OUT_BE, s);
-  launch_dpir_matvec_multi(d_tasks + t_a1, tasks.size() - t_a1, d_vecs, S->c1, vmax_a1, 1, DPIR_MV_B_BE | DPIR_MV_OUT_BE, s);
+  pass(tc_h1, t_h1, t_a1, S->c1, vmax_h1, false, DPIR_MV_B_BE | DPIR_MV_OUT_BE);
+  pass(false, t_a1, tasks.size(), S->c1, vmax_a1, false, DPIR_MV_B_BE | DPIR_MV_OUT_BE);
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(S->h_resp, S->d_resp.p, resp_total, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
@@ -2548,13 +2588,16 @@ int b200pir_dpir_server_create(int device, const b200pir_dpir_params* params, ui
   } sg{S.get()};
   const uint64_t Q = max_queries, e = S->e;
   // bounds of one call: at most Q requests and Q queries; the database pass has at most Q row segments (each request of k
-  // queries adds k - 1 cuts), each tiled and repeated once per 16 requests
+  // queries adds k - 1 cuts), each tiled and repeated once per pass of vectors.  A pass on k_dpir_matvec_multi (32 rows a task,
+  // 16 vectors a pass) makes at least as many tasks as one on the tensor cores (64 rows, 64 vectors), so its count bounds both.
   S->task_cap = (ceil_div(l, kDpirMvRows) + Q) * ceil_div(Q, kDpirMvMaxVecs)
               + ceil_div(S->rows1, kDpirMvRows) * ceil_div(Q * e, kDpirMvMaxVecs)
               + ceil_div(S->dx, kDpirMvRows) * Q * e;
   S->vec_cap = Q * Q + 2 * Q * e;
   S->stage_cap = Q * (align_up(3 * S->dcols * 4, 16) + e * align_up(3 * S->c1 * 4, 16)) + align_up(S->task_cap * sizeof(DpirMvTask), 16)
-               + S->vec_cap * sizeof(DpirMvVec);
+               + align_up(S->vec_cap * sizeof(DpirMvVec), 16) + Q * (1 + e) * sizeof(DpirTcImage);
+  S->img_q1 = dtc_img_bytes(S->dcols);
+  S->img_q2 = dtc_img_bytes(S->c1);
   S->resp_cap = Q * (12 + S->dx * S->n * 4) + Q * e * DpirResponseLayout{1, e, S->dx, S->n, S->rows1}.pair_bytes();
   B200_CUDA(cudaMallocHost(&S->h_stage, S->stage_cap));
   B200_CUDA(cudaMallocHost(&S->h_resp, S->resp_cap));
@@ -2563,6 +2606,7 @@ int b200pir_dpir_server_create(int device, const b200pir_dpir_params* params, ui
   S->d_a1.alloc(Q * l);
   S->d_a1sq.alloc(Q * S->dx * S->c1);
   S->d_msg0.alloc(Q * S->dx * S->n);
+  S->d_img.alloc(Q * S->img_q1 + Q * e * S->img_q2);
   S->h1.alloc(S->rows1 * S->c1);
   S->a2t.alloc(S->n * S->lx3);
   B200_CUDA(cudaMemcpyAsync(S->h1.p, h1_squished, S->h1.n * 4, cudaMemcpyHostToDevice, S->stream));
@@ -2635,39 +2679,61 @@ int b200pir_dpir_answer_many(b200pir_dpir_server* S, const uint8_t* const* reque
   API_END
 }
 
-// matrix_mul_vec_packed for `count` vectors, one pass over the matrix per 16 (host buffers; the multi-vector kernel's test face)
-int b200pir_dpir_matvec_packed_many(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out) {
+// matrix_mul_vec_packed for `count` vectors, one pass over the matrix per 64 (tensor cores) or 16 (k_dpir_matvec_multi) of them
+// (host buffers; the multi-vector kernels' test face).  kernel: B200PIR_DPIR_MV_AUTO picks as the answer path does.
+int b200pir_dpir_matvec_packed_many_on(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out, int kernel) {
   API_BEGIN
   if (!m || !b || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  if (kernel != B200PIR_DPIR_MV_AUTO && kernel != B200PIR_DPIR_MV_MULTI && kernel != B200PIR_DPIR_MV_TC)
+    throw Error(B200PIR_E_BADARG, "unknown matvec kernel");
   if (count == 0) return 0;
   if (m->rows > 0xFFFFFFFFull || count > 0xFFFFFFFFull) throw Error(B200PIR_E_SHAPE, "too many rows or vectors");
   std::lock_guard<std::mutex> lk(m->mu);
   cudaSetDevice(m->device);
   int sms = 0;
   B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
+  const bool tc = kernel == B200PIR_DPIR_MV_TC || (kernel == B200PIR_DPIR_MV_AUTO && dpir_use_tc(count, m->rows));
+  const size_t cap = tc ? DTC_VECS : kDpirMvMaxVecs, task_rows = tc ? DTC_ROWS : kDpirMvRows, img = dtc_img_bytes(m->cols);
   DevBuf<uint32_t> d_b(count * 3 * m->cols), d_out(count * m->rows);
+  DevBuf<uint8_t> d_img(tc ? count * img : 0);
   std::vector<DpirMvTask> tasks;
   std::vector<DpirMvVec> vecs;
+  std::vector<DpirTcImage> jobs;
   int vmax = 1;
-  for (size_t v0 = 0; v0 < count; v0 += kDpirMvMaxVecs) {
-    const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(kDpirMvMaxVecs, count - v0);
-    for (size_t v = v0; v < v0 + nv; v++) vecs.push_back(DpirMvVec{d_b.p + v * 3 * m->cols, d_out.p + v * m->rows});
+  for (size_t v0 = 0; v0 < count; v0 += cap) {
+    const uint32_t vec0 = (uint32_t)vecs.size(), nv = (uint32_t)std::min<size_t>(cap, count - v0);
+    for (size_t v = v0; v < v0 + nv; v++) {
+      const uint32_t* bv = d_b.p + v * 3 * m->cols;
+      if (tc) jobs.push_back(DpirTcImage{bv, d_img.p + v * img, (uint32_t)m->cols});
+      vecs.push_back(DpirMvVec{tc ? reinterpret_cast<const uint32_t*>(d_img.p + v * img) : bv, d_out.p + v * m->rows});
+    }
     vmax = std::max<int>(vmax, nv);
-    for (uint64_t t0 = 0; t0 < m->rows; t0 += kDpirMvRows)
-      tasks.push_back(DpirMvTask{m->a.p + t0 * m->cols, (uint32_t)std::min<uint64_t>(kDpirMvRows, m->rows - t0), vec0, nv, (uint32_t)t0});
+    for (uint64_t t0 = 0; t0 < m->rows; t0 += task_rows)
+      tasks.push_back(DpirMvTask{m->a.p + t0 * m->cols, (uint32_t)std::min<uint64_t>(task_rows, m->rows - t0), vec0, nv, (uint32_t)t0});
   }
   DevBuf<DpirMvTask> d_tasks(tasks.size());
   DevBuf<DpirMvVec> d_vecs(vecs.size());
+  DevBuf<DpirTcImage> d_jobs(jobs.size());
   B200_CUDA(cudaMemcpyAsync(d_tasks.p, tasks.data(), tasks.size() * sizeof(DpirMvTask), cudaMemcpyHostToDevice, m->stream));
   B200_CUDA(cudaMemcpyAsync(d_vecs.p, vecs.data(), vecs.size() * sizeof(DpirMvVec), cudaMemcpyHostToDevice, m->stream));
+  if (tc) B200_CUDA(cudaMemcpyAsync(d_jobs.p, jobs.data(), jobs.size() * sizeof(DpirTcImage), cudaMemcpyHostToDevice, m->stream));
   B200_CUDA(cudaMemcpyAsync(d_b.p, b, d_b.n * 4, cudaMemcpyHostToDevice, m->stream));
   B200_CUDA(cudaMemsetAsync(d_out.p, 0, d_out.n * 4, m->stream));
-  launch_dpir_matvec_multi(d_tasks.p, tasks.size(), d_vecs.p, m->cols, vmax, dpir_mv_ksplit(tasks.size(), m->cols, sms), 0, m->stream);
+  if (tc) {
+    launch_dpir_tc_image(d_jobs.p, jobs.size(), m->cols, 0, m->stream);
+    launch_dpir_matvec_tc(d_tasks.p, tasks.size(), d_vecs.p, m->cols, dpir_tc_ksplit(tasks.size(), m->cols, sms), 0, m->stream);
+  } else {
+    launch_dpir_matvec_multi(d_tasks.p, tasks.size(), d_vecs.p, m->cols, vmax, dpir_mv_ksplit(tasks.size(), m->cols, sms), 0, m->stream);
+  }
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(out, d_out.p, d_out.n * 4, cudaMemcpyDeviceToHost, m->stream));
   B200_CUDA(cudaStreamSynchronize(m->stream));
   B200_CUDA(cudaGetLastError());
   API_END
+}
+
+int b200pir_dpir_matvec_packed_many(b200pir_dpir* m, const uint32_t* b, size_t count, uint32_t* out) {
+  return b200pir_dpir_matvec_packed_many_on(m, b, count, out, B200PIR_DPIR_MV_AUTO);
 }
 
 }  // extern "C"

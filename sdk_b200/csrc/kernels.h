@@ -9,6 +9,7 @@
 #pragma once
 #include "common.cuh"
 #include "item_place.cuh"    // POLY, MulGeom, ImmaGeom, DbLayout and where an item lives in each layout
+#include "dpir_tc_layout.cuh"   // DTC_ROWS, DTC_VECS, dtc_img_bytes
 
 namespace b200pir {
 
@@ -205,6 +206,18 @@ void launch_dpir_matvec_multi(const DpirMvTask* tasks, size_t ntasks, const Dpir
 int dpir_mv_ksplit(size_t ntasks, size_t cols, int sm_count);
 // dst[i] = byte-swapped src[i]
 void launch_dpir_bswap(uint32_t* dst, const uint32_t* src, size_t words, cudaStream_t s);
+
+// ---- the same passes on the tensor cores (dpir_tc.cu, index maps in dpir_tc_layout.cuh): tasks of up to DTC_ROWS rows and
+// DTC_VECS vectors, whose DpirMvVec::b points at the vector's query image (dtc_img_bytes(cols) bytes, 16-byte aligned) instead of
+// its words.  Flags and ksplit as launch_dpir_matvec_multi (DPIR_MV_B_BE is applied when the images are built).
+struct DpirTcImage { const uint32_t* b; uint8_t* img; uint32_t cols; };   // b: 3 * cols words -> img
+void launch_dpir_tc_image(const DpirTcImage* jobs, size_t njobs, size_t max_cols, int flags, cudaStream_t s);
+void launch_dpir_matvec_tc(const DpirMvTask* tasks, size_t ntasks, const DpirMvVec* vecs, size_t cols, int ksplit, int flags,
+                           cudaStream_t s);
+// the k split that gives `ntasks` tasks about four waves of one CTA an SM, each at least one 32-word chunk
+int dpir_tc_ksplit(size_t ntasks, size_t cols, int sm_count);
+// which kernel a pass of `nv` vectors (the most any task of the pass holds) over `rows` matrix rows runs on
+bool dpir_use_tc(size_t nv, size_t rows);
 
 // ---- DoublePIR offline setup (dpir_gemm.cu): doublepir.rs:76-108
 // c (rows x n_cols) = a (rows x k_dim, entries in [-2^15, 2^15) as wrapping u32) * b (k_dim x n_cols) mod 2^32; device pointers;

@@ -59,10 +59,20 @@ def matrix_mul_vec_packed(a, b, basis=10, compression=3):
 
 
 def matrix_mul_vec_packed_many(a, bs):
-    """matrix_mul_vec_packed(a, b) for every b of bs in one pass over a per 16 vectors: (len(bs), a.rows) uint32."""
+    """matrix_mul_vec_packed(a, b) for every b of bs, one pass over a per 64 vectors on the tensor cores (per 16 when too few
+    vectors make the integer kernel the faster one): (len(bs), a.rows) uint32."""
+    return _matvec_packed_many_on(a, bs, MV_AUTO)
+
+
+MV_AUTO, MV_MULTI, MV_TC = 0, 1, 2        # B200PIR_DPIR_MV_*
+
+
+def _matvec_packed_many_on(a, bs, kernel):
+    """matrix_mul_vec_packed_many on a named kernel (MV_MULTI: the integer kernel, MV_TC: the tensor cores): for tests and
+    measurements; the results do not depend on the kernel."""
     bs = np.ascontiguousarray(np.asarray(bs, dtype=np.uint32).reshape(-1, 3 * a.cols))
     out = np.zeros((bs.shape[0], a.rows), dtype=np.uint32)
-    check(LIB.b200pir_dpir_matvec_packed_many(a._h, bs.ctypes.data, bs.shape[0], out.ctypes.data))
+    check(LIB.b200pir_dpir_matvec_packed_many_on(a._h, bs.ctypes.data, bs.shape[0], out.ctypes.data, kernel))
     return out
 
 
@@ -183,7 +193,8 @@ class Server:
         return out.raw[:n.value]
 
     def answer_many(self, requests):
-        """answer() of every request (different clients, unchunked) in one call."""
+        """answer() of every request (different clients, unchunked) in one call: the database is read once per 64 requests on
+        the tensor cores (once per 16 when the call has 8 or fewer)."""
         requests = [bytes(r) for r in requests]
         k = len(requests)
         sizes = [self._size_or_zero(r) for r in requests]
