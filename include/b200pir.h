@@ -48,7 +48,11 @@ int b200pir_device_count(void);
 /* Params::init (params.rs:224-296): builds NTT tables, Barrett constants, v_neg1 on `device`. */
 int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** out);
 void b200pir_ctx_destroy(b200pir_ctx* ctx);
-/* Use an externally owned cudaStream_t (e.g. torch's current stream) for all work of this context. */
+/* Use an externally owned cudaStream_t for all work of this context from now on: a non-blocking stream of the caller's, or NULL
+ * for the legacy default stream (torch's current stream unless one is set).  Waits for the work already queued on the old
+ * stream, then destroys it if the context created it; the caller's stream must outlive the context or the next set_stream.
+ * Every kernel launch and copy of the context, host entry points included, then goes to that stream; the _dev entry points
+ * are ordered after whatever the caller queued there before the call. */
 int b200pir_ctx_set_stream(b200pir_ctx* ctx, void* cuda_stream);
 int b200pir_ctx_synchronize(b200pir_ctx* ctx);
 /* knobs: "mul_variant" (kernel tiling), "batch" (max queries per database pass: 1, 2, 4, 8 or 16;
@@ -63,8 +67,10 @@ int b200pir_ctx_synchronize(b200pir_ctx* ctx);
  * unknown keys -> B200PIR_E_BADARG */
 int b200pir_ctx_set_option(b200pir_ctx* ctx, const char* key, int64_t value);
 /* Size the context's workspace once, up front, for `queries` concurrent queries against a database with `rows_local`
- * second-dimension rows (num_per for an unsharded database): afterwards no entry point allocates device memory for batches up
- * to that size (the workspace otherwise grows on first use; coalesced single-query calls size it for 32 queries).
+ * second-dimension rows (num_per for an unsharded database): afterwards the query, expansion, first-dimension, fold, pack and
+ * response buffers are not reallocated for batches up to that size (the workspace otherwise grows on first use; coalesced
+ * single-query calls size it for 32 queries).  Three small buffers still grow on the first call with a larger batch than
+ * before: the expansion rounds' scratch, the first dimension's query tile images and the per-query parameter table.
  * B200PIR_E_CUDA when the device cannot hold it. */
 int b200pir_ctx_reserve(b200pir_ctx* ctx, size_t queries, size_t rows_local);
 /* params.setup_bytes / query_bytes / response length (params.rs:146-182, server.rs:476-481) */
@@ -153,7 +159,8 @@ void b200pir_pp_destroy(b200pir_pp* pp);
 /* ntt.rs:67-113 ntt_forward / :212-258 ntt_inverse over `count` polys of [2][2048] u64, in place. */
 int b200pir_ntt_forward(b200pir_ctx* ctx, uint64_t* polys, size_t count);
 int b200pir_ntt_inverse(b200pir_ctx* ctx, uint64_t* polys, size_t count);
-/* Device-resident batch (BASELINE config #5): `count` polys of u32 [2][2048] residues, in place, stream-ordered. */
+/* Device-resident batch (BASELINE config #5): `count` polys of u32 [2][2048] residues, in place, stream-ordered: enqueued on the
+ * context's stream, nothing synchronised, nothing allocated (the tables of both sizes are built by b200pir_ctx_create). */
 int b200pir_ntt32_dev(b200pir_ctx* ctx, uint32_t* polys_dev, size_t count, int inverse);
 /* BASELINE config #5, poly_len = 4096 (not a size the reference's parameterisation uses, util.rs:246): the same transform
  * definition (ntt.rs:67-113, :212-258) and table construction (ntt.rs:39-65) over the same two moduli.
@@ -216,8 +223,15 @@ int b200pir_coalesce_stats(b200pir_ctx* ctx, uint64_t* batches, uint64_t* querie
 int b200pir_process_query_batch(b200pir_ctx* ctx, b200pir_db* db, b200pir_pp* pp, const uint64_t* query_cts,
                                 size_t count, uint8_t* out, size_t* out_len_each);
 /* Device-resident variants for measurement and multi-GPU composition: inputs/outputs are DEVICE pointers
- * and nothing is synchronised (stream-ordered).  query_dev: count x PolyMatrixRaw(2,1) (u64);
- * out_dev: count x response_bytes. */
+ * and nothing is synchronised (stream-ordered): the call reads its inputs and writes its outputs in the order of the context's
+ * stream (b200pir_ctx_set_stream) and returns without waiting for that stream or the legacy default stream, so the caller
+ * may queue the input copies before the call and the output copies after it, on the same stream.  The same holds for the
+ * three-phase and stage _dev entry points below.  What may still block the host on first use: growing a workspace buffer
+ * (cudaFree of the smaller one waits for the whole device) on the first call with a larger batch than the context has served
+ * or reserved (b200pir_ctx_reserve, which lists the buffers it does not size), and a per-query parameter table whose contents
+ * changed (a different pp or count than the previous call: a small pageable copy, which the driver may stage synchronously).
+ * A warmed call, same pp and count as the previous one, does neither.
+ * query_dev: count x PolyMatrixRaw(2,1) (u64); out_dev: count x response_bytes. */
 int b200pir_process_query_batch_dev(b200pir_ctx* ctx, b200pir_db* db, b200pir_pp* pp, const uint64_t* query_cts_dev,
                                     size_t count, uint8_t* out_dev);
 /* Multi-GPU row sharding (DESIGN.md "multi-GPU"): stage A = expansion + first dimension + local fold rounds

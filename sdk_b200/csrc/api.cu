@@ -94,7 +94,7 @@ struct b200pir_ctx {
   int q1_bits;
   DevParams dp;
   DevBuf<Twiddle> d_tw;      // fwd0, inv0, fwd1, inv1, inv_lz0, inv_lz1
-  DevBuf<Twiddle> d_tw4k;    // same for poly_len 4096 (config #5 sweep), built on first use
+  DevBuf<Twiddle> d_tw4k;    // fwd0, inv0, fwd1, inv1 for poly_len 4096 (config #5 sweep)
   DevBuf<uint32_t> d_neg1;   // [11][2][2048] ntt32 (params.rs:98-107)
   // options
   int mul_variant = 0, max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
@@ -279,7 +279,9 @@ struct b200pir_db {
     present_count = 0;
     h_tile_mask.assign((size_t)ctx->slices * layout.T.mt, 0u);
     tile_mask.alloc(h_tile_mask.size());
-    B200_CUDA(cudaMemset(tile_mask.p, 0, h_tile_mask.size() * 4));
+    // on the context's stream: a cudaMemset would queue on the legacy default stream, behind whatever the caller has there,
+    // and could land after the first writer's mask upload on the context's stream
+    B200_CUDA(cudaMemsetAsync(tile_mask.p, 0, h_tile_mask.size() * 4, ctx->stream));
   }
   // one item written, host side only: returns true when its tile-mask word changed (the device copy is then stale)
   bool mark_host(int slice, int il, int j) {
@@ -676,21 +678,35 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   std::vector<Twiddle> l0, l1;                                     // relaxed-range inverse tables (ntt_core.cuh "lz")
   b200pir::tables::build_inverse_table_lz(q0, l0);
   b200pir::tables::build_inverse_table_lz(q1m, l1);
+  // Every table goes up on the context's own stream, which the synchronise at the end of this function waits for: copies on
+  // the legacy default stream would wait for whatever the caller has queued there, and a pageable cudaMemcpy may return
+  // before its data has landed, while the first transform below already runs on the non-blocking context stream.  The host
+  // vectors outlive that synchronise.
   c->d_tw.alloc(6 * POLY);
-  B200_CUDA(cudaMemcpy(c->d_tw.p + 4 * POLY, l0.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(c->d_tw.p + 5 * POLY, l1.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(c->d_tw.p, f0.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(c->d_tw.p + POLY, i0.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(c->d_tw.p + 2 * POLY, f1.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(c->d_tw.p + 3 * POLY, i1.data(), POLY * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  {
-    std::vector<Twiddle> lo(2 * 3 * 64);                           // [n][forward, inverse, relaxed-range inverse][64]
-    for (int i = 0; i < 64; i++) { lo[(0 * 3 + 0) * 64 + i] = f0[i]; lo[(0 * 3 + 1) * 64 + i] = i0[i]; lo[(0 * 3 + 2) * 64 + i] = l0[i];
-                                   lo[(1 * 3 + 0) * 64 + i] = f1[i]; lo[(1 * 3 + 1) * 64 + i] = i1[i]; lo[(1 * 3 + 2) * 64 + i] = l1[i]; }
-    upload_poly_constants(lo.data());
-    upload_mul_constants(lo.data());
-    upload_imma_constants(lo.data());
+  const size_t tw_bytes = POLY * sizeof(Twiddle);
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p + 4 * POLY, l0.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p + 5 * POLY, l1.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p, f0.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p + POLY, i0.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p + 2 * POLY, f1.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->d_tw.p + 3 * POLY, i1.data(), tw_bytes, cudaMemcpyHostToDevice, c->stream));
+  std::vector<Twiddle> lo(2 * 3 * 64);                             // [n][forward, inverse, relaxed-range inverse][64]
+  for (int i = 0; i < 64; i++) { lo[(0 * 3 + 0) * 64 + i] = f0[i]; lo[(0 * 3 + 1) * 64 + i] = i0[i]; lo[(0 * 3 + 2) * 64 + i] = l0[i];
+                                 lo[(1 * 3 + 0) * 64 + i] = f1[i]; lo[(1 * 3 + 1) * 64 + i] = i1[i]; lo[(1 * 3 + 2) * 64 + i] = l1[i]; }
+  upload_poly_constants(lo.data(), c->stream);
+  upload_mul_constants(lo.data(), c->stream);
+  upload_imma_constants(lo.data(), c->stream);
+  // poly_len = 4096 (config #5): built here rather than on the first b200pir_ntt4096_dev call, so that call neither allocates
+  // nor copies from the host
+  std::vector<Twiddle> tw4k;
+  for (const uint64_t q : {q0, q1m}) {
+    std::vector<Twiddle> f, i;
+    build_tables(q, f, i, 4096, 12);
+    tw4k.insert(tw4k.end(), f.begin(), f.end());
+    tw4k.insert(tw4k.end(), i.begin(), i.end());
   }
+  c->d_tw4k.alloc(tw4k.size());
+  B200_CUDA(cudaMemcpyAsync(c->d_tw4k.p, tw4k.data(), tw4k.size() * sizeof(Twiddle), cudaMemcpyHostToDevice, c->stream));
   DevParams& dp = c->dp;
   dp.q[0] = (uint32_t)q0; dp.q[1] = (uint32_t)q1m;
   dp.cr1[0] = (uint64_t)(((u128)1 << 64) / q0);
@@ -710,7 +726,7 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
       h[((size_t)i * 2 + 1) * POLY + idx] = (uint32_t)(q1m - 1);
     }
     c->d_neg1.alloc(h.size());
-    B200_CUDA(cudaMemcpy(c->d_neg1.p, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpyAsync(c->d_neg1.p, h.data(), h.size() * 4, cudaMemcpyHostToDevice, c->stream));
     launch_ntt32(dp, c->d_neg1.p, NTT_LOG_N, false, c->stream);
     B200_CUDA(cudaStreamSynchronize(c->stream));
   }
@@ -1339,29 +1355,13 @@ int b200pir_ntt32_dev(b200pir_ctx* c, uint32_t* polys_dev, size_t count, int inv
   API_END
 }
 
-// ---- poly_len = 4096 transforms (BASELINE config #5; not part of the reference's parameterisation, util.rs:246)
-namespace {
-const Twiddle* tables_4k(b200pir_ctx* c) {
-  if (!c->d_tw4k.p) {
-    const int N = 4096, LG = 12;
-    std::vector<Twiddle> all;
-    for (int n = 0; n < 2; n++) {
-      std::vector<Twiddle> f, i;
-      build_tables(c->dp.q[n], f, i, N, LG);
-      all.insert(all.end(), f.begin(), f.end());
-      all.insert(all.end(), i.begin(), i.end());
-    }
-    c->d_tw4k.alloc(all.size());
-    B200_CUDA(cudaMemcpy(c->d_tw4k.p, all.data(), all.size() * sizeof(Twiddle), cudaMemcpyHostToDevice));
-  }
-  return c->d_tw4k.p;
-}
-}  // namespace
+// ---- poly_len = 4096 transforms (BASELINE config #5; not part of the reference's parameterisation, util.rs:246); the tables
+// are built in b200pir_ctx_create
 int b200pir_ntt4096_dev(b200pir_ctx* c, uint32_t* polys_dev, size_t count, int inverse) {
   API_BEGIN
   if (!c || !polys_dev) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
-  launch_ntt32_4k(c->dp.q[0], c->dp.q[1], tables_4k(c), polys_dev, count, inverse != 0, c->stream);
+  launch_ntt32_4k(c->dp.q[0], c->dp.q[1], c->d_tw4k.p, polys_dev, count, inverse != 0, c->stream);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -1375,7 +1375,7 @@ int b200pir_ntt4096(b200pir_ctx* c, uint64_t* polys, size_t count, int inverse) 
   DevBuf<uint32_t> nar(words);
   B200_CUDA(cudaMemcpyAsync(wide.p, polys, words * 8, cudaMemcpyHostToDevice, c->stream));
   launch_narrow(nar.p, wide.p, words, c->stream);
-  launch_ntt32_4k(c->dp.q[0], c->dp.q[1], tables_4k(c), nar.p, count, inverse != 0, c->stream);
+  launch_ntt32_4k(c->dp.q[0], c->dp.q[1], c->d_tw4k.p, nar.p, count, inverse != 0, c->stream);
   launch_widen(wide.p, nar.p, words, c->stream);
   B200_CUDA(cudaMemcpyAsync(polys, wide.p, words * 8, cudaMemcpyDeviceToHost, c->stream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
@@ -2052,7 +2052,10 @@ int b200pir_dpir_create(int device, const uint32_t* a, uint64_t rows, uint64_t c
   API_BEGIN
   if (!a || !out) throw Error(B200PIR_E_BADARG, "null argument");
   b200pir_dpir* m = dpir_new(device, rows, cols);
-  cudaError_t e = cudaMemcpy(m->a.p, a, rows * cols * 4, cudaMemcpyHostToDevice);
+  // on the handle's stream, and waited for: a pageable cudaMemcpy queues behind the legacy default stream's work and may return
+  // before its data has landed, while the matvecs run on the non-blocking m->stream
+  cudaError_t e = cudaMemcpyAsync(m->a.p, a, rows * cols * 4, cudaMemcpyHostToDevice, m->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
   if (e != cudaSuccess) { b200pir_dpir_destroy(m); throw Error(B200PIR_E_CUDA, cudaGetErrorString(e)); }
   *out = m;
   API_END

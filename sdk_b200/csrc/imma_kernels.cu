@@ -420,8 +420,8 @@ inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + blo
 
 }  // namespace
 
-void upload_imma_constants(const Twiddle* lo) {
-  B200_CUDA(cudaMemcpyToSymbol(c_tw_lo_imma, lo, sizeof(Twiddle) * 2 * 3 * 64));
+void upload_imma_constants(const Twiddle* lo, cudaStream_t s) {
+  B200_CUDA(cudaMemcpyToSymbolAsync(c_tw_lo_imma, lo, sizeof(Twiddle) * 2 * 3 * 64, 0, cudaMemcpyHostToDevice, s));
 }
 size_t imma_query_cells(const ImmaGeom& F) { return (size_t)2 * POLY * 4 * F.ks * 4 * 32; }   // up to 4 column tiles
 // 16 queries per pass need the B operand (4 tiles) plus the A rings in one CTA's shared memory

@@ -46,8 +46,9 @@ void launch_from_ntt(const DevParams& P, uint64_t* out_raw, const uint32_t* in, 
 void launch_raw_to_res(const DevParams& P, uint32_t* out, const uint64_t* raw, size_t polys, cudaStream_t s);
 void launch_res_to_raw(const DevParams& P, uint64_t* out, const uint32_t* res, size_t polys, cudaStream_t s);
 // twiddle entries 0..63 of every (modulus, direction) -> constant bank of the poly kernels' module
-void upload_poly_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */);
-void upload_mul_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */);
+// stream-ordered on s; `lo` must stay valid until s has reached the copy
+void upload_poly_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */, cudaStream_t s);
+void upload_mul_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */, cudaStream_t s);
 // format converters for the C ABI (u64 [n][z] words < 2^32  <->  ntt32)
 void launch_widen(uint64_t* out, const uint32_t* in, size_t words, cudaStream_t s);
 void launch_narrow(uint32_t* out, const uint64_t* in, size_t words, cudaStream_t s);
@@ -77,7 +78,7 @@ void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_d
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
 bool imma_supports_16(const ImmaGeom& F);                 // 16 queries per database pass fit one CTA's shared memory
 inline int imma_query_tiles(int nq) { return nq > 8 ? 4 : (nq > 4 ? 2 : 1); }   // column tiles of 4 queries
-void upload_imma_constants(const Twiddle* lo);
+void upload_imma_constants(const Twiddle* lo, cudaStream_t s);
 // one slice in the IMAD layout (uint4 [row][jp][z]) -> fragment order
 void launch_db_to_frag(const ImmaGeom& F, const uint4* db0_slice, uint4* dbf, int slice, cudaStream_t s);
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s);

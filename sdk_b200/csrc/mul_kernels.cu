@@ -418,8 +418,8 @@ void launch_dpir_transpose_expand(uint32_t* out, const uint32_t* a, size_t rows,
   k_dpir_transpose_expand<<<grid1d(out_rows * out_cols, 256), 256, 0, s>>>(out, a, rows, cols, modulus, delta, concat,
                                                                            out_rows, out_cols);
 }
-void upload_mul_constants(const Twiddle* lo) {
-  B200_CUDA(cudaMemcpyToSymbol(c_tw_lo_mul, lo, sizeof(Twiddle) * 2 * 3 * 64));
+void upload_mul_constants(const Twiddle* lo, cudaStream_t s) {
+  B200_CUDA(cudaMemcpyToSymbolAsync(c_tw_lo_mul, lo, sizeof(Twiddle) * 2 * 3 * 64, 0, cudaMemcpyHostToDevice, s));
 }
 void launch_multiply(const DevParams& P, const MulGeom& G, const uint4* db_dev, const uint4* q_dev, uint32_t* out,
                      int slice_begin, int slice_count, int nq, size_t q_stride, size_t out_stride, int variant,

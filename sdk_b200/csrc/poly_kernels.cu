@@ -1014,8 +1014,8 @@ const size_t kDynSmemFold = (size_t)(2 * NTT_SMEM_WORDS) * 4 + (size_t)HI_TW * 8
 
 }  // namespace
 
-void upload_poly_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */) {
-  B200_CUDA(cudaMemcpyToSymbol(c_tw_lo, lo, sizeof(Twiddle) * 2 * 3 * 64));
+void upload_poly_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */, cudaStream_t s) {
+  B200_CUDA(cudaMemcpyToSymbolAsync(c_tw_lo, lo, sizeof(Twiddle) * 2 * 3 * 64, 0, cudaMemcpyHostToDevice, s));
 }
 void launch_ntt_u64(const DevParams& P, uint64_t* polys, size_t count, bool inverse, cudaStream_t s) {
   if (count) ++g_kernel_launches, k_ntt_u64<<<dim3((unsigned)count, 2), 256, 0, s>>>(P, polys, inverse ? 1 : 0);
