@@ -348,7 +348,9 @@ int b200pir_dpir_derive_from_seed(int device, const uint8_t key[16], uint64_t ro
  * on the device from the two keys above, the `len` bytes of `data` laid out as the l x m matrix (database.rs:168-247; BITS gives
  * 8 len entries, including the trailing bits of the last byte), then setup() (doublepir.rs:76-108) as b200pir_dpir_setup.  The
  * squished database stays in HBM: *db_out is a new handle of l x ceil(m/3) packed words for the matvec entry points.
- * h1_squished, a2_t and h2 are host buffers shaped as b200pir_dpir_setup's.  Synchronous, on a stream of its own.
+ * h1_squished, a2_t and h2 are host buffers shaped as b200pir_dpir_setup's.  Synchronous, on a non-blocking stream of its own.
+ * The l x m layout is never held whole: the rows are laid out and multiplied band by band (b200pir_dpir_load_banded with the
+ * default scratch budget), so the device holds the squished store, setup()'s n-wide buffers and one band of scratch.
  * Errors (no handle is returned and no device memory stays allocated): those of b200pir_dpir_db_info; null pointers, a bad
  * device or an unknown entry_format -> B200PIR_E_BADARG; entries that would index past the l x m matrix (where the reference
  * panics), or l not a multiple of x -> B200PIR_E_SHAPE; a laid-out word outside [-2^15, 2^15) (bytes far wider than
@@ -356,6 +358,27 @@ int b200pir_dpir_derive_from_seed(int device, const uint8_t key[16], uint64_t ro
 int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
                       const uint8_t* data, uint64_t len, int entry_format, b200pir_dpir** db_out, uint32_t* h1_squished,
                       uint32_t* a2_t, uint32_t* h2);
+/* b200pir_dpir_load with a budget of scratch_bytes bytes of device scratch for a band of layout rows (0: 1 GiB).  The band is
+ * the largest whole number of row groups (ne rows when entries take several Z_p elements, else 1 row) whose
+ * b200pir_dpir_band_bytes fit the budget, and at least one group.  The input is staged through two pinned host buffers of at
+ * most 16 MiB, so that copying the next band's bytes overlaps the current band's kernels.  Outputs and errors as
+ * b200pir_dpir_load; they do not depend on the budget. */
+int b200pir_dpir_load_banded(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                             const uint8_t* data, uint64_t len, int entry_format, uint64_t scratch_bytes, b200pir_dpir** db_out,
+                             uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2);
+/* b200pir_dpir_load_banded with the raw bytes read from the file at `path` band by band (pread into the pinned staging), as
+ * Db::load_data_fast reads a file without holding it: `len` is the file's size.  Errors as b200pir_dpir_load, and: a file that
+ * cannot be opened -> B200PIR_E_BADARG; a read that fails or comes up short (a directory, a file truncated while it loads)
+ * -> B200PIR_E_SHAPE. */
+int b200pir_dpir_load_file(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                           const char* path, int entry_format, uint64_t scratch_bytes, b200pir_dpir** db_out, uint32_t* h1_squished,
+                           uint32_t* a2_t, uint32_t* h2);
+/* The device scratch a band of `rows` layout rows takes: 4 rows m (its centred words) + the GEMM operand image of the band
+ * (2 bytes a word, rows rounded up to 128 and m to 32) + the input bytes it can span (rows m packing entries, or rows / ne
+ * m entries when packing = 0; one byte each, or one bit each plus one byte).  Host only.  rows not a positive multiple of the
+ * group, or more than l -> B200PIR_E_SHAPE. */
+int b200pir_dpir_band_bytes(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, int entry_format,
+                            uint64_t rows, uint64_t* out);
 /* Reads a packed matrix back (rows * cols u32): the squished database server.rs:147-153 writes as `.dbp`. */
 int b200pir_dpir_download(b200pir_dpir* m, uint32_t* out);
 

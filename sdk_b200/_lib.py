@@ -116,6 +116,12 @@ def _load():
         "b200pir_dpir_derive_from_seed": (C.c_int, [C.c_int, u8p, C.c_uint64, C.c_uint64, u32p]),
         "b200pir_dpir_load": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, u8p, C.c_uint64, C.c_int,
                                         C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_load_banded": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, u8p, C.c_uint64, C.c_int,
+                                               C.c_uint64, C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_load_file": (C.c_int, [C.c_int, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, C.c_char_p, C.c_int, C.c_uint64,
+                                             C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_band_bytes": (C.c_int, [C.POINTER(DpirParams), C.c_uint64, C.c_uint64, C.c_int, C.c_uint64,
+                                              C.POINTER(C.c_uint64)]),
         "b200pir_dpir_download": (C.c_int, [vp, u32p]),
         "b200pir_dpir_matvec_packed_many": (C.c_int, [vp, u32p, C.c_size_t, u32p]),
         "b200pir_dpir_matvec_packed_many_on": (C.c_int, [vp, u32p, C.c_size_t, u32p, C.c_int]),

@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cerrno>
 #include <fcntl.h>
+#include <sys/stat.h>
 #include <unistd.h>
 #include <algorithm>
 #include <cmath>
@@ -19,9 +20,12 @@
 #include <condition_variable>
 #include <chrono>
 #include <deque>
+#include <exception>
+#include <functional>
 #include <mutex>
 #include <set>
 #include <string>
+#include <thread>
 #include <utility>
 #include <vector>
 
@@ -2076,17 +2080,24 @@ int b200pir_dpir_create_synthetic(int device, uint64_t rows, uint64_t cols, uint
   API_END
 }
 namespace {
-// doublepir.rs:76-108 setup() on device-resident inputs: db (l x m, centred), a1 (m x n), a2 (l/x x n).  db_squished is a device
-// buffer of l x ceil(m/3) words; h1_squished, a2_t and h2 are host buffers.  Synchronises s.
-void dpir_setup_dev(const uint32_t* d_db, const uint32_t* d_a1, const uint32_t* d_a2, uint64_t l, uint64_t m, uint64_t n, uint32_t p,
-                    uint64_t delta, uint64_t x, uint32_t* d_dbsq, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2, cudaStream_t s) {
+// doublepir.rs:76-108 setup() in two parts, so that the l x m layout never has to be on the device at once.
+// The per-row part, for the centred layout rows [r0, r0 + rows) in d_band (rows x m, device): those rows of h_1 = db.data * a_1
+// (against a_1's GEMM image a1_img, through the caller's a image a_img of dpir_gemm_a_bytes(rows, m) bytes) into d_h (l x n),
+// and db.data += p/2; db.squish() of the same rows into d_dbsq (l x ceil(m/3)).  No allocation, no synchronisation.
+void dpir_setup_rows(const uint32_t* d_band, uint64_t r0, uint64_t rows, uint64_t m, uint64_t n, uint32_t p, const uint8_t* a1_img,
+                     uint8_t* a_img, uint32_t* d_h, uint32_t* d_dbsq, cudaStream_t s) {
+  launch_dpir_gemm_rows(d_h + r0 * n, a_img, d_band, rows, m, a1_img, n, s);                // h_1 = db.data * a_1
+  launch_dpir_add_squish(d_dbsq + r0 * ((m + 2) / 3), d_band, rows, m, p / 2, s);         // db.data += p/2; db.squish()
+}
+// The tail, on the whole h_1 (l x n, device) and a2 (l/x x n, device): transpose / expand / concat, h_2 = h_1 * a_2, h_1 += p/2
+// and squish, a_2_copy.  h1_squished, a2_t and h2 are host buffers.  Synchronises s.
+void dpir_setup_tail(const uint32_t* d_h, const uint32_t* d_a2, uint64_t l, uint64_t n, uint32_t p, uint64_t delta, uint64_t x,
+                     uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2, cudaStream_t s) {
   const size_t lx = l / x, rows1 = n * delta * x, lx3 = lx + (3 - lx % 3) % 3;
-  DevBuf<uint32_t> d_h(l * n), d_hc(rows1 * lx), d_h2(rows1 * n);
+  DevBuf<uint32_t> d_hc(rows1 * lx), d_h2(rows1 * n);
   DevBuf<uint32_t> d_h1sq(rows1 * ((lx + 2) / 3)), d_a2t(n * lx3);
-  launch_dpir_gemm(d_h.p, d_db, d_a1, l, m, n, s);                                       // h_1 = db.data * a_1
-  launch_dpir_transpose_expand_concat(d_hc.p, d_h.p, l, n, p, (int)delta, x, s);        // transpose, expand, concat_cols
+  launch_dpir_transpose_expand_concat(d_hc.p, d_h, l, n, p, (int)delta, x, s);          // transpose, expand, concat_cols
   launch_dpir_gemm(d_h2.p, d_hc.p, d_a2, rows1, lx, n, s);                               // h_2 = h_1 * a_2
-  launch_dpir_add_squish(d_dbsq, d_db, l, m, p / 2, s);                                  // db.data += p/2; db.squish()
   launch_dpir_add_squish(d_h1sq.p, d_hc.p, rows1, lx, p / 2, s);                         // h_1 += p/2; squish
   launch_dpir_pad_transpose(d_a2t.p, d_a2, lx, n, lx3, s);                               // a_2_copy
   B200_CUDA(cudaMemcpyAsync(h1_squished, d_h1sq.p, d_h1sq.n * 4, cudaMemcpyDeviceToHost, s));
@@ -2113,11 +2124,14 @@ int b200pir_dpir_setup(int device, const uint32_t* db, uint64_t l, uint64_t m, c
   B200_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   try {
     const size_t lx = l / x;
-    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n), d_dbsq(l * ((m + 2) / 3));
+    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n), d_dbsq(l * ((m + 2) / 3)), d_h(l * n);
+    DevBuf<uint8_t> a1_img(dpir_gemm_b_bytes(m, n)), a_img(dpir_gemm_a_bytes(l, m));
     B200_CUDA(cudaMemcpyAsync(d_db.p, db, l * m * 4, cudaMemcpyHostToDevice, s));
     B200_CUDA(cudaMemcpyAsync(d_a1.p, a1, m * n * 4, cudaMemcpyHostToDevice, s));
     B200_CUDA(cudaMemcpyAsync(d_a2.p, a2, lx * n * 4, cudaMemcpyHostToDevice, s));
-    dpir_setup_dev(d_db.p, d_a1.p, d_a2.p, l, m, n, p, delta, x, d_dbsq.p, h1_squished, a2_t, h2, s);
+    launch_dpir_gemm_b_image(a1_img.p, d_a1.p, m, n, s);
+    dpir_setup_rows(d_db.p, 0, l, m, n, p, a1_img.p, a_img.p, d_h.p, d_dbsq.p, s);        // every row as one band
+    dpir_setup_tail(d_h.p, d_a2.p, l, n, p, delta, x, h1_squished, a2_t, h2, s);
     B200_CUDA(cudaMemcpyAsync(db_squished, d_dbsq.p, d_dbsq.n * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
     B200_CUDA(cudaGetLastError());
@@ -2302,19 +2316,118 @@ int b200pir_dpir_derive_from_seed(int device, const uint8_t key[16], uint64_t ro
   API_END
 }
 
-int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
-                      const uint8_t* data, uint64_t len, int entry_format, b200pir_dpir** db_out, uint32_t* h1_squished,
-                      uint32_t* a2_t, uint32_t* h2) {
-  API_BEGIN
-  if (!params || !data || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+namespace {
+constexpr uint64_t kDpirDefaultScratch = 1ull << 30;   // device bytes of band scratch when the caller passes 0
+constexpr size_t kDpirStagePiece = 16ull << 20;        // bytes of one pinned staging buffer (two of them)
+
+// The input of a load: copies bytes [off, off + n) of the raw entries to dst, or throws
+using DpirFill = std::function<void(uint8_t* dst, uint64_t off, size_t n)>;
+
+// One band of layout rows, and the input it reads
+struct DpirBandGeom {
+  bool bits_format;
+  uint64_t l, m, packing, ne, count;   // count: the entries the iterator yields
+  // rows in a band come in groups: a base-p entry spans ne rows, so bands are whole groups of ne rows
+  uint64_t group() const { return packing ? 1 : ne; }
+  // the first entry of layout row r (r a multiple of group()): packed elements r m .., or entries (r / ne) m ..
+  uint64_t first_entry(uint64_t r) const { return packing ? r * m * packing : (r / ne) * m; }
+  // bytes of the input a band of `rows` rows can span: one more in the bit format, where a band may start mid-byte
+  uint64_t raw_bytes(uint64_t rows) const {
+    const uint64_t e = packing ? rows * m * packing : (rows / ne) * m;
+    return bits_format ? (e + 7) / 8 + 1 : e;
+  }
+  // device scratch a band of `rows` rows takes: its centred words, its GEMM image and its input bytes
+  uint64_t band_bytes(uint64_t rows) const { return 4 * rows * m + dpir_gemm_a_bytes(rows, m) + raw_bytes(rows); }
+  // the most rows, a whole number of groups and at least one, whose band fits `budget` bytes of scratch
+  uint64_t band_rows(uint64_t budget) const {
+    uint64_t lo = 1, hi = l / group();                 // in groups
+    if (band_bytes(group()) > budget) return group();
+    while (lo < hi) {
+      const uint64_t mid = lo + (hi - lo + 1) / 2;
+      if (band_bytes(mid * group()) <= budget) lo = mid;
+      else hi = mid - 1;
+    }
+    return lo * group();
+  }
+};
+
+DpirBandGeom dpir_band_geom(const b200pir_dpir_params* params, const b200pir_dpir_info& info, int entry_format, uint64_t len) {
   if (entry_format != B200PIR_DPIR_ENTRY_BYTES && entry_format != B200PIR_DPIR_ENTRY_BITS)
     throw Error(B200PIR_E_BADARG, "unknown entry format");
-  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, nullptr);
   const bool bits_format = entry_format == B200PIR_DPIR_ENTRY_BITS;
-  const uint64_t l = params->l, m = params->m, n = params->n, x = info.x;
-  const uint32_t p = (uint32_t)params->p;
   if (bits_format && len > UINT64_MAX / 8) throw Error(B200PIR_E_SHAPE, "too many entries");
-  const uint64_t count = bits_format ? 8 * len : len;           // the number of items the reference's iterator yields
+  return DpirBandGeom{bits_format, params->l, params->m, info.packing, info.ne, bits_format ? 8 * len : len};
+}
+
+// fill(dst, off, n) split over up to 4 threads: a large copy out of host memory or the page cache runs at several times one
+// thread's rate
+void dpir_fill_parallel(const DpirFill& fill, uint8_t* dst, uint64_t off, size_t n) {
+  constexpr size_t kPart = 4ull << 20;
+  const size_t parts = std::min<size_t>(4, (n + kPart - 1) / kPart);
+  if (parts <= 1) {
+    if (n) fill(dst, off, n);
+    return;
+  }
+  const size_t per = (n + parts - 1) / parts;
+  std::vector<std::exception_ptr> err(parts);
+  std::vector<std::thread> th;
+  for (size_t t = 0; t < parts; t++)
+    th.emplace_back([&, t] {
+      const size_t a = t * per, b = std::min(n, a + per);
+      try {
+        if (a < b) fill(dst + a, off + a, b - a);
+      } catch (...) { err[t] = std::current_exception(); }
+    });
+  for (auto& t : th) t.join();
+  for (auto& e : err)
+    if (e) std::rethrow_exception(e);
+}
+
+// Two pinned host buffers that take turns: a buffer is refilled once the upload that last read it has run
+struct DpirStaging {
+  cudaStream_t s;
+  uint8_t* buf[2] = {nullptr, nullptr};
+  cudaEvent_t done[2] = {nullptr, nullptr};
+  size_t cap = 0;
+  int next = 0;
+  DpirStaging(cudaStream_t st, size_t bytes) : s(st), cap(bytes) {
+    for (int i = 0; i < 2; i++) {
+      B200_CUDA(cudaMallocHost(&buf[i], std::max<size_t>(cap, 1)));
+      B200_CUDA(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
+    }
+  }
+  ~DpirStaging() {
+    cudaStreamSynchronize(s);                          // no upload may still read a buffer that is freed
+    for (int i = 0; i < 2; i++) {
+      if (done[i]) cudaEventDestroy(done[i]);
+      if (buf[i]) cudaFreeHost(buf[i]);
+    }
+  }
+  // input bytes [off, off + n) to dst (device) on s
+  void upload(const DpirFill& fill, uint8_t* dst, uint64_t off, uint64_t n) {
+    for (uint64_t done_bytes = 0; done_bytes < n;) {
+      const size_t piece = (size_t)std::min<uint64_t>(cap, n - done_bytes);
+      const int i = next;
+      next ^= 1;
+      B200_CUDA(cudaEventSynchronize(done[i]));
+      dpir_fill_parallel(fill, buf[i], off + done_bytes, piece);
+      B200_CUDA(cudaMemcpyAsync(dst + done_bytes, buf[i], piece, cudaMemcpyHostToDevice, s));
+      B200_CUDA(cudaEventRecord(done[i], s));
+      done_bytes += piece;
+    }
+  }
+};
+
+// DoublePirServer::new + load_data / load_data_fast + setup() (server.rs:160-165, 201-229), band by band: for each band of
+// layout rows the band's input bytes are staged and uploaded, laid out, multiplied into h_1's rows and squished into the
+// resident store; setup()'s tail then runs on the whole h_1.  The band scratch is allocated once, sized by scratch_bytes.
+b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                              uint64_t len, int entry_format, uint64_t scratch_bytes, const DpirFill& fill, uint32_t* h1_squished,
+                              uint32_t* a2_t, uint32_t* h2) {
+  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, nullptr);
+  const DpirBandGeom G = dpir_band_geom(params, info, entry_format, len);
+  const uint64_t l = params->l, m = params->m, n = params->n, x = info.x, count = G.count;
+  const uint32_t p = (uint32_t)params->p;
   // where load_data would index past the matrix (and panic): the last packed element, or the last digit row of the last entry
   if (info.packing ? (count + info.packing - 1) / info.packing > l * m : (count && ((count - 1) / m + 1) > l / info.ne))
     throw Error(B200PIR_E_SHAPE, "the entries do not fit the l x m database");
@@ -2322,26 +2435,94 @@ int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t nu
   dpir_device(device);
   std::unique_ptr<b200pir_dpir, DpirDeleter> h(dpir_new(device, l, (m + 2) / 3));
   cudaStream_t s = h->stream;
+  const uint64_t band = G.band_rows(scratch_bytes ? scratch_bytes : kDpirDefaultScratch);
+  DevBuf<uint32_t> d_h(l * n), d_a2((l / x) * n);
   {
-    const size_t lx = l / x;
-    DevBuf<uint8_t> d_raw(len);
-    DevBuf<uint32_t> d_db(l * m), d_a1(m * n), d_a2(lx * n);
+    DevBuf<uint8_t> a1_img(dpir_gemm_b_bytes(m, n));
+    {
+      DevBuf<uint32_t> d_a1(m * n);
+      launch_dpir_derive(d_a1.p, d_a1.n, dpir_aes_key(kDpirSeedA1), s);           // init(): A_1 = derive(m x n, SEEDS_SHORT[0])
+      launch_dpir_gemm_b_image(a1_img.p, d_a1.p, m, n, s);                        // a_1 is only read through its GEMM image
+      B200_CUDA(cudaStreamSynchronize(s));
+    }
+    launch_dpir_derive(d_a2.p, d_a2.n, dpir_aes_key(kDpirSeedA2), s);              //         A_2 = derive(l/x x n, SEEDS_SHORT[1])
+    DevBuf<uint32_t> d_band(band * m);
+    DevBuf<uint8_t> a_img(dpir_gemm_a_bytes(band, m)), d_raw(G.raw_bytes(band));
     DevBuf<int> d_flag(1);
     B200_CUDA(cudaMemsetAsync(d_flag.p, 0, sizeof(int), s));
-    if (len) B200_CUDA(cudaMemcpyAsync(d_raw.p, data, len, cudaMemcpyHostToDevice, s));
-    launch_dpir_derive(d_a1.p, d_a1.n, dpir_aes_key(kDpirSeedA1), s);              // init(): A_1 = derive(m x n, SEEDS_SHORT[0])
-    launch_dpir_derive(d_a2.p, d_a2.n, dpir_aes_key(kDpirSeedA2), s);              //         A_2 = derive(l/x x n, SEEDS_SHORT[1])
-    launch_dpir_layout(d_db.p, d_raw.p, count, bits_format, l, m, (uint32_t)info.packing, (uint32_t)bits_per_entry,
-                       (uint32_t)info.ne, p, d_flag.p, s);
+    DpirStaging stage(s, (size_t)std::min<uint64_t>(kDpirStagePiece, G.raw_bytes(band)));
+    for (uint64_t r0 = 0; r0 < l; r0 += band) {
+      const uint64_t rows = std::min(band, l - r0);
+      // the band's entries [e0, e1) are bytes [b0, b1) of the input (bits: the band may start and end mid-byte)
+      const uint64_t e0 = std::min(G.first_entry(r0), count), e1 = std::min(G.first_entry(r0 + rows), count);
+      const uint64_t b0 = G.bits_format ? e0 / 8 : e0, b1 = G.bits_format ? (e1 + 7) / 8 : e1;
+      stage.upload(fill, d_raw.p, b0, b1 - b0);
+      launch_dpir_layout(d_band.p, d_raw.p, G.bits_format ? 8 * b0 : b0, count, G.bits_format, r0, rows, m, (uint32_t)info.packing,
+                         (uint32_t)bits_per_entry, (uint32_t)info.ne, p, d_flag.p, s);
+      dpir_setup_rows(d_band.p, r0, rows, m, n, p, a1_img.p, a_img.p, d_h.p, h->a.p, s);
+    }
     B200_CUDA(cudaGetLastError());
     int flag = 0;
     B200_CUDA(cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
     if (flag) throw Error(B200PIR_E_UNSUPPORTED, "load: a packed database word lies outside [-2^15, 2^15) (entries far wider than bits_per_entry)");
-    d_raw.release();
-    dpir_setup_dev(d_db.p, d_a1.p, d_a2.p, l, m, n, p, info.delta, x, h->a.p, h1_squished, a2_t, h2, s);
   }
-  *db_out = h.release();
+  dpir_setup_tail(d_h.p, d_a2.p, l, n, p, info.delta, x, h1_squished, a2_t, h2, s);
+  return h.release();
+}
+}  // namespace
+
+int b200pir_dpir_load(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                      const uint8_t* data, uint64_t len, int entry_format, b200pir_dpir** db_out, uint32_t* h1_squished,
+                      uint32_t* a2_t, uint32_t* h2) {
+  return b200pir_dpir_load_banded(device, params, num_entries, bits_per_entry, data, len, entry_format, 0, db_out, h1_squished,
+                                  a2_t, h2);
+}
+
+int b200pir_dpir_load_banded(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                             const uint8_t* data, uint64_t len, int entry_format, uint64_t scratch_bytes, b200pir_dpir** db_out,
+                             uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
+  API_BEGIN
+  if (!params || !data || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, len, entry_format, scratch_bytes,
+                            [data](uint8_t* dst, uint64_t off, size_t n) { std::memcpy(dst, data + off, n); }, h1_squished, a2_t, h2);
+  API_END
+}
+
+int b200pir_dpir_load_file(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                           const char* path, int entry_format, uint64_t scratch_bytes, b200pir_dpir** db_out, uint32_t* h1_squished,
+                           uint32_t* a2_t, uint32_t* h2) {
+  API_BEGIN
+  if (!params || !path || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+  struct Closer { int fd; ~Closer() { if (fd >= 0) close(fd); } } file{open(path, O_RDONLY | O_CLOEXEC)};
+  if (file.fd < 0) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
+  struct stat st;
+  if (fstat(file.fd, &st)) throw Error(B200PIR_E_BADARG, std::string("cannot stat ") + path);
+  // the entry count comes from the file size, as load_data_fast's takes it from the bytes it is given; a directory or a
+  // device has no such size, and reading it fails
+  if (!S_ISREG(st.st_mode)) throw Error(B200PIR_E_SHAPE, "short read from the database file (not a regular file)");
+  const int fd = file.fd;
+  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, (uint64_t)st.st_size, entry_format, scratch_bytes,
+                            [fd](uint8_t* dst, uint64_t off, size_t n) {
+                              while (n) {
+                                const ssize_t r = pread(fd, dst, n, (off_t)off);
+                                if (r < 0 && errno == EINTR) continue;
+                                if (r <= 0) throw Error(B200PIR_E_SHAPE, "short read from the database file");
+                                dst += r; off += (uint64_t)r; n -= (size_t)r;
+                              }
+                            },
+                            h1_squished, a2_t, h2);
+  API_END
+}
+
+int b200pir_dpir_band_bytes(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, int entry_format,
+                            uint64_t rows, uint64_t* out) {
+  API_BEGIN
+  if (!out) throw Error(B200PIR_E_BADARG, "null argument");
+  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, nullptr);
+  const DpirBandGeom G = dpir_band_geom(params, info, entry_format, 0);
+  if (rows == 0 || rows > G.l || rows % G.group()) throw Error(B200PIR_E_SHAPE, "rows must be a whole number of groups of at most l");
+  *out = G.band_bytes(rows);
   API_END
 }
 

@@ -195,14 +195,19 @@ inline unsigned blocks(size_t total, int block) { return (unsigned)((total + blo
 }  // namespace
 
 // c (rows x n_cols, device) = a (rows x k_dim, device, entries in [-2^15, 2^15) as wrapping u32) * b (k_dim x n_cols, device) mod 2^32
-void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t rows, size_t k_dim, size_t n_cols, cudaStream_t s) {
-  const int mt = (int)((rows + 127) / 128), nt = (int)((n_cols + 127) / 128), ks = (int)((k_dim + 31) / 32);
-  uint8_t *a_img = nullptr, *b_img = nullptr;
-  B200_CUDA(cudaMalloc(&a_img, (size_t)2 * mt * ks * TC5_TILE));
-  B200_CUDA(cudaMalloc(&b_img, (size_t)4 * nt * ks * TC5_TILE));
-  g_kernel_launches += 2;
-  k_gemm_a_image<<<blocks((size_t)mt * ks * 1024, 256), 256, 0, s>>>(a_img, a, rows, k_dim, mt, ks);
+size_t dpir_gemm_a_bytes(size_t rows, size_t k_dim) { return 2 * ((rows + 127) / 128) * ((k_dim + 31) / 32) * TC5_TILE; }
+size_t dpir_gemm_b_bytes(size_t k_dim, size_t n_cols) { return 4 * ((n_cols + 127) / 128) * ((k_dim + 31) / 32) * TC5_TILE; }
+void launch_dpir_gemm_b_image(uint8_t* b_img, const uint32_t* b, size_t k_dim, size_t n_cols, cudaStream_t s) {
+  const int nt = (int)((n_cols + 127) / 128), ks = (int)((k_dim + 31) / 32);
+  ++g_kernel_launches;
   k_gemm_b_image<<<blocks((size_t)nt * ks * 1024, 256), 256, 0, s>>>(b_img, b, k_dim, n_cols, nt, ks);
+}
+void launch_dpir_gemm_rows(uint32_t* c, uint8_t* a_img, const uint32_t* a, size_t rows, size_t k_dim, const uint8_t* b_img,
+                           size_t n_cols, cudaStream_t s) {
+  if (rows == 0) return;
+  const int mt = (int)((rows + 127) / 128), nt = (int)((n_cols + 127) / 128), ks = (int)((k_dim + 31) / 32);
+  ++g_kernel_launches;
+  k_gemm_a_image<<<blocks((size_t)mt * ks * 1024, 256), 256, 0, s>>>(a_img, a, rows, k_dim, mt, ks);
   const size_t smem = (size_t)G_STAGES * G_STAGE_BYTES + sizeof(GemmSmem) + 16;
   opt_in_smem(k_dpir_gemm, (int)smem);
   // gridDim.y is capped at 65535: more than 128 * 65535 rows take several launches
@@ -210,6 +215,16 @@ void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t 
     ++g_kernel_launches;
     k_dpir_gemm<<<dim3(4 * nt, std::min(mt - m_t0, 65535)), G_THREADS, smem, s>>>(a_img, b_img, c, rows, n_cols, mt, nt, ks, m_t0);
   }
+}
+void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t rows, size_t k_dim, size_t n_cols, cudaStream_t s) {
+  uint8_t *a_img = nullptr, *b_img = nullptr;
+  B200_CUDA(cudaMalloc(&a_img, dpir_gemm_a_bytes(rows, k_dim)));
+  if (cudaMalloc(&b_img, dpir_gemm_b_bytes(k_dim, n_cols)) != cudaSuccess) {
+    cudaFree(a_img);
+    throw Error(-3, "dpir gemm: out of device memory");
+  }
+  launch_dpir_gemm_b_image(b_img, b, k_dim, n_cols, s);
+  launch_dpir_gemm_rows(c, a_img, a, rows, k_dim, b_img, n_cols, s);
   cudaError_t e = cudaGetLastError();
   const cudaError_t se = cudaStreamSynchronize(s);
   if (e == cudaSuccess) e = se;

@@ -9,8 +9,10 @@
 // memory.  The lookups are data-dependent, so this is NOT constant-time: that is fine here, because the key and the output are
 // public (the reference derives public matrices only, matrix.rs:120-124) and nothing secret ever passes through this kernel.
 //
-// k_dpir_layout: Db::load_data / load_data_fast (database/database.rs:168-247) as a gather, one thread per word of the l x m
-// matrix, then "Map DB elems to [-p/2; p/2]" (the wrapping subtraction of p/2 from every word, touched or not).
+// k_dpir_layout: Db::load_data / load_data_fast (database/database.rs:168-247) as a gather, one thread per word of one band of
+// rows of the l x m matrix, then "Map DB elems to [-p/2; p/2]" (the wrapping subtraction of p/2 from every word, touched or
+// not).  A band's entries are one contiguous range of the input, so only that range needs to be on the device (api.cu stages
+// the input band by band).
 #include "kernels.h"
 
 namespace b200pir {
@@ -91,7 +93,8 @@ __device__ __forceinline__ uint32_t entry(const uint8_t* __restrict__ data, size
   return data[i];
 }
 
-// word k of the l x m matrix (row-major, k = row * m + col), then minus p/2.  `count` = number of entries the iterator yields.
+// word k of the l x m matrix (row-major, k = row * m + col), then minus p/2, for the words of rows [r0, r0 + rows): band word
+// kb is word r0 m + kb.  `count` = number of entries the iterator yields; entry i is read at i - base of the staged data.
 //   packing > 0: element k = sum_t e_{k packing + t} * coeff_t, coeff_0 = 1, coeff_{t+1} = coeff_t * 2^bits (wrapping u32, no
 //                masking: an entry wider than `bits` spills into the next field); the last group may be partial
 //                (the `iter.peek().is_none()` flush).
@@ -99,33 +102,35 @@ __device__ __forceinline__ uint32_t entry(const uint8_t* __restrict__ data, size
 //                (row / ne) m + col.
 // Sets *out_of_range when a centred word lies outside [-2^15, 2^15), the operand range of the setup GEMM (dpir_gemm.cu).
 template <bool BITS>
-__global__ void k_dpir_layout(uint32_t* __restrict__ db, const uint8_t* __restrict__ data, size_t count, size_t l, size_t m,
-                              uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p, int* __restrict__ out_of_range) {
-  const size_t words = l * m;
+__global__ void k_dpir_layout(uint32_t* __restrict__ band, const uint8_t* __restrict__ data, uint64_t base, uint64_t count,
+                              uint64_t r0, uint64_t rows, uint64_t m, uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p,
+                              int* __restrict__ out_of_range) {
+  const uint64_t words = rows * m, k0 = r0 * m;
   bool bad = false;
-  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < words; k += (size_t)gridDim.x * blockDim.x) {
+  for (uint64_t kb = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; kb < words; kb += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t k = k0 + kb;
     uint32_t v = 0;
     if (packing) {
-      const size_t first = k * packing;
+      const uint64_t first = k * packing;
       if (first < count) {
         uint32_t coeff = 1;
-        const size_t last = first + packing < count ? first + packing : count;
-        for (size_t i = first; i < last; i++) {
-          v += entry<BITS>(data, i) * coeff;
+        const uint64_t last = first + packing < count ? first + packing : count;
+        for (uint64_t i = first; i < last; i++) {
+          v += entry<BITS>(data, i - base) * coeff;
           coeff *= 1u << bits;
         }
       }
     } else {
-      const size_t row = k / m, col = k - row * m;
-      const size_t i = (row / ne) * m + col;
+      const uint64_t row = k / m, col = k - row * m;
+      const uint64_t i = (row / ne) * m + col;
       if (i < count) {
-        uint32_t e = entry<BITS>(data, i);
-        for (uint32_t j = row % ne; j; j--) e /= p;                   // base_p (arith.rs:16-22)
+        uint32_t e = entry<BITS>(data, i - base);
+        for (uint32_t j = (uint32_t)(row % ne); j; j--) e /= p;       // base_p (arith.rs:16-22)
         v = e % p;
       }
     }
     v -= p / 2;
-    db[k] = v;
+    band[kb] = v;
     bad |= (int32_t)v < -32768 || (int32_t)v > 32767;
   }
   if (bad) atomicOr(out_of_range, 1);
@@ -166,12 +171,13 @@ void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cuda
   k_dpir_derive<<<grid_for((words + 3) / 4, 256), 256, 0, s>>>(out, words, key);
 }
 
-void launch_dpir_layout(uint32_t* db, const uint8_t* data, size_t count, bool bits_format, size_t l, size_t m, uint32_t packing,
-                        uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range, cudaStream_t s) {
+void launch_dpir_layout(uint32_t* band, const uint8_t* data, uint64_t base, uint64_t count, bool bits_format, uint64_t r0,
+                        uint64_t rows, uint64_t m, uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range,
+                        cudaStream_t s) {
   ++g_kernel_launches;
-  const unsigned g = grid_for(l * m, 256);
-  if (bits_format) k_dpir_layout<true><<<g, 256, 0, s>>>(db, data, count, l, m, packing, bits, ne, p, out_of_range);
-  else k_dpir_layout<false><<<g, 256, 0, s>>>(db, data, count, l, m, packing, bits, ne, p, out_of_range);
+  const unsigned g = grid_for(rows * m, 256);
+  if (bits_format) k_dpir_layout<true><<<g, 256, 0, s>>>(band, data, base, count, r0, rows, m, packing, bits, ne, p, out_of_range);
+  else k_dpir_layout<false><<<g, 256, 0, s>>>(band, data, base, count, r0, rows, m, packing, bits, ne, p, out_of_range);
 }
 
 }  // namespace b200pir

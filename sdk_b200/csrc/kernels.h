@@ -224,6 +224,13 @@ bool dpir_use_tc(size_t nv, size_t rows);
 // c (rows x n_cols) = a (rows x k_dim, entries in [-2^15, 2^15) as wrapping u32) * b (k_dim x n_cols) mod 2^32; device pointers;
 // 8-bit limb products on the tensor cores (wgmma) (exact); synchronises the stream
 void launch_dpir_gemm(uint32_t* c, const uint32_t* a, const uint32_t* b, size_t rows, size_t k_dim, size_t n_cols, cudaStream_t s);
+// The same in two steps on caller-owned operand images, with no allocation and no synchronisation: the image of b once
+// (dpir_gemm_b_bytes), then any number of row ranges of a, each through an a image of dpir_gemm_a_bytes(rows, k_dim) bytes
+size_t dpir_gemm_a_bytes(size_t rows, size_t k_dim);
+size_t dpir_gemm_b_bytes(size_t k_dim, size_t n_cols);
+void launch_dpir_gemm_b_image(uint8_t* b_img, const uint32_t* b, size_t k_dim, size_t n_cols, cudaStream_t s);
+void launch_dpir_gemm_rows(uint32_t* c, uint8_t* a_img, const uint32_t* a, size_t rows, size_t k_dim, const uint8_t* b_img,
+                           size_t n_cols, cudaStream_t s);
 // transpose + expand (contract.rs:62-78) + concat_cols (indexing.rs:82-101): h (l x n) -> out ((n delta x) x (l / x)), centred digits
 void launch_dpir_transpose_expand_concat(uint32_t* out, const uint32_t* h, size_t l, size_t n, uint32_t p, int delta, size_t x,
                                          cudaStream_t s);
@@ -238,9 +245,12 @@ struct DpirAesKey { uint32_t rk[44]; uint32_t te0[256]; uint8_t sbox[256]; };
 DpirAesKey dpir_aes_key(const uint8_t key[16]);
 // Matrix::derive_from_seed (matrix.rs:125-135, derivation.rs:11-22): out[0 .. words) = the AES-128-Ctr64BE keystream, 64 KiB chunks
 void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cudaStream_t s);
-// Db::load_data (bits_format false) / load_data_fast (true), database.rs:168-247: `count` entries of `data` -> the l x m matrix
-// minus p/2 (every word written); *out_of_range |= 1 when a word lies outside the setup GEMM's [-2^15, 2^15)
-void launch_dpir_layout(uint32_t* db, const uint8_t* data, size_t count, bool bits_format, size_t l, size_t m, uint32_t packing,
-                        uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range, cudaStream_t s);
+// Db::load_data (bits_format false) / load_data_fast (true), database.rs:168-247, for the band of layout rows [r0, r0 + rows):
+// the band's words of the l x m matrix minus p/2 (every word written) into band (rows x m).  Of the `count` entries the
+// iterator yields, `data` holds those from entry `base` on (entry i is at data[i - base], or at bit (i - base) % 8 of byte
+// (i - base) / 8).  *out_of_range |= 1 when a word lies outside the setup GEMM's [-2^15, 2^15)
+void launch_dpir_layout(uint32_t* band, const uint8_t* data, uint64_t base, uint64_t count, bool bits_format, uint64_t r0,
+                        uint64_t rows, uint64_t m, uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range,
+                        cudaStream_t s);
 
 }  // namespace b200pir

@@ -1,5 +1,6 @@
 """Host-side mirror of DoublePIR's packed matvec (lib/doublepir/src/matrix/kernels.rs:118-178)."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -272,20 +273,45 @@ def derive_from_seed(rows, cols, key, device=0):
     return out
 
 
-def load(params, num_entries, bits_per_entry, data, entry_format=ENTRY_BYTES, device=0):
-    """DoublePirServer::new + load_data (ENTRY_BYTES) / load_data_fast (ENTRY_BITS) + setup() on the GPU (server.rs:160-165,
-    201-229): A_1 and A_2 are derived from SEED_A1 / SEED_A2 on the device.  data: the raw bytes.  Returns
-    (PackedMatrix of the squished database, resident in HBM; dict(h1_squished, a2_t, h2); db_info dict)."""
-    info = db_info(params, num_entries, bits_per_entry)
-    data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
-    n, l, m = int(params["n"]), int(params["l"]), int(params["m"])
+def _load_outputs(params, info):
+    n, l = int(params["n"]), int(params["l"])
     x, delta = info["x"], info["delta"]
     lx = l // x
     rows1 = n * delta * x
-    out = dict(h1_squished=np.zeros((rows1, (lx + 2) // 3), dtype=np.uint32), a2_t=np.zeros((n, lx + (3 - lx % 3) % 3), dtype=np.uint32),
-               h2=np.zeros((rows1, n), dtype=np.uint32))
+    return dict(h1_squished=np.zeros((rows1, (lx + 2) // 3), dtype=np.uint32), a2_t=np.zeros((n, lx + (3 - lx % 3) % 3), dtype=np.uint32),
+                h2=np.zeros((rows1, n), dtype=np.uint32))
+
+
+def load(params, num_entries, bits_per_entry, data, entry_format=ENTRY_BYTES, device=0, scratch_bytes=0):
+    """DoublePirServer::new + load_data (ENTRY_BYTES) / load_data_fast (ENTRY_BITS) + setup() on the GPU (server.rs:160-165,
+    201-229): A_1 and A_2 are derived from SEED_A1 / SEED_A2 on the device.  data: the raw bytes.  The layout is built and
+    multiplied band by band of rows, each band in at most scratch_bytes of device scratch (0: 1 GiB); the outputs do not
+    depend on it.  Returns (PackedMatrix of the squished database, resident in HBM; dict(h1_squished, a2_t, h2); db_info dict)."""
+    info = db_info(params, num_entries, bits_per_entry)
+    data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
+    out = _load_outputs(params, info)
     h = C.c_void_p()
-    check(LIB.b200pir_dpir_load(device, C.byref(_params(params)), num_entries, bits_per_entry, data.ctypes.data, data.size,
-                                entry_format, C.byref(h), out["h1_squished"].ctypes.data, out["a2_t"].ctypes.data,
-                                out["h2"].ctypes.data))
-    return PackedMatrix._adopt(h, l, (m + 2) // 3), out, info
+    check(LIB.b200pir_dpir_load_banded(device, C.byref(_params(params)), num_entries, bits_per_entry, data.ctypes.data, data.size,
+                                       entry_format, int(scratch_bytes), C.byref(h), out["h1_squished"].ctypes.data,
+                                       out["a2_t"].ctypes.data, out["h2"].ctypes.data))
+    return PackedMatrix._adopt(h, int(params["l"]), (int(params["m"]) + 2) // 3), out, info
+
+
+def load_file(params, num_entries, bits_per_entry, path, entry_format=ENTRY_BITS, device=0, scratch_bytes=0):
+    """load() with the raw bytes read from the file at `path` band by band, never held whole in host memory: what
+    Db::load_data_fast does with a file (ENTRY_BITS, the default) or load_data with one entry a byte (ENTRY_BYTES)."""
+    info = db_info(params, num_entries, bits_per_entry)
+    out = _load_outputs(params, info)
+    h = C.c_void_p()
+    check(LIB.b200pir_dpir_load_file(device, C.byref(_params(params)), num_entries, bits_per_entry, os.fsencode(path), entry_format,
+                                     int(scratch_bytes), C.byref(h), out["h1_squished"].ctypes.data, out["a2_t"].ctypes.data,
+                                     out["h2"].ctypes.data))
+    return PackedMatrix._adopt(h, int(params["l"]), (int(params["m"]) + 2) // 3), out, info
+
+
+def band_bytes(params, num_entries, bits_per_entry, rows, entry_format=ENTRY_BITS):
+    """The device scratch a load's band of `rows` layout rows takes (b200pir_dpir_band_bytes): a scratch_bytes of at least this
+    gives bands of at least `rows` rows."""
+    out = C.c_uint64()
+    check(LIB.b200pir_dpir_band_bytes(C.byref(_params(params)), num_entries, bits_per_entry, entry_format, rows, C.byref(out)))
+    return out.value
