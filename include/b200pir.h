@@ -430,6 +430,28 @@ int b200pir_dpir_answer(b200pir_dpir_server* s, const uint8_t* request, size_t l
  * error nothing is written to any output. */
 int b200pir_dpir_answer_many(b200pir_dpir_server* s, const uint8_t* const* requests, const size_t* lens, size_t count,
                              uint8_t* const* outs, size_t* out_lens);
+/* Db::_set for `count` entries (database.rs:264-266, a todo!() in the reference), on the database this server borrows, and
+ * setup()'s outputs patched to match: afterwards the squished store (b200pir_dpir_download), the server's h_1
+ * (b200pir_dpir_server_state) and h2 are byte for byte what b200pir_dpir_load* returns for the same bytes with those entries
+ * replaced.  values[k] = entry indices[k] as the load read it: a byte (ENTRY_BYTES) or a bit 0/1 (ENTRY_BITS).  A repeated
+ * index ends with its last value.  h2: (n delta x) x n host matrix in/out, the hint as the load or the previous update left it.
+ * The cost grows with the number of changed entries, not with the database (DESIGN §4.5): the changed store fields are
+ * rewritten, only the rows of A_1 at changed columns are derived, and the hint moves by a rank-k product on the setup GEMM.
+ * count = 0 succeeds and changes nothing.  Everything is checked before any device work, and a refused call writes nothing
+ * (store, h_1 and h2 stay as they were, and the server keeps serving): null pointers -> B200PIR_E_BADARG; an index at or past
+ * the entries the load read (len, or 8 len bits) -> B200PIR_E_SHAPE; a value the format cannot hold (above 1 for bits, or
+ * 2^bits_per_entry or more where entries are packed several to an element) -> B200PIR_E_BADARG; a server whose parameters,
+ * num_entries or bits_per_entry differ from its database's load -> B200PIR_E_SHAPE; a database not made by b200pir_dpir_load*
+ * (b200pir_dpir_create of a `.dbp`, say), a server holding fewer than l rows (a chunk), or a load that packed entries wider
+ * than bits_per_entry (its elements then do not decode field by field), or n above 51200 -> B200PIR_E_UNSUPPORTED.
+ * Holds the server's and the database handle's mutexes, so an answer sees all of an update or none of it; runs on the
+ * server's stream and synchronises.  Scratch belongs to the server: allocated by the first update, grown only by a larger
+ * batch.  Large batches are applied in groups of 4096 changed elements; the results do not depend on the grouping.  Other
+ * servers that borrow the same database handle keep their own h_1, which goes stale. */
+int b200pir_dpir_server_update(b200pir_dpir_server* s, const uint64_t* indices, const uint8_t* values, size_t count, uint32_t* h2);
+/* server_state[0] as the server now holds it: h1_squished, (n delta x) x ceil((l/x)/3) u32 (what save_to_files writes as
+ * .state).  Null pointers -> B200PIR_E_BADARG. */
+int b200pir_dpir_server_state(b200pir_dpir_server* s, uint32_t* h1_squished);
 
 #ifdef __cplusplus
 }

@@ -132,6 +132,8 @@ def _load():
         "b200pir_dpir_answer": (C.c_int, [vp, u8p, C.c_size_t, C.c_int64, u8p, szp]),
         "b200pir_dpir_answer_many": (C.c_int, [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_void_p),
                                                C.POINTER(C.c_size_t)]),
+        "b200pir_dpir_server_update": (C.c_int, [vp, u64p, u8p, C.c_size_t, u32p]),
+        "b200pir_dpir_server_state": (C.c_int, [vp, u32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # raises AttributeError if the .so does not export a declared symbol

@@ -7,6 +7,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstring>
 #include <functional>
@@ -26,6 +27,13 @@ struct b200pir_dpir {
   uint64_t rows, cols;
   DevBuf<uint32_t> a;
   DevBuf<uint32_t> b, out;
+  // what b200pir_dpir_load* laid out in `a`, for b200pir_dpir_server_update; from_load stays false for b200pir_dpir_create*
+  bool from_load = false;
+  int entry_format = 0;
+  uint64_t load_count = 0;               // entries the load iterated: len bytes, or 8 len bits
+  uint64_t num_entries = 0, bits_per_entry = 0;
+  b200pir_dpir_params params{};
+  bool fields_exact = false;             // no packed entry was wider than bits_per_entry: every element decodes field by field
 };
 
 extern "C" {
@@ -446,9 +454,16 @@ b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uin
     int flag = 0;
     B200_CUDA(cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
-    if (flag) throw Error(B200PIR_E_UNSUPPORTED, "load: a packed database word lies outside [-2^15, 2^15) (entries far wider than bits_per_entry)");
+    if (flag & 1) throw Error(B200PIR_E_UNSUPPORTED, "load: a packed database word lies outside [-2^15, 2^15) (entries far wider than bits_per_entry)");
+    h->fields_exact = !(flag & 2);
   }
   dpir_setup_tail(d_h.p, d_a2.p, l, n, p, info.delta, x, h1_squished, a2_t, h2, s);
+  h->from_load = true;
+  h->entry_format = entry_format;
+  h->load_count = count;
+  h->num_entries = num_entries;
+  h->bits_per_entry = bits_per_entry;
+  h->params = *params;
   return h.release();
 }
 }  // namespace
@@ -537,6 +552,18 @@ struct b200pir_dpir_server {
   DevBuf<uint32_t> d_a1, d_a1sq, d_msg0;
   DevBuf<uint8_t> d_img;         // query images of the passes that run on the tensor cores (every q_1, then every q_2)
   size_t img_q1 = 0, img_q2 = 0; // bytes of one q_1 / q_2 image
+  b200pir_dpir_params params{};  // as created, with num_entries and bits_per_entry: an update checks them against the load
+  uint64_t num_entries = 0, bits_per_entry = 0;
+  // update scratch, allocated by the first update and grown only for a larger one: per group of at most upd_cap elements
+  // (and as many rows), plus the tables of the whole batch and the hint
+  size_t upd_cap = 0, upd_tab = 0;
+  DevBuf<DpirUpdElem> u_el;
+  DevBuf<DpirUpdRow> u_rows;
+  DevBuf<int32_t> u_delta, u_D;
+  DevBuf<uint32_t> u_dh1, u_a2g, u_dh2, u_h2;
+  DevBuf<uint8_t> u_aimg, u_bimg;
+  DpirAesKey a1_key;             // SEED_A1's tables, expanded by the first update
+  bool have_a1_key = false;
   ~b200pir_dpir_server() {
     if (h_stage) cudaFreeHost(h_stage);
     if (h_resp) cudaFreeHost(h_resp);
@@ -751,6 +778,9 @@ int b200pir_dpir_server_create(int device, const b200pir_dpir_params* params, ui
   std::unique_ptr<b200pir_dpir_server> S(new b200pir_dpir_server());
   S->device = device;
   S->db = db;
+  S->params = *params;
+  S->num_entries = num_entries;
+  S->bits_per_entry = bits_per_entry;
   S->n = params->n; S->l = l; S->p = params->p; S->delta = info.delta; S->x = x; S->e = info.ne / x;
   S->dx = info.delta * x; S->rows1 = S->n * S->dx; S->c1 = (l / x + 2) / 3; S->lx3 = 3 * S->c1; S->dcols = db->cols;
   S->max_queries = max_queries;
@@ -847,6 +877,168 @@ int b200pir_dpir_answer_many(b200pir_dpir_server* S, const uint8_t* const* reque
   std::lock_guard<std::mutex> lk(S->mu);
   cudaSetDevice(S->device);
   dpir_serve(S, calls, -1, outs, out_lens);
+  API_END
+}
+
+// ---------------------------------------------------------------- DoublePIR entry updates (dpir_update.cu)
+namespace {
+constexpr size_t kDpirUpdGroup = 4096;    // changed elements (and so at most as many changed rows) patched per group
+
+// The batch as element patches sorted by (row, column): a repeated index ends with its last value, and the entries of one
+// packed element are combined into one patch.  Everything has been checked.
+std::vector<DpirUpdElem> dpir_update_elems(const b200pir_dpir* db, const b200pir_dpir_info& info, const uint64_t* idx, const uint8_t* val,
+                                           size_t count) {
+  std::vector<size_t> ord(count);
+  for (size_t k = 0; k < count; k++) ord[k] = k;
+  std::stable_sort(ord.begin(), ord.end(), [idx](size_t a, size_t b) { return idx[a] < idx[b]; });
+  const uint64_t m = db->params.m, bits = db->bits_per_entry;
+  const uint32_t p = (uint32_t)db->params.p;
+  std::vector<DpirUpdElem> el;
+  for (size_t k = 0; k < count; k++) {
+    if (k + 1 < count && idx[ord[k + 1]] == idx[ord[k]]) continue;        // a later value of the same index wins
+    const uint64_t i = idx[ord[k]];
+    const uint32_t v = val[ord[k]];
+    if (info.packing) {                   // bit field i % packing of element i / packing (sorted indices: elements in order)
+      const uint64_t e = i / info.packing;
+      const uint32_t sh = (uint32_t)(bits * (i % info.packing)), fm = ((1u << bits) - 1) << sh;
+      if (el.empty() || el.back().r * m + el.back().c != e) el.push_back(DpirUpdElem{e / m, e % m, 0, 0});
+      el.back().mask |= fm;
+      el.back().val = (el.back().val & ~fm) | (v << sh);
+    } else {                              // digit j = base_p(p, v, j) at row (i / m) ne + j, column i % m
+      uint32_t d = v;
+      for (uint64_t j = 0; j < info.ne; j++, d /= p) el.push_back(DpirUpdElem{(i / m) * info.ne + j, i % m, 0xFFFFFFFFu, d % p});
+    }
+  }
+  if (!info.packing)
+    std::sort(el.begin(), el.end(), [](const DpirUpdElem& a, const DpirUpdElem& b) { return a.r != b.r ? a.r < b.r : a.c < b.c; });
+  return el;
+}
+
+// One group of the batch: elements [e_off, e_off + n_el) and their rows [r_off, r_off + n_rows); blocks: (b, k0_b, k_b) of the
+// blocks b = r % x that have changed rows
+struct DpirUpdGroup {
+  size_t e_off, n_el, r_off, n_rows;
+  std::vector<std::array<uint64_t, 3>> blocks;
+};
+
+// Store, h_1 and hint patches of every group on the server's stream; h2 (host, (n delta x) x n) in and out.  Synchronises.
+void dpir_update(b200pir_dpir_server* S, const std::vector<DpirUpdElem>& el, uint32_t* h2) {
+  const cudaStream_t s = S->stream;
+  const uint64_t n = S->n, x = S->x, nd = n * S->delta;
+  std::vector<DpirUpdRow> rows;
+  std::vector<DpirUpdGroup> groups;
+  for (size_t g0 = 0; g0 < el.size(); g0 += kDpirUpdGroup) {
+    DpirUpdGroup G{g0, std::min(kDpirUpdGroup, el.size() - g0), rows.size(), 0, {}};
+    std::vector<DpirUpdRow> gr;
+    for (size_t k = 0; k < G.n_el; k++) {
+      if (gr.empty() || gr.back().r != el[g0 + k].r) gr.push_back(DpirUpdRow{el[g0 + k].r, 0, (uint32_t)k, 0, 0, 0});
+      gr.back().ne++;
+    }
+    std::stable_sort(gr.begin(), gr.end(), [x](const DpirUpdRow& a, const DpirUpdRow& b) { return a.r % x < b.r % x; });
+    for (size_t k0 = 0; k0 < gr.size();) {
+      size_t k1 = k0;
+      while (k1 < gr.size() && gr[k1].r % x == gr[k0].r % x) k1++;
+      for (size_t k = k0; k < k1; k++) {
+        gr[k].doff = nd * k0;
+        gr[k].dcol = (uint32_t)(k - k0);
+        gr[k].kb = (uint32_t)(k1 - k0);
+      }
+      G.blocks.push_back({gr[k0].r % x, k0, k1 - k0});
+      k0 = k1;
+    }
+    G.n_rows = gr.size();
+    rows.insert(rows.end(), gr.begin(), gr.end());
+    groups.push_back(std::move(G));
+  }
+  // scratch: sized for the largest group this batch can have, grown only for a larger batch
+  const size_t cap = std::min(kDpirUpdGroup, el.size());
+  if (cap > S->upd_cap) {
+    S->u_dh1.alloc(cap * n);
+    S->u_a2g.alloc(cap * n);
+    S->u_D.alloc(nd * cap);
+    S->u_aimg.alloc(dpir_gemm_a_bytes(nd, cap));
+    S->u_bimg.alloc(dpir_gemm_b_bytes(cap, n));
+    S->upd_cap = cap;
+  }
+  if (el.size() > S->upd_tab) {
+    S->u_el.alloc(el.size());
+    S->u_rows.alloc(el.size());
+    S->u_delta.alloc(el.size());
+    S->upd_tab = el.size();
+  }
+  S->u_dh2.ensure(nd * n);
+  S->u_h2.ensure(nd * x * n);
+  if (!S->have_a1_key) {
+    S->a1_key = dpir_aes_key(kDpirSeedA1);
+    S->have_a1_key = true;
+  }
+  b200pir_dpir* db = S->db;
+  B200_CUDA(cudaStreamSynchronize(db->stream));          // work still queued on the database handle's own stream first
+  B200_CUDA(cudaMemcpyAsync(S->u_el.p, el.data(), el.size() * sizeof(DpirUpdElem), cudaMemcpyHostToDevice, s));
+  B200_CUDA(cudaMemcpyAsync(S->u_rows.p, rows.data(), rows.size() * sizeof(DpirUpdRow), cudaMemcpyHostToDevice, s));
+  B200_CUDA(cudaMemcpyAsync(S->u_h2.p, h2, nd * x * n * 4, cudaMemcpyHostToDevice, s));
+  for (const DpirUpdGroup& G : groups) {
+    const DpirUpdElem* gel = S->u_el.p + G.e_off;
+    const DpirUpdRow* grows = S->u_rows.p + G.r_off;
+    int32_t* gdelta = S->u_delta.p + G.e_off;
+    launch_dpir_upd_store(db->a.p, db->cols, gel, (uint32_t)G.n_el, gdelta, s);
+    launch_dpir_upd_dh1(S->u_dh1.p, grows, (uint32_t)G.n_rows, gel, gdelta, n, S->a1_key, s);
+    launch_dpir_upd_digits(S->h1.p, S->c1, S->u_D.p, grows, (uint32_t)G.n_rows, S->u_dh1.p, n, (uint32_t)S->p, (uint32_t)S->delta, x, s);
+    launch_dpir_upd_gather_a2(S->u_a2g.p, S->a2t.p, S->lx3, grows, (uint32_t)G.n_rows, n, x, s);
+    for (const auto& B : G.blocks) {                     // dh_2[block b] = D_b (nd x k_b) * A_2 rows (k_b x n)
+      const uint64_t b = B[0], k0 = B[1], kb = B[2];
+      launch_dpir_gemm_b_image(S->u_bimg.p, S->u_a2g.p + k0 * n, kb, n, s);
+      launch_dpir_gemm_rows(S->u_dh2.p, S->u_aimg.p, reinterpret_cast<const uint32_t*>(S->u_D.p) + nd * k0, nd, kb, S->u_bimg.p, n, s);
+      launch_dpir_upd_add(S->u_h2.p + b * nd * n, S->u_dh2.p, nd * n, s);
+    }
+  }
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaMemcpyAsync(h2, S->u_h2.p, nd * x * n * 4, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  B200_CUDA(cudaGetLastError());
+}
+}  // namespace
+
+int b200pir_dpir_server_update(b200pir_dpir_server* S, const uint64_t* indices, const uint8_t* values, size_t count, uint32_t* h2) {
+  API_BEGIN
+  if (!S || !h2 || (count && (!indices || !values))) throw Error(B200PIR_E_BADARG, "null argument");
+  b200pir_dpir* db = S->db;
+  if (!db->from_load) throw Error(B200PIR_E_UNSUPPORTED, "update: the server's database was not laid out by b200pir_dpir_load*");
+  if (db->rows < S->l) throw Error(B200PIR_E_UNSUPPORTED, "update: the server holds a chunk of the database (fewer than l rows)");
+  if (!db->fields_exact)
+    throw Error(B200PIR_E_UNSUPPORTED, "update: the load packed entries wider than bits_per_entry; its elements do not decode field by field");
+  const b200pir_dpir_params& P = db->params;
+  if (S->num_entries != db->num_entries || S->bits_per_entry != db->bits_per_entry || S->params.n != P.n || S->params.l != P.l ||
+      S->params.m != P.m || S->params.logq != P.logq || S->params.p != P.p)
+    throw Error(B200PIR_E_SHAPE, "update: the server's parameters, num_entries or bits_per_entry differ from its database's load");
+  if (S->n * 4 > 200 * 1024) throw Error(B200PIR_E_UNSUPPORTED, "update: n above 51200");
+  const b200pir_dpir_info info = dpir_info(&P, db->num_entries, db->bits_per_entry, nullptr);
+  const bool bits_format = db->entry_format == B200PIR_DPIR_ENTRY_BITS;
+  for (size_t k = 0; k < count; k++) {
+    if (indices[k] >= db->load_count)
+      throw Error(B200PIR_E_SHAPE, "update: index " + std::to_string(indices[k]) + " is past the " + std::to_string(db->load_count) +
+                                       " entries the load read");
+    if ((bits_format && values[k] > 1) || (info.packing && (values[k] >> db->bits_per_entry)))
+      throw Error(B200PIR_E_BADARG, "update: value " + std::to_string(values[k]) + " of entry " + std::to_string(indices[k]) +
+                                        " does not fit the entry format");
+  }
+  if (count == 0) return 0;
+  const std::vector<DpirUpdElem> el = dpir_update_elems(db, info, indices, values, count);
+  std::lock_guard<std::mutex> lk(S->mu);
+  std::lock_guard<std::mutex> lk_db(db->mu);
+  cudaSetDevice(S->device);
+  dpir_update(S, el, h2);
+  API_END
+}
+
+int b200pir_dpir_server_state(b200pir_dpir_server* S, uint32_t* h1_squished) {
+  API_BEGIN
+  if (!S || !h1_squished) throw Error(B200PIR_E_BADARG, "null argument");
+  std::lock_guard<std::mutex> lk(S->mu);
+  cudaSetDevice(S->device);
+  B200_CUDA(cudaMemcpyAsync(h1_squished, S->h1.p, S->h1.n * 4, cudaMemcpyDeviceToHost, S->stream));
+  B200_CUDA(cudaStreamSynchronize(S->stream));
+  B200_CUDA(cudaGetLastError());
   API_END
 }
 

@@ -5,15 +5,13 @@
 // k_dpir_derive: Matrix::derive_from_seed (matrix/matrix.rs:125-135) = derive_with_aes (matrix/derivation.rs:11-22): the
 // matrix's bytes are the AES-128 keystream in Ctr64BE mode, restarted every 64 KiB chunk with IV = BE64(chunk) || 0^8, i.e.
 // block b of the matrix encrypts BE64(b / 4096) || BE64(b % 4096).  u32 words are read little-endian from the keystream.
-// One thread per 16-byte block; T-tables (FIPS-197 section 5.2.1's round as four 32-bit table lookups per column) in shared
-// memory.  The lookups are data-dependent, so this is NOT constant-time: that is fine here, because the key and the output are
-// public (the reference derives public matrices only, matrix.rs:120-124) and nothing secret ever passes through this kernel.
+// One thread per 16-byte block, through the block function of dpir_aes.cuh.
 //
 // k_dpir_layout: Db::load_data / load_data_fast (database/database.rs:168-247) as a gather, one thread per word of one band of
 // rows of the l x m matrix, then "Map DB elems to [-p/2; p/2]" (the wrapping subtraction of p/2 from every word, touched or
 // not).  A band's entries are one contiguous range of the input, so only that range needs to be on the device (api.cu stages
 // the input band by band).
-#include "kernels.h"
+#include "dpir_aes.cuh"
 
 namespace b200pir {
 
@@ -41,46 +39,21 @@ void aes_sbox(uint8_t s[256]) {
   }
 }
 
-__device__ __forceinline__ uint32_t ror8(uint32_t v, int n) { return __funnelshift_r(v, v, n); }
-
 // grid-stride over the 16-byte blocks of an out_words-word matrix
 __global__ void __launch_bounds__(256) k_dpir_derive(uint32_t* __restrict__ out, size_t out_words, const __grid_constant__ DpirAesKey key) {
   __shared__ uint32_t te[4][256];
   __shared__ uint32_t sb[256];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-    const uint32_t t = key.te0[i];
-    te[0][i] = t; te[1][i] = ror8(t, 8); te[2][i] = ror8(t, 16); te[3][i] = ror8(t, 24);
-    sb[i] = key.sbox[i];
-  }
+  dpir_aes_tables(te, sb, key);
   __syncthreads();
   const size_t blocks = (out_words + 3) / 4;
   for (size_t b = (size_t)blockIdx.x * blockDim.x + threadIdx.x; b < blocks; b += (size_t)gridDim.x * blockDim.x) {
-    // derive_with_aes_at(key, i as u32, chunk): the chunk index is cast to u32 before it is widened into the IV
-    const uint64_t chunk = (uint32_t)(b >> 12), ctr = b & 4095;
-    // state columns as big-endian words (FIPS-197 section 3.4), round key 0 added
-    uint32_t s0 = (uint32_t)(chunk >> 32) ^ key.rk[0], s1 = (uint32_t)chunk ^ key.rk[1];
-    uint32_t s2 = (uint32_t)(ctr >> 32) ^ key.rk[2], s3 = (uint32_t)ctr ^ key.rk[3];
-#pragma unroll
-    for (int r = 1; r < 10; r++) {
-      const uint32_t t0 = te[0][s0 >> 24] ^ te[1][(s1 >> 16) & 255] ^ te[2][(s2 >> 8) & 255] ^ te[3][s3 & 255] ^ key.rk[4 * r];
-      const uint32_t t1 = te[0][s1 >> 24] ^ te[1][(s2 >> 16) & 255] ^ te[2][(s3 >> 8) & 255] ^ te[3][s0 & 255] ^ key.rk[4 * r + 1];
-      const uint32_t t2 = te[0][s2 >> 24] ^ te[1][(s3 >> 16) & 255] ^ te[2][(s0 >> 8) & 255] ^ te[3][s1 & 255] ^ key.rk[4 * r + 2];
-      const uint32_t t3 = te[0][s3 >> 24] ^ te[1][(s0 >> 16) & 255] ^ te[2][(s1 >> 8) & 255] ^ te[3][s2 & 255] ^ key.rk[4 * r + 3];
-      s0 = t0; s1 = t1; s2 = t2; s3 = t3;
-    }
-    uint32_t o[4];
-    // last round: SubBytes, ShiftRows, AddRoundKey (no MixColumns)
-    o[0] = (sb[s0 >> 24] << 24 | sb[(s1 >> 16) & 255] << 16 | sb[(s2 >> 8) & 255] << 8 | sb[s3 & 255]) ^ key.rk[40];
-    o[1] = (sb[s1 >> 24] << 24 | sb[(s2 >> 16) & 255] << 16 | sb[(s3 >> 8) & 255] << 8 | sb[s0 & 255]) ^ key.rk[41];
-    o[2] = (sb[s2 >> 24] << 24 | sb[(s3 >> 16) & 255] << 16 | sb[(s0 >> 8) & 255] << 8 | sb[s1 & 255]) ^ key.rk[42];
-    o[3] = (sb[s3 >> 24] << 24 | sb[(s0 >> 16) & 255] << 16 | sb[(s1 >> 8) & 255] << 8 | sb[s2 & 255]) ^ key.rk[43];
-    // keystream bytes 4w..4w+3 are big-endian column w; the matrix reads them as a little-endian u32.  The last block may
-    // be partial (rows * cols * 4 is a multiple of 4 only): its words past the end are not written.
+    const uint4 o = dpir_aes_block(te, sb, key, b);
+    // the last block may be partial (rows * cols * 4 is a multiple of 4 only): its words past the end are not written
     if (4 * b + 4 <= out_words) {
-      *reinterpret_cast<uint4*>(out + 4 * b) = make_uint4(__byte_perm(o[0], 0, 0x0123), __byte_perm(o[1], 0, 0x0123),
-                                                          __byte_perm(o[2], 0, 0x0123), __byte_perm(o[3], 0, 0x0123));
+      *reinterpret_cast<uint4*>(out + 4 * b) = o;
     } else {
-      for (int w = 0; w < 4 && 4 * b + w < out_words; w++) out[4 * b + w] = __byte_perm(o[w], 0, 0x0123);
+      const uint32_t w[4] = {o.x, o.y, o.z, o.w};
+      for (int i = 0; i < 4 && 4 * b + i < out_words; i++) out[4 * b + i] = w[i];
     }
   }
 }
@@ -100,13 +73,15 @@ __device__ __forceinline__ uint32_t entry(const uint8_t* __restrict__ data, size
 //                (the `iter.peek().is_none()` flush).
 //   packing = 0: data[(i / m) ne + j][i % m] = base_p(p, e_i, j), so word (row, col) holds digit row % ne of entry
 //                (row / ne) m + col.
-// Sets *out_of_range when a centred word lies outside [-2^15, 2^15), the operand range of the setup GEMM (dpir_gemm.cu).
+// Sets bit 0 of *out_of_range when a centred word lies outside [-2^15, 2^15), the operand range of the setup GEMM
+// (dpir_gemm.cu), and bit 1 when a packed entry is wider than `bits` (its element then no longer decodes field by field).
 template <bool BITS>
 __global__ void k_dpir_layout(uint32_t* __restrict__ band, const uint8_t* __restrict__ data, uint64_t base, uint64_t count,
                               uint64_t r0, uint64_t rows, uint64_t m, uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p,
                               int* __restrict__ out_of_range) {
   const uint64_t words = rows * m, k0 = r0 * m;
   bool bad = false;
+  uint32_t wide = 0;
   for (uint64_t kb = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; kb < words; kb += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t k = k0 + kb;
     uint32_t v = 0;
@@ -116,7 +91,9 @@ __global__ void k_dpir_layout(uint32_t* __restrict__ band, const uint8_t* __rest
         uint32_t coeff = 1;
         const uint64_t last = first + packing < count ? first + packing : count;
         for (uint64_t i = first; i < last; i++) {
-          v += entry<BITS>(data, i - base) * coeff;
+          const uint32_t e = entry<BITS>(data, i - base);
+          if (!BITS) wide |= e >> bits;                                // a bit always fits its field
+          v += e * coeff;
           coeff *= 1u << bits;
         }
       }
@@ -133,7 +110,7 @@ __global__ void k_dpir_layout(uint32_t* __restrict__ band, const uint8_t* __rest
     band[kb] = v;
     bad |= (int32_t)v < -32768 || (int32_t)v > 32767;
   }
-  if (bad) atomicOr(out_of_range, 1);
+  if (bad || wide) atomicOr(out_of_range, (bad ? 1 : 0) | (wide ? 2 : 0));
 }
 
 unsigned grid_for(size_t items, int block) {

@@ -248,9 +248,31 @@ void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cuda
 // Db::load_data (bits_format false) / load_data_fast (true), database.rs:168-247, for the band of layout rows [r0, r0 + rows):
 // the band's words of the l x m matrix minus p/2 (every word written) into band (rows x m).  Of the `count` entries the
 // iterator yields, `data` holds those from entry `base` on (entry i is at data[i - base], or at bit (i - base) % 8 of byte
-// (i - base) / 8).  *out_of_range |= 1 when a word lies outside the setup GEMM's [-2^15, 2^15)
+// (i - base) / 8).  *out_of_range |= 1 when a word lies outside the setup GEMM's [-2^15, 2^15), |= 2 when a packed entry
+// is wider than `bits` (b200pir_dpir_server_update can then not rebuild its element from the store)
 void launch_dpir_layout(uint32_t* band, const uint8_t* data, uint64_t base, uint64_t count, bool bits_format, uint64_t r0,
                         uint64_t rows, uint64_t m, uint32_t packing, uint32_t bits, uint32_t ne, uint32_t p, int* out_of_range,
                         cudaStream_t s);
+
+// ---- DoublePIR entry updates (dpir_update.cu): Db::_set on a loaded database, and setup()'s outputs patched to match
+// One changed Z_p element of the l x m layout: new = (old & ~mask) | val, old read from its squished store field
+struct DpirUpdElem { uint64_t r, c; uint32_t mask, val; };
+// One changed layout row of a group: its elements are [e0, e0 + ne) of the group's element table.  Rows are ordered by block
+// r % x, so row k of the table is column k of the group's digit-difference matrix D, and the rows of block b are columns
+// [k0_b, k0_b + k_b); D_b (n delta x k_b, row-major) starts at word doff = n delta k0_b of D, and this row is its column dcol.
+struct DpirUpdRow { uint64_t r, doff; uint32_t e0, ne, dcol, kb; };
+// store patch: each element's field rewritten in the squished store (dcols words a row) and its change new - old to delta[]
+void launch_dpir_upd_store(uint32_t* store, uint64_t dcols, const DpirUpdElem* el, uint32_t n_el, int32_t* delta, cudaStream_t s);
+// dh1 (nrows x n) = sum over each row's elements of delta * A_1[c, :], the A_1 rows derived from `key` in the kernel
+void launch_dpir_upd_dh1(uint32_t* dh1, const DpirUpdRow* rows, uint32_t nrows, const DpirUpdElem* el, const int32_t* delta, uint64_t n,
+                         const DpirAesKey& key, cudaStream_t s);
+// h_1's base-p digits in h1_squished (c1 words a row) moved by dh1, the digit differences written into D
+void launch_dpir_upd_digits(uint32_t* h1sq, uint64_t c1, int32_t* D, const DpirUpdRow* rows, uint32_t nrows, const uint32_t* dh1,
+                            uint64_t n, uint32_t p, uint32_t delta, uint64_t x, cudaStream_t s);
+// a2g (nrows x n) = the rows A_2[r / x, :] of the changed rows, read from a_2^T (a2t: n x lx3)
+void launch_dpir_upd_gather_a2(uint32_t* a2g, const uint32_t* a2t, uint64_t lx3, const DpirUpdRow* rows, uint32_t nrows, uint64_t n,
+                               uint64_t x, cudaStream_t s);
+// dst[i] += src[i], wrapping
+void launch_dpir_upd_add(uint32_t* dst, const uint32_t* src, size_t words, cudaStream_t s);
 
 }  // namespace b200pir

@@ -172,6 +172,8 @@ class Server:
         check(LIB.b200pir_dpir_server_create(device, C.byref(_params(params)), num_entries, bits_per_entry, db._h, h1.ctypes.data,
                                              a2.ctypes.data, max_queries, C.byref(h)))
         self._h = h
+        self._h1_shape = h1.shape
+        self._h2_words = h1.shape[0] * int(params["n"]) if h1.ndim == 2 else None     # h2: (n delta x) x n
 
     def answer_size(self, request):
         n = C.c_size_t()
@@ -206,6 +208,30 @@ class Server:
         olen = (C.c_size_t * k)(*sizes)
         check(LIB.b200pir_dpir_answer_many(self._h, reqs, lens, k, optr, olen))
         return [o.raw[:olen[i]] for i, o in enumerate(outs)]
+
+    def update(self, indices, values, h2):
+        """Db::_set of entries `indices` to `values` (bytes, or bits 0/1 for ENTRY_BITS, as the load read them) on the database
+        this server borrows, with the store, this server's h_1 and the hint patched to match (b200pir_dpir_server_update): returns
+        the new hint, what load() returns as h2 for the modified bytes.  h2: the hint as load() or the previous update left it.
+        A repeated index ends with its last value.  Clients must fetch the new hint before they query the updated entries."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint64).reshape(-1)
+        vals = np.asarray(values).reshape(-1)
+        if vals.size != idx.size:
+            raise ValueError("%d indices but %d values" % (idx.size, vals.size))
+        if vals.size and (vals.min() < 0 or vals.max() > 255):
+            raise ValueError("values must be bytes")
+        vals = np.ascontiguousarray(vals, dtype=np.uint8)
+        out = np.array(h2, dtype=np.uint32, order="C", copy=True)
+        if self._h2_words is not None and out.size != self._h2_words:
+            raise ValueError("h2 has %d words; this server's hint has %d" % (out.size, self._h2_words))
+        check(LIB.b200pir_dpir_server_update(self._h, idx.ctypes.data, vals.ctypes.data, idx.size, out.ctypes.data))
+        return out
+
+    def state(self):
+        """server_state[0] as the server now holds it: h1_squished, shaped as it was given to the constructor."""
+        out = np.zeros(self._h1_shape, dtype=np.uint32)
+        check(LIB.b200pir_dpir_server_state(self._h, out.ctypes.data))
+        return out
 
     def close(self):
         if getattr(self, "_h", None):
