@@ -1,6 +1,8 @@
-"""Read-back rate of the HBM database on one GPU, parameter set S8 (format 2, 8 GiB in HBM).
+"""Read-back and load rates of the HBM database on one GPU, parameter set S8 (8 GiB in HBM) in database format --format.
 
 Prints the card's name and power limit, then
+  - b200pir_db_fill_synthetic and Database.from_words (b200pir_db_upload from a host array), wall time ending in a device
+    synchronise (median of --reps runs);
   - b200pir_db_download of the whole database and b200pir_db_save_file to --dir, wall time ending in a device synchronise,
     with GB/s (median of --reps runs);
   - the device time of the un-tiling kernels alone (torch.profiler's CUDA activity of k_db_export_*, summed over one
@@ -8,7 +10,7 @@ Prints the card's name and power limit, then
   - b200pir_db_load_file of the saved file;
   - single-query latency (random public parameters and query: no client keys needed) while a save runs, against idle.
 
-    python scripts/db_export_probe.py [--reps 3] [--dir /tmp] [--out DIR]
+    python scripts/db_export_probe.py [--format 2] [--reps 3] [--dir /tmp] [--out DIR]
 """
 import argparse
 import json
@@ -42,6 +44,7 @@ def rand_ntt(rng, words):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--format", type=int, default=2, choices=(0, 1, 2))
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--dir", default=tempfile.gettempdir())
     ap.add_argument("--out", default=None)
@@ -49,11 +52,14 @@ def main():
     import sdk_b200.spiral as S
     card = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], text=True)
     print("card:", card.strip().splitlines()[0])
-    rec = {"card": card.strip().splitlines()[0], "params": "S8", "format": 2, "reps": args.reps}
+    rec = {"card": card.strip().splitlines()[0], "params": "S8", "format": args.format, "reps": args.reps}
     G = S.Params(**S8)
-    db = S.Database(G, fmt=2)
-    db.fill_synthetic(1)
+    db = S.Database(G, fmt=args.format)
+    db.fill_synthetic(1)                                                   # first fill: the kernel's module is loaded here
     nbytes = G.slices * G.dim0 * G.num_per * G.poly_len * 8
+    t = [timed(lambda: db.fill_synthetic(1), G) for _ in range(args.reps)]
+    rec["fill_synthetic_s"] = statistics.median(t)
+    print("fill_synthetic: %.3f s  %.2f GB/s" % (rec["fill_synthetic_s"], nbytes / rec["fill_synthetic_s"] / 1e9))
     words = np.empty(nbytes // 8, dtype=np.uint64)
     words.fill(0)                                                          # fault the pages in outside the timed window
     db.to_words(out=words)                                                 # first export: staging allocated here
@@ -61,6 +67,14 @@ def main():
     rec["download_s"] = statistics.median(t)
     rec["download_GBps"] = nbytes / rec["download_s"] / 1e9
     print("download: %.3f s  %.2f GB/s" % (rec["download_s"], rec["download_GBps"]))
+
+    def upload():
+        S.Database.from_words(G, words, fmt=args.format).close()
+
+    upload()
+    t = [timed(upload, G) for _ in range(args.reps)]
+    rec["from_words_s"] = statistics.median(t)
+    print("from_words: %.3f s  %.2f GB/s" % (rec["from_words_s"], nbytes / rec["from_words_s"] / 1e9))
 
     path = os.path.join(args.dir, "db_export_probe_%d.bin" % os.getpid())
     try:
@@ -84,7 +98,7 @@ def main():
         except Exception as e:                                             # the probe still reports the rest
             print("kernel timing unavailable:", e)
 
-        fresh = S.Database(G, fmt=2)
+        fresh = S.Database(G, fmt=args.format)
         t = [timed(lambda: S.LIB.b200pir_db_load_file(G._h, fresh._h, path.encode()), G) for _ in range(args.reps)]
         rec["load_file_s"] = statistics.median(t)
         print("load_file: %.3f s  %.2f GB/s" % (rec["load_file_s"], nbytes / rec["load_file_s"] / 1e9))

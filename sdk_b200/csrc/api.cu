@@ -235,22 +235,6 @@ struct b200pir_db {
   DevBuf<uint8_t> store;    // db_bytes(layout, slices) bytes
   // The first dimension's product is z-major (formats 1 and 2: u32 [query][slice][n][z][row][ct_row]) or ntt32 (format 0)
   bool zmajor_product() const { return layout.format != 0; }
-  // The bulk loaders (upload, synthetic fill) build a slice in the format-0 layout and then place_slice0 it.  Where slice s is
-  // built: returned as the base pointer the format-0 kernels address slice s from (imad_cell).  For format 0 that is the
-  // store.  Otherwise the slice is built in `scratch`, one format-0 slice allocated on first use, and the base is `scratch`
-  // minus s format-0 slices: only slice s is ever addressed from it, and that slice is the scratch.
-  uint4* slice0_base(int s, DevBuf<uint8_t>& scratch) {
-    if (layout.format == 0) return reinterpret_cast<uint4*>(store.p);
-    const size_t slice0_bytes = imad_cell(layout.G, 1, 0, 0, 0) * sizeof(uint4);
-    if (!scratch.p) scratch.alloc(slice0_bytes);
-    return reinterpret_cast<uint4*>(reinterpret_cast<uintptr_t>(scratch.p) - (uintptr_t)s * slice0_bytes);
-  }
-  // slice s, built at slice0_base(s, scratch), into the store: nothing to do for format 0, a re-tiling for formats 1 and 2
-  void place_slice0(int s, const DevBuf<uint8_t>& scratch, cudaStream_t st) {
-    const uint4* src = reinterpret_cast<const uint4*>(scratch.p);
-    if (layout.format == 1) launch_db_to_frag(layout.F, src, reinterpret_cast<uint4*>(store.p), s, st);
-    else if (layout.format == 2) launch_db_to_tc5(layout.T, src, store.p, s, st);
-  }
   // Presence (lib/server's SparseDb, db/sparse_db.rs:5-47: an item exists once it has been written).  Storage stays dense in HBM
   // (absent = zero polynomial, so every sum is unchanged); what the map buys is COST: on the wgmma path whole 32-row x 32-j
   // tiles without a present item are neither fetched nor multiplied (tile_mask, one bit per tile, kept on the device).
@@ -815,21 +799,19 @@ namespace {
 // to that range of the slice (valid until the next call).
 template <typename Fetch>
 void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fetch) {
-  // reference layout is z-major: stage a range of z at a time (<= 64 MiB)
+  // reference layout is z-major: stage a range of z at a time in the writers' staging (w_wbytes, at least 64 MiB).  An export
+  // may still be copying its last chunk out of it; that copy is queued on the context's stream, ahead of this upload's copies.
   const size_t per_z = (size_t)c->dim0 * c->num_per;
-  int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, ((size_t)64 << 20) / (per_z * 8)));
-  DevBuf<uint64_t> stage(per_z * zc);
-  const MulGeom& G = db->layout.G;
-  DevBuf<uint8_t> scratch;
-  uint4* dst = db->slice0_base((int)slice, scratch) + imad_cell(G, (int)slice, 0, 0, 0);
+  int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
+  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, per_z * zc * 8));
+  uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
   for (int z0 = 0; z0 < POLY; z0 += zc) {
     int cur = std::min(zc, POLY - z0);
     const uint64_t* src = fetch((size_t)z0 * per_z, per_z * cur);
-    B200_CUDA(cudaMemcpyAsync(stage.p, src, per_z * cur * 8, cudaMemcpyHostToDevice, c->stream));
-    launch_db_retile_chunk(G, db->shard, dst, stage.p, z0, cur, c->stream);
+    B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, c->stream));
+    launch_db_import(db->layout, db->shard, (int)slice, stage, z0, cur, c->stream);
     B200_CUDA(cudaStreamSynchronize(c->stream));
   }
-  db->place_slice0((int)slice, scratch, c->stream);
   db->mark_slice((int)slice, c->stream);
   B200_CUDA(cudaStreamSynchronize(c->stream));
   B200_CUDA(cudaGetLastError());
@@ -1165,16 +1147,7 @@ int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
   if (!c) throw Error(B200PIR_E_BADARG, "null ctx");
   Guard gd(c);
   check_db(c, db);
-  // keep each launch's grid below 2^31 CTAs; slices built in the scratch go one at a time
-  size_t per_slice = (size_t)db->rows * (c->dim0 / 2);
-  int step = (int)std::max<size_t>(1, std::min<size_t>(c->slices, ((size_t)1 << 30) / per_slice));
-  if (db->layout.format != 0) step = 1;
-  DevBuf<uint8_t> scratch;
-  for (int s0 = 0; s0 < c->slices; s0 += step) {
-    launch_db_synth(c->dp, db->layout.G, db->shard, db->slice0_base(s0, scratch), seed, c->hp.p, s0,
-                    std::min(step, c->slices - s0), c->stream);
-    db->place_slice0(s0, scratch, c->stream);
-  }
+  launch_write_synthetic(c->dp, db->layout, db->shard, seed, c->hp.p, c->stream);
   for (int s0 = 0; s0 < c->slices; s0++) db->mark_slice(s0, c->stream);
   B200_CUDA(cudaStreamSynchronize(c->stream));
   B200_CUDA(cudaGetLastError());

@@ -37,50 +37,6 @@ __device__ __forceinline__ uint32_t limb4(uint32_t x0, uint32_t x1, uint32_t x2,
   return ((x0 >> sh) & 127u) | (((x1 >> sh) & 127u) << 8) | (((x2 >> sh) & 127u) << 16) | (((x3 >> sh) & 127u) << 24);
 }
 
-// format 0 (mul_kernels.cu: uint4 [row][jp][z]) of one slice  ->  fragment order.  One warp per (z, mt, ks).
-__global__ void __launch_bounds__(256)
-k_db_to_frag(ImmaGeom F, const uint4* __restrict__ db0_slice, uint4* __restrict__ dbf, int slice) {
-  const int lane = threadIdx.x & 31;
-  const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const size_t total = (size_t)POLY * F.mt * F.ks;
-  if (warp >= total) return;
-  const int ks = (int)(warp % F.ks);
-  const int mt = (int)((warp / F.ks) % F.mt);
-  const int z = (int)(warp / ((size_t)F.ks * F.mt));
-  const int g = lane >> 2, t = lane & 3;
-  const int half = F.dim0 >> 1;
-  uint32_t res[2][2][2][4];        // [n][row half (g, g+8)][k half (0, +16)][i]
-#pragma unroll
-  for (int rh = 0; rh < 2; rh++) {
-    const int ii = mt * 16 + g + 8 * rh;
-#pragma unroll
-    for (int kh = 0; kh < 2; kh++) {
-      const int j0 = ks * 32 + 16 * kh + 4 * t;       // j0 .. j0+3
-#pragma unroll
-      for (int p = 0; p < 2; p++) {                   // two uint4 cells: (j0, j0+1), (j0+2, j0+3)
-        const int jp = (j0 >> 1) + p;
-        uint4 w = make_uint4(0, 0, 0, 0);
-        if (ii < F.rows && jp < half) w = db0_slice[((size_t)ii * half + jp) * POLY + z];
-        res[0][rh][kh][2 * p] = w.x; res[1][rh][kh][2 * p] = w.y;
-        res[0][rh][kh][2 * p + 1] = w.z; res[1][rh][kh][2 * p + 1] = w.w;
-      }
-    }
-  }
-#pragma unroll
-  for (int n = 0; n < 2; n++) {
-    uint4* dst = dbf + (((((size_t)slice * 2 + n) * POLY + z) * F.mt + mt) * F.ks + ks) * 4 * 32 + lane;
-#pragma unroll
-    for (int l = 0; l < 4; l++) {
-      uint4 o;
-      o.x = limb4(res[n][0][0][0], res[n][0][0][1], res[n][0][0][2], res[n][0][0][3], l);   // a0: row g,   k 4t..
-      o.y = limb4(res[n][1][0][0], res[n][1][0][1], res[n][1][0][2], res[n][1][0][3], l);   // a1: row g+8
-      o.z = limb4(res[n][0][1][0], res[n][0][1][1], res[n][0][1][2], res[n][0][1][3], l);   // a2: row g,   k 16+4t..
-      o.w = limb4(res[n][1][1][0], res[n][1][1][1], res[n][1][1][2], res[n][1][1][3], l);   // a3: row g+8
-      dst[(size_t)l * 32] = o;
-    }
-  }
-}
-
 // expanded queries (format of mul_kernels.cu: uint4 [jp][jb][z]) -> B fragments
 //   qf[n][z][nt][ks][limb m][lane] = uint2{b0, b1};  column (nt*8 + g) = 2*query + ciphertext row
 __global__ void __launch_bounds__(256)
@@ -429,11 +385,6 @@ bool imma_supports_16(const ImmaGeom& F) {
   return (size_t)4 * F.ks * 128 * sizeof(uint2) + (size_t)8 * IMMA_STAGES16 * 128 * sizeof(uint4) <= 224 * 1024;
 }
 
-void launch_db_to_frag(const ImmaGeom& F, const uint4* db0_slice, uint4* dbf, int slice, cudaStream_t s) {
-  size_t warps = (size_t)POLY * F.mt * F.ks;
-  ++g_kernel_launches;
-  k_db_to_frag<<<grid1d(warps * 32, 256), 256, 0, s>>>(F, db0_slice, dbf, slice);
-}
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s) {
   const int ntiles = imma_query_tiles(nq);
   size_t warps = (size_t)POLY * ntiles * F.ks;

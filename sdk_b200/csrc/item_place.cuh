@@ -1,10 +1,10 @@
 // Where one NTT coordinate z of one database item lives in each device layout, and how it is read back.  Item (slice, local
 // row il, column j) holds, at every z, the residue mod q0 (`lo`) and mod q1 (`hi`) of the packed word lo | hi << 32
-// (loading.rs:34-41 pack_ntt_poly).  The single-item upsert, the batched raw-byte writer (k_write_items) and the export
-// kernels (export_kernels.cu) all address the database through these maps, so every writer and reader agrees on the layouts;
-// the host sizes the store with db_bytes.  The maps are __host__ __device__ and use no CUDA types:
-// tests/cpp/db_layout_inverse.cpp checks on the CPU that place and fetch are mutually inverse, that no two items share a
-// byte and that every byte a writer touches lies inside db_bytes.
+// (loading.rs:34-41 pack_ntt_poly).  The single-item upsert, the batched item writer (k_write_items: raw bytes or the
+// synthetic database) and the import and export kernels (export_kernels.cu) all address the database through these maps, so
+// every writer and reader agrees on the layouts; the host sizes the store with db_bytes.  The maps are __host__ __device__
+// and use no CUDA types: tests/cpp/db_layout_inverse.cpp checks on the CPU that place and fetch are mutually inverse, that no
+// two items share a byte and that every byte a writer touches lies inside db_bytes.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -63,6 +63,10 @@ TC5_HD size_t frag_in_plane(const ImmaGeom& F, int il, int j, int l) {
   return ((size_t)(il >> 4) * F.ks + (j >> 5)) * FRAG_GROUP + frag_byte(il & 15, j & 31, l);
 }
 TC5_HD size_t frag_plane(const ImmaGeom& F, int slice, int n, int z) { return limb_plane(F.mt, F.ks, FRAG_GROUP, slice, n, z); }
+// index of the group (mt, ks) of plane (slice, n, z), in FRAG_GROUP-byte units (the import kernel writes whole groups)
+TC5_HD size_t frag_db_group(const ImmaGeom& F, int slice, int n, int z, int mt, int ks) {
+  return ((((size_t)slice * 2 + n) * POLY + z) * F.mt + mt) * F.ks + ks;
+}
 
 // format 2 (tc5_kernels.cu): tile images dbT[slice][n][z][mt][ks][4096 B], byte tc5_tile_off(4 row + l, k)
 TC5_HD size_t tc5_in_plane(const Tc5Geom& T, int il, int j, int l) {

@@ -66,21 +66,12 @@ void launch_query_to_dev(const MulGeom& G, uint4* q_dev, const uint64_t* v_first
 // Row sharding of the second-dimension index: this GPU holds global rows ii = il*count + index
 // (il = local row, G.num_per local rows).  index=0,count=1 is the whole database.
 struct Shard { int index, count; };
-// reference layout u64 [zc][num_per_global][dim0] (z in [z0,z0+zc))  ->  db_dev slice (local rows)
-void launch_db_retile_chunk(const MulGeom& G, Shard sh, uint4* db_dev_slice, const uint64_t* ref_chunk, int z0, int zc,
-                            cudaStream_t s);
-// synthetic DB: plaintext coeff = splitmix64(seed, ((slice*items + item)*2048 + z)) % p, recentred, NTT'd, packed
-// (server.rs:223-275 with a counter PRNG; item = j*num_per_global + ii)
-void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_dev, uint64_t seed, uint64_t pt_modulus,
-                     int slice_begin, int slice_count, cudaStream_t s);
 
 // ---- first dimension on INT8 tensor cores (imma_kernels.cu): database in MMA fragment order
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
 bool imma_supports_16(const ImmaGeom& F);                 // 16 queries per database pass fit one CTA's shared memory
 inline int imma_query_tiles(int nq) { return nq > 8 ? 4 : (nq > 4 ? 2 : 1); }   // column tiles of 4 queries
 void upload_imma_constants(const Twiddle* lo, cudaStream_t s);
-// one slice in the IMAD layout (uint4 [row][jp][z]) -> fragment order
-void launch_db_to_frag(const ImmaGeom& F, const uint4* db0_slice, uint4* dbf, int slice, cudaStream_t s);
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s);
 // out_zm: u32 [query][slice][n][z][row][ct_row]  (queries out_stride words apart)
 void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* dbf, const uint2* qf, uint32_t* out_zm,
@@ -94,7 +85,6 @@ void launch_zmajor_to_ntt32(const ImmaGeom& F, const uint32_t* in_zm, uint32_t* 
 // ---- first dimension on wgmma (tc5_kernels.cu): operands stored as shared-memory tile images (database format 2)
 size_t tc5_query_bytes(const Tc5Geom& T);                 // 16 queries
 bool tc5_supported(const Tc5Geom& T);
-void launch_db_to_tc5(const Tc5Geom& T, const uint4* db0_slice, uint8_t* dbt, int slice, cudaStream_t s);
 void launch_query_to_tc5(const Tc5Geom& T, const uint4* q_dev, size_t q_stride, int nq, uint8_t* qt, cudaStream_t s);
 // out_zm as launch_multiply_imma; up to 16 queries per pass; one persistent CTA per SM
 // reorient_reg_ciphertexts (util.rs:323-355) fused with the re-tiling: expansion workspace v (ntt32 [query][slot][row][n][z]) ->
@@ -115,8 +105,15 @@ struct ItemWrite { uint32_t off, len, il, j; };
 // (recenter_mod, NTT, pack: loading.rs:278-299, 34-41) and placed at the item's cell of slice c.  One launch.
 void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
                         int bpc, uint64_t pt_modulus, cudaStream_t s);
-// ---- database export (export_kernels.cu), the inverse of the loaders: the local rows of slice `slice` at z in [z0, z0 + zc) ->
-// out u64 [zc][rows][dim0] (the reference layout [z][ii][j] restricted to this GPU's rows), words lo | hi << 32.  One launch.
+// the synthetic database: plaintext coefficient i of slice c of item = j * num_per_global + ii is
+// splitmix64(seed, ((c * items + item) * 2048 + i)) % p, converted and placed like raw bytes (server.rs:223-275 with a counter
+// PRNG).  Every local item of every slice, one launch.
+void launch_write_synthetic(const DevParams& P, const DbLayout& L, Shard sh, uint64_t seed, uint64_t pt_modulus, cudaStream_t s);
+// ---- database import and export (export_kernels.cu), slice `slice` at z in [z0, z0 + zc), words lo | hi << 32.  One launch each.
+// import: ref_chunk u64 [zc][num_per_global][dim0] (the reference layout [z][ii][j], all rows) -> the local rows
+// ii = il * sh.count + sh.index of the store, in its layout
+void launch_db_import(const DbLayout& L, Shard sh, int slice, const uint64_t* ref_chunk, int z0, int zc, cudaStream_t s);
+// export: the local rows -> out u64 [zc][rows][dim0] (the reference layout restricted to this GPU's rows)
 void launch_db_export(const DbLayout& L, int slice, int z0, int zc, uint64_t* out, cudaStream_t s);
 
 // ---- second dimension

@@ -1,11 +1,11 @@
 // First-dimension kernels: multiply_reg_by_database (lib/spiral-rs/src/server.rs:155-221) over an
-// HBM-resident database, the database loaders that produce its device layout, and DoublePIR's packed
+// HBM-resident database, the item writers that convert and place items in any of its layouts, and DoublePIR's packed
 // matvec (lib/doublepir/src/matrix/kernels.rs:14-178).  All of these are pure streams of the
 // database: 8 bytes read -> 4 (u32 x u32 -> u64) multiply-adds, so the design goal is coalesced
 // 16-byte loads, many of them in flight per SM, and no shared-memory or shuffle traffic at all.
 //
-// Device layout of one slice (re-tiled at upload; the C ABI accepts the reference layout
-// [z][ii][j], server.rs:263-266):
+// Device layout of one slice (format 0, built from the reference layout at upload, export_kernels.cu; the C ABI accepts
+// the reference layout [z][ii][j], server.rs:263-266):
 //     db_dev[ii][jp][z] = uint4{ w(j=2jp).lo, w(2jp).hi, w(2jp+1).lo, w(2jp+1).hi }      (lo = mod q0, hi = mod q1)
 // so thread z of a warp reads 16 contiguous bytes and the warp 512 contiguous bytes.  The NTT
 // coordinate z is the one fully independent axis of the product, so it is the thread axis: each
@@ -139,22 +139,6 @@ __global__ void k_query_to_dev(MulGeom G, uint4* q_dev, const uint64_t* v) {
       make_uint4((uint32_t)a0, (uint32_t)(a0 >> 32), (uint32_t)a1, (uint32_t)(a1 >> 32));
 }
 
-// ref: u64 [zc][num_per_global][dim0] for z in [z0, z0+zc)  ->  db_dev slice [il][jp][z], ii = il*count + index
-__global__ void k_db_retile(MulGeom G, Shard sh, uint4* db_slice, const uint64_t* ref, int z0, int zc) {
-  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;     // over num_per * half * zc, z fastest
-  const int half = G.dim0 >> 1;
-  size_t total = (size_t)G.num_per * half * zc;
-  if (idx >= total) return;
-  int zl = (int)(idx % zc);
-  size_t rest = idx / zc;
-  int jp = (int)(rest % half), ii = (int)(rest / half);
-  const size_t ii_global = (size_t)ii * sh.count + sh.index;
-  const uint64_t* src = ref + ((size_t)zl * G.num_per * sh.count + ii_global) * G.dim0 + 2 * jp;
-  uint64_t w0 = src[0], w1 = src[1];
-  db_slice[((size_t)ii * half + jp) * POLY + z0 + zl] =
-      make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
-}
-
 __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index) {
   uint64_t z = seed + (index + 1) * 0x9E3779B97F4A7C15ULL;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
@@ -162,71 +146,59 @@ __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index)
   return z ^ (z >> 31);
 }
 
-// CTA (512 threads) = one (slice, ii, jp) cell pair: builds the two items j = 2jp, 2jp+1 from their
-// plaintext (server.rs:245-270: uniform mod p, recenter_mod, NTT, pack) and writes 2048 uint4.
-__global__ void __launch_bounds__(512, 1)
-k_db_synth(DevParams P, MulGeom G, Shard sh, uint4* db, uint64_t seed, uint64_t pt, int slice_begin) {
-  extern __shared__ __align__(16) uint32_t synth_smem[];
-  uint32_t* ntt_smem = synth_smem;                       // 2 * NTT_SMEM_WORDS
-  uint32_t* cell = synth_smem + 2 * NTT_SMEM_WORDS;      // POLY * 4
-  const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
-  const int half = G.dim0 >> 1;
-  const int jp = blockIdx.x % half;
-  const int ii = (blockIdx.x / half) % G.num_per;                 // local row
-  const int slice = slice_begin + blockIdx.x / (half * G.num_per);
-  const uint32_t q = n ? P.q[1] : P.q[0];
-  const uint64_t num_per_global = (uint64_t)G.num_per * sh.count;
-  const uint64_t num_items = (uint64_t)G.dim0 * num_per_global;
-  struct S { __device__ __forceinline__ void operator()() const { __syncthreads(); } };
-#pragma unroll 1
-  for (int jb = 0; jb < 2; jb++) {
-    const uint64_t item = (uint64_t)(2 * jp + jb) * num_per_global + ((uint64_t)ii * sh.count + sh.index);
-    const uint64_t base = ((uint64_t)slice * num_items + item) * POLY;
-    uint32_t x[8];
-#pragma unroll
-    for (int a = 0; a < 8; a++) {
-      uint64_t v = splitmix64_at(seed, base + a * 256 + tid) % pt;
-      x[a] = (v > pt / 2) ? (uint32_t)(q - (uint32_t)(pt - v)) : (uint32_t)v;     // recenter_mod, then mod q_n
-    }
-    ntt_forward_group_lz<NTT_OUT_CANON>(tid, x, ntt_smem + n * NTT_SMEM_WORDS, TwConstM{n, 0}, TwGlobalM{n ? P.fwd[1] : P.fwd[0]}, q, S());   // inputs canonical
-#pragma unroll
-    for (int k = 0; k < 8; k++) cell[(tid * 8 + k) * 4 + jb * 2 + n] = x[k];
+// Plaintext sources of k_write_items: item(b) is the item CTA column b writes (its local row il and column j), coef(it, c, i, pt)
+// coefficient i < 2048 of its chunk c, a value below pt.
+// Raw bytes (lib/server/src/db/loading.rs:317-359 update_item_raw): item b of `items`; chunk c is the bpc bytes at
+// item.off + c * bpc of `bytes`, zero past item.len (the zero padding of update_item_raw), coefficient i = byte i.
+struct ItemBytes {
+  const uint8_t* bytes; const ItemWrite* items; int bpc;
+  struct Item { int il, j; const uint8_t* src; uint32_t len; };
+  __device__ Item item(unsigned b) const { const ItemWrite it = items[b]; return Item{(int)it.il, (int)it.j, bytes + it.off, it.len}; }
+  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t) const {
+    const int begin = c * bpc;
+    return (i < bpc && (uint32_t)(begin + i) < it.len) ? (uint64_t)it.src[begin + i] : 0;
   }
-  __syncthreads();
-  uint4* dst = db + (((size_t)slice * G.num_per + ii) * half + jp) * POLY;
-  const uint4* c4 = reinterpret_cast<const uint4*>(cell);
-  for (int z = threadIdx.x; z < POLY; z += 512) dst[z] = c4[z];
-}
+};
+// The synthetic database (server.rs:223-275 with a counter PRNG): item b is (il, j) = (b / dim0, b % dim0) of this GPU's rows;
+// coefficient i of slice c is splitmix64_at(seed, (c * num_items + item) * 2048 + i) % pt, item = j * num_per_global + ii.
+struct ItemSynthetic {
+  MulGeom G; Shard sh; uint64_t seed;
+  struct Item { int il, j; uint64_t item; };
+  __device__ Item item(unsigned b) const {
+    const int il = (int)(b / G.dim0), j = (int)(b % G.dim0);
+    return Item{il, j, (uint64_t)j * G.num_per * sh.count + (uint64_t)il * sh.count + sh.index};
+  }
+  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t pt) const {
+    const uint64_t num_items = (uint64_t)G.dim0 * G.num_per * sh.count;
+    return splitmix64_at(seed, ((uint64_t)c * num_items + it.item) * POLY + i) % pt;
+  }
+};
 
-// lib/server/src/db/loading.rs:317-359 update_item_raw for many items at once, conversion and placement fused.  CTA = (item,
-// chunk c): chunk c of the item is the bpc bytes at item.off + c * bpc of `bytes`, zero past item.len (the zero padding of
-// update_item_raw); coefficient i = byte i, recenter_mod, forward NTT mod both q_n (convert_pt_to_poly :278-299), and the
-// two residues go straight to the item's place in the database of slice c.  512 threads: one 256-thread group per modulus;
-// 2 CTAs per SM (64 registers, no spills on sm_90a).
+// Many items at once, conversion and placement fused.  CTA = (item, chunk c): the chunk's coefficients from the source,
+// recenter_mod, forward NTT mod both q_n (loading.rs:278-299 convert_pt_to_poly), and the two residues go straight to the
+// item's place in the database of slice c.  512 threads: one 256-thread group per modulus; 2 CTAs per SM (64 registers, no
+// spills on sm_90a).
+template <typename Src>
 __global__ void __launch_bounds__(512, 2)
-k_write_items(DevParams P, DbLayout L, const uint8_t* __restrict__ bytes, const ItemWrite* __restrict__ items, int bpc, uint64_t pt) {
+k_write_items(DevParams P, DbLayout L, Src src, uint64_t pt) {
   __shared__ __align__(16) uint32_t ntt_smem[2 * NTT_SMEM_WORDS];
   __shared__ uint32_t halves[2][POLY];
   const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
   const int slice = blockIdx.y;
   const uint32_t q = n ? P.q[1] : P.q[0];
-  const ItemWrite it = items[blockIdx.x];
-  const uint8_t* src = bytes + it.off;
-  const int begin = slice * bpc;
+  const typename Src::Item it = src.item(blockIdx.x);
   struct S { __device__ __forceinline__ void operator()() const { __syncthreads(); } };
   uint32_t x[8];
 #pragma unroll
   for (int a = 0; a < 8; a++) {
-    const int i = a * 256 + tid;
-    const uint64_t v = (i < bpc && (uint32_t)(begin + i) < it.len) ? (uint64_t)src[begin + i] : 0;
+    const uint64_t v = src.coef(it, slice, a * 256 + tid, pt);
     x[a] = (v > pt / 2) ? (uint32_t)(q - (uint32_t)(pt - v)) : (uint32_t)v;       // recenter_mod, then mod q_n
   }
   ntt_forward_group_lz<NTT_OUT_CANON>(tid, x, ntt_smem + n * NTT_SMEM_WORDS, TwConstM{n, 0}, TwGlobalM{n ? P.fwd[1] : P.fwd[0]}, q, S());   // inputs canonical
 #pragma unroll
   for (int k = 0; k < 8; k++) halves[n][tid * 8 + k] = x[k];
   __syncthreads();
-  const int il = (int)it.il, j = (int)it.j;
-  for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, il, j, z, halves[0][z], halves[1][z]);
+  for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, it.il, it.j, z, halves[0][z], halves[1][z]);
 }
 
 // one item polynomial (2048 packed words lo|hi<<32) into the database, in any layout
@@ -452,12 +424,6 @@ void launch_query_to_dev(const MulGeom& G, uint4* q_dev, const uint64_t* v_first
   ++g_kernel_launches;
   k_query_to_dev<<<grid1d(total, 256), 256, 0, s>>>(G, q_dev, v_firstdim);
 }
-void launch_db_retile_chunk(const MulGeom& G, Shard sh, uint4* db_dev_slice, const uint64_t* ref_chunk, int z0, int zc,
-                            cudaStream_t s) {
-  size_t total = (size_t)G.num_per * (G.dim0 >> 1) * zc;
-  ++g_kernel_launches;
-  k_db_retile<<<grid1d(total, 256), 256, 0, s>>>(G, sh, db_dev_slice, ref_chunk, z0, zc);
-}
 void launch_db_upsert(const DbLayout& L, int slice, int il, int j, const uint64_t* poly, cudaStream_t s) {
   ++g_kernel_launches;
   k_db_upsert<<<POLY / 256, 256, 0, s>>>(L, slice, il, j, poly);
@@ -467,17 +433,14 @@ void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* by
   if (count == 0) return;
   if (chunks > 65535) throw Error(-2, "write_items: more than 65535 slices");
   ++g_kernel_launches;
-  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, bytes, items, bpc, pt_modulus);
+  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, ItemBytes{bytes, items, bpc}, pt_modulus);
 }
-void launch_db_synth(const DevParams& P, const MulGeom& G, Shard sh, uint4* db_dev, uint64_t seed, uint64_t pt_modulus,
-                     int slice_begin, int slice_count, cudaStream_t s) {
-  size_t ctas = (size_t)slice_count * G.num_per * (G.dim0 >> 1);
-  if (ctas == 0) return;
-  if (ctas > 0x7fffffffULL) throw Error(-2, "db_synth: grid too large");
-  const size_t smem = (size_t)(2 * NTT_SMEM_WORDS + 4 * POLY) * 4;
-  opt_in_smem(k_db_synth, (int)smem);
+void launch_write_synthetic(const DevParams& P, const DbLayout& L, Shard sh, uint64_t seed, uint64_t pt_modulus, cudaStream_t s) {
+  const size_t count = (size_t)L.G.num_per * L.G.dim0;
+  if (count == 0) return;
+  if (count > 0x7fffffffULL || L.G.slices > 65535) throw Error(-2, "write_synthetic: grid too large");
   ++g_kernel_launches;
-  k_db_synth<<<(unsigned)ctas, 512, smem, s>>>(P, G, sh, db_dev, seed, pt_modulus, slice_begin);
+  k_write_items<<<dim3((unsigned)count, (unsigned)L.G.slices), 512, 0, s>>>(P, L, ItemSynthetic{L.G, sh, seed}, pt_modulus);
 }
 void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t rows, size_t cols, int variant,
                         cudaStream_t s) {

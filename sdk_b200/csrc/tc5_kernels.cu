@@ -39,24 +39,6 @@ constexpr int TC5_THREADS = 2 * 128 + 32;              // two consumer warpgroup
 using namespace tc5;
 
 // ---- operand images ---------------------------------------------------------------------------------------------------
-// format 0 slice (uint4 [row][jp][z]) -> tile images.  CTA = (z, mt, ks); thread = (row_local, group of 4 values of j).
-__global__ void __launch_bounds__(256)
-k_db_to_tc5(Tc5Geom T, const uint4* __restrict__ db0_slice, uint8_t* __restrict__ dbt, int slice) {
-  const int z = blockIdx.x, mt = blockIdx.y, ks = blockIdx.z;
-  const Tc5DbThread t = tc5_db_thread(threadIdx.x, mt, ks);
-  const int half = T.dim0 >> 1;
-  uint32_t res[2][4];
-#pragma unroll
-  for (int p = 0; p < 2; p++) {
-    const int jp = t.jp0 + p;
-    uint4 w = make_uint4(0, 0, 0, 0);
-    if (t.ii < T.rows && jp < half) w = db0_slice[((size_t)t.ii * half + jp) * POLY + z];
-    res[0][2 * p] = w.x; res[1][2 * p] = w.y; res[0][2 * p + 1] = w.z; res[1][2 * p + 1] = w.w;
-  }
-#pragma unroll
-  for (int n = 0; n < 2; n++) tc5_db_store(dbt + tc5_db_tile(T, slice, n, z, mt, ks) * TC5_TILE, t, res[n]);
-}
-
 // expanded queries (uint4 [j][z] per query, q_stride apart) -> qT.  CTA = (pair of z, ks): every 32-byte sector it reads is
 // fully used; the four 4 KiB tiles (2 z x 2 n) are assembled in shared memory and written out contiguously.
 __global__ void __launch_bounds__(256)
@@ -273,10 +255,6 @@ static size_t tc5_smem_bytes(const Tc5Geom& T, int ksps, int bbufs) {
 // at least two ring stages beside a single-buffered query operand
 bool tc5_supported(const Tc5Geom& T) { return T.dim0 % 2 == 0 && tc5_ring_stages(T.ks, 4, 1) >= 2; }
 
-void launch_db_to_tc5(const Tc5Geom& T, const uint4* db0_slice, uint8_t* dbt, int slice, cudaStream_t s) {
-  ++g_kernel_launches;
-  k_db_to_tc5<<<dim3(POLY, T.mt, T.ks), 256, 0, s>>>(T, db0_slice, dbt, slice);
-}
 void launch_query_to_tc5(const Tc5Geom& T, const uint4* q_dev, size_t q_stride, int nq, uint8_t* qt, cudaStream_t s) {
   if (nq < 1 || nq > 16) throw Error(-2, "wgmma multiply: 1..16 queries per pass");
   ++g_kernel_launches;

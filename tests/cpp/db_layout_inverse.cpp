@@ -1,6 +1,6 @@
 // The item maps of sdk_b200/csrc/item_place.cuh, on the CPU: for every geometry, every (il, j) and several z,
 //   - db_bytes is each layout's store size in bytes, as restated here, and slice_bytes is its share of one slice;
-//   - every byte an item is placed at, and every byte the bulk slice writers address, lies inside db_bytes;
+//   - every byte an item is placed at, and every byte the slice import kernels address, lies inside db_bytes;
 //   - the bytes different items (and moduli, limbs, z) occupy never overlap, in all three layouts;
 //   - fetch_item(place_item(w)) == w for canonical residues, including the all-(q - 1) words, and an unwritten cell fetches as 0;
 //   - the four limb-l bytes of j = 4 kq .. 4 kq + 3 are one 4-byte word at frag_word / tc5_word (what the export kernels read),
@@ -53,21 +53,18 @@ static void check_geometry(int dim0, int rows) {
       CHECK(slice_bytes(L[f]) * slices == want[f], "format %d: slice_bytes (dim0 %d rows %d)", f, dim0, rows);
     }
   }
-  // ---- the bulk writers stay inside the store: the format-0 slice builders (k_db_retile, k_db_synth) write the cells of
-  // imad_cell, ending at slices * slice_bytes; the re-tilers write slice s of formats 1 (k_db_to_frag's address, restated) and 2
-  // (tc5_db_tile) within [s, s + 1) * slice_bytes
-  CHECK((imad_cell(G, slices - 1, rows - 1, dim0 - 1, POLY - 1) + 1) * 16 <= slices * slice_bytes(L[0]) &&
-        slices * slice_bytes(L[0]) <= db_bytes(L[0], slices), "format 0 slice builders past the store (dim0 %d rows %d)", dim0, rows);
+  // ---- the bulk writers stay inside the store: the import kernels write slice s of format 0 at imad_cell (k_db_import_imad),
+  // of format 1 in whole groups at frag_db_group (k_db_import_frag) and of format 2 in whole tiles at tc5_db_tile
+  // (k_db_import_tc5), within [s, s + 1) * slice_bytes
   for (int s = 0; s < slices; s++) {
-    auto frag_cell = [&](int n, int z, int mt, int ks, int l, int lane) {
-      return (((((size_t)s * 2 + n) * POLY + z) * F.mt + mt) * F.ks + ks) * 4 * 32 + (size_t)l * 32 + lane;
-    };
-    const size_t lo[2] = {frag_cell(0, 0, 0, 0, 0, 0) * 16, tc5_db_tile(T, s, 0, 0, 0, 0) * TC5_TILE};
-    const size_t end[2] = {(frag_cell(1, POLY - 1, F.mt - 1, F.ks - 1, 3, 31) + 1) * 16,
+    const size_t lo[3] = {imad_cell(G, s, 0, 0, 0) * 16, frag_db_group(F, s, 0, 0, 0, 0) * FRAG_GROUP,
+                          tc5_db_tile(T, s, 0, 0, 0, 0) * TC5_TILE};
+    const size_t end[3] = {(imad_cell(G, s, rows - 1, dim0 - 1, POLY - 1) + 1) * 16,
+                           (frag_db_group(F, s, 1, POLY - 1, F.mt - 1, F.ks - 1) + 1) * FRAG_GROUP,
                            (tc5_db_tile(T, s, 1, POLY - 1, T.mt - 1, T.ks - 1) + 1) * TC5_TILE};
-    for (int f = 1; f < 3; f++)
-      CHECK(lo[f - 1] == s * slice_bytes(L[f]) && end[f - 1] <= (s + 1) * slice_bytes(L[f]) &&
-            (s + 1) * slice_bytes(L[f]) <= db_bytes(L[f], slices), "format %d re-tiler of slice %d past its slice (dim0 %d rows %d)",
+    for (int f = 0; f < 3; f++)
+      CHECK(lo[f] == s * slice_bytes(L[f]) && end[f] <= (s + 1) * slice_bytes(L[f]) &&
+            (s + 1) * slice_bytes(L[f]) <= db_bytes(L[f], slices), "format %d import of slice %d past its slice (dim0 %d rows %d)",
             f, s, dim0, rows);
   }
   if (failures) return;      // the stores below are db_bytes long: a wrong size would be written out of bounds

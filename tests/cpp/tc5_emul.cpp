@@ -34,7 +34,7 @@ int main() {
       std::vector<uint32_t> a((size_t)rows * dim0), b((size_t)nq * 2 * dim0);
       for (auto& x : a) x = trial == 1 ? q - 1 : (uint32_t)(rng() % q);
       for (auto& x : b) x = trial == 1 ? q - 1 : (uint32_t)(rng() % q);
-      // ---- database image: CTA (mt, ks), 256 threads each (k_db_to_tc5); the other modulus' tile is not needed here
+      // ---- database image: CTA (mt, ks), 256 threads each (k_db_import_tc5); the other modulus' tile is not needed here
       std::vector<uint8_t> dbt((size_t)T.mt * T.ks * TC5_TILE, 0xEE);
       for (int mt = 0; mt < T.mt; mt++)
         for (int ks = 0; ks < T.ks; ks++)

@@ -174,9 +174,8 @@ class _Flow:
             self.close()
             pytest.skip("S256's workspace does not fit: %.1f GiB free of %.1f GiB (%s)" % (self.free_at_start / GIB, total / GIB, e))
         self.free_beside_workspace = torch.cuda.mem_get_info()[0]
-        # Beside it: a shard, and either the one-slice scratch b200pir_db_fill_synthetic builds each slice of a format-1 or 2
-        # store in, or the 8 images (shard() releases them while it fills); 1 GiB for the stages' temporaries.
-        need = _shard_bytes(P) + max(_shard_bytes(P) // P.slices, WORLD * self.img_bytes) + GIB
+        # Beside it: a shard, the 8 images and 1 GiB for the stages' temporaries.
+        need = _shard_bytes(P) + WORLD * self.img_bytes + GIB
         if self.free_beside_workspace < need:
             self.close()
             pytest.skip("S256's shard needs %.1f GiB beside the workspace (%.1f GiB); %.1f GiB are left of %.1f GiB"
@@ -214,9 +213,7 @@ class _Flow:
         self.torch.cuda.empty_cache()           # back to the device, where the library allocates
 
     def shard(self, s, fmt=2):
-        """Shard s, filled.  The images are released first (and re-expanded, identically, on their next use), so that the
-        fill's scratch does not have to fit beside them."""
-        self.release_images()
+        """Shard s, filled."""
         db = self.S.Database(self.G, shard_index=s, shard_count=WORLD, fmt=fmt)
         db.fill_synthetic(SEED)
         return db
@@ -399,8 +396,6 @@ def test_fragment_and_imad_layouts_at_32_gib(flow):
     qexp_words = DIM0 * P.N * 4
     qexp = vf = None
     for fmt in (1, 0):
-        # the shard is filled before the expanded queries are allocated: the fill's one-slice scratch (formats 1 and 2) and
-        # the 4 GiB of expanded queries are never held together
         db = flow.shard(WORLD - 1, fmt=fmt)
         try:
             if qexp is None:
