@@ -55,11 +55,11 @@ void b200pir_ctx_destroy(b200pir_ctx* ctx);
  * are ordered after whatever the caller queued there before the call. */
 int b200pir_ctx_set_stream(b200pir_ctx* ctx, void* cuda_stream);
 int b200pir_ctx_synchronize(b200pir_ctx* ctx);
-/* knobs: "mul_variant" (kernel tiling), "batch" (max queries per database pass: 1, 2, 4, 8 or 16;
+/* knobs: "batch" (max queries per database pass: 1, 2, 4, 8 or 16;
  * the IMAD layout uses at most 4), "db_format" (layout of databases created afterwards: -1 = automatic (default): 2 wherever the
  * wgmma kernel supports the geometry, else 1; 0 = IMAD, 1 = mma.sync INT8 fragments, 2 = wgmma tile images, tc5_kernels.cu), "profile" (0 off, 1 per call,
- * 2 accumulate over calls until set again); "fold_variant", "intt_variant", "imma_variant", "expand_variant",
- * "expand_pair_min_ctas" (accepted, no effect: one kernel or schedule each remains); "coalesce" (1 = default: concurrent single-query callers
+ * 2 accumulate over calls until set again); "mul_variant", "fold_variant", "intt_variant", "imma_variant", "expand_variant",
+ * "expand_pair_min_ctas" (accepted, no effect: one kernel, tiling or schedule each remains); "coalesce" (1 = default: concurrent single-query callers
  * share database passes, see b200pir_coalesce_stats), "coalesce_window_us" (default 200: how long a batch that directly
  * follows a multi-query batch is held open for the callers of that batch to return; 0 = never), "sparse_fold" (1 = fold like lib/server's sparse server,
  * compute/fold.rs:15-65: an all-zero ciphertext short-cuts the external product; 0 = spiral-rs's dense fold, default; version-1
@@ -304,6 +304,7 @@ void b200pir_dpir_destroy(b200pir_dpir* m);
 int b200pir_dpir_set_stream(b200pir_dpir* m, void* cuda_stream);
 /* b: 3*cols u32 ; out: rows u32 */
 int b200pir_dpir_matvec_packed(b200pir_dpir* m, const uint32_t* b, uint32_t* out);
+/* _dev: device pointers, on the handle's stream.  `variant` is accepted and has no effect: one kernel per shape remains. */
 int b200pir_dpir_matvec_packed_dev(b200pir_dpir* m, const uint32_t* b_dev, uint32_t* out_dev, int variant);
 /* same over the row range [row_begin, row_begin+row_count): answer()'s `db.rows(start, batch)` (doublepir.rs:301) */
 int b200pir_dpir_matvec_packed_rows(b200pir_dpir* m, uint64_t row_begin, uint64_t row_count, const uint32_t* b, uint32_t* out);

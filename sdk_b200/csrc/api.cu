@@ -82,7 +82,7 @@ struct b200pir_ctx {
   DevBuf<Twiddle> d_tw4k;    // fwd0, inv0, fwd1, inv1 for poly_len 4096 (config #5 sweep)
   DevBuf<uint32_t> d_neg1;   // [11][2][2048] ntt32 (params.rs:98-107)
   // options
-  int mul_variant = 0, max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
+  int max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
   int sparse_fold = 0;           // 1: lib/server's fold (all-zero ciphertext shortcut, compute/fold.rs:37-43); 0: spiral-rs dense fold
   int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the wgmma kernel
                                  // supports the geometry, else 1), 0 = IMAD layout, 1 = mma.sync fragments, 2 = wgmma tile images
@@ -460,7 +460,7 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
       if (count - qi >= 4 && c->max_group >= 4) nq = 4;
       else if (count - qi >= 2 && c->max_group >= 2) nq = 2;
       launch_multiply(c->dp, L.G, reinterpret_cast<const uint4*>(L.base), qdev + qi * q_stride, out + qi * out_stride,
-                      slice_begin, slice_count, nq, q_stride, out_stride, c->mul_variant, c->stream);
+                      slice_begin, slice_count, nq, q_stride, out_stride, c->stream);
       c->mul_launches++;
       qi += nq;
     }
@@ -651,8 +651,6 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   for (int i = 0; i < 64; i++) { lo[(0 * 3 + 0) * 64 + i] = f0[i]; lo[(0 * 3 + 1) * 64 + i] = i0[i]; lo[(0 * 3 + 2) * 64 + i] = l0[i];
                                  lo[(1 * 3 + 0) * 64 + i] = f1[i]; lo[(1 * 3 + 1) * 64 + i] = i1[i]; lo[(1 * 3 + 2) * 64 + i] = l1[i]; }
   upload_poly_constants(lo.data(), c->stream);
-  upload_mul_constants(lo.data(), c->stream);
-  upload_imma_constants(lo.data(), c->stream);
   // poly_len = 4096 (config #5): built here rather than on the first b200pir_ntt4096_dev call, so that call neither allocates
   // nor copies from the host
   std::vector<Twiddle> tw4k;
@@ -736,10 +734,9 @@ int b200pir_ctx_set_option(b200pir_ctx* c, const char* key, int64_t value) {
   if (!c || !key) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   std::string k(key);
-  if (k == "mul_variant") c->mul_variant = (int)value;
-  else if (k == "batch") { if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) throw Error(B200PIR_E_BADARG, "batch must be 1, 2, 4, 8 or 16"); c->max_group = (int)value; }
+  if (k == "batch") { if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) throw Error(B200PIR_E_BADARG, "batch must be 1, 2, 4, 8 or 16"); c->max_group = (int)value; }
   // one kernel each now; the keys stay accepted so existing callers keep working
-  else if (k == "fold_variant" || k == "intt_variant" || k == "imma_variant" || k == "expand_variant" ||
+  else if (k == "mul_variant" || k == "fold_variant" || k == "intt_variant" || k == "imma_variant" || k == "expand_variant" ||
            k == "expand_pair_min_ctas") {}
   else if (k == "sparse_fold") c->sparse_fold = value != 0;
   else if (k == "coalesce") c->coalesce = value != 0;

@@ -73,6 +73,17 @@ __device__ __forceinline__ uint4 ld_stream_v4(const uint4* p) {
   return r;
 }
 
+// Value `index` of the counter-based splitmix64 stream of `seed`: the synthetic Spiral database and the synthetic DoublePIR matrix
+__device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index) {
+  uint64_t z = seed + (index + 1) * 0x9E3779B97F4A7C15ULL;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+
+// blocks of `block` threads that cover `total` threads
+inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + block - 1) / block); }
+
 // ---- host-side error plumbing
 struct Error : std::runtime_error {
   int code;

@@ -52,11 +52,7 @@ struct OwnedStream {
 __global__ void k_dpir_synth(uint32_t* a, size_t words, uint64_t seed, size_t index0) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= words) return;
-  uint64_t z = seed + (index0 + i + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  z ^= z >> 31;
-  a[i] = (uint32_t)z & 0x3FFFFFFFu;
+  a[i] = (uint32_t)splitmix64_at(seed, index0 + i) & 0x3FFFFFFFu;
 }
 b200pir_dpir* dpir_new(int device, uint64_t rows, uint64_t cols) {
   use_device(device);
@@ -185,12 +181,12 @@ int b200pir_dpir_set_stream(b200pir_dpir* m, void* cuda_stream) {
   m->own_stream = false;
   API_END
 }
-int b200pir_dpir_matvec_packed_dev(b200pir_dpir* m, const uint32_t* b_dev, uint32_t* out_dev, int variant) {
+int b200pir_dpir_matvec_packed_dev(b200pir_dpir* m, const uint32_t* b_dev, uint32_t* out_dev, int /* variant: selects nothing */) {
   API_BEGIN
   if (!m || !b_dev || !out_dev) throw Error(B200PIR_E_BADARG, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   cudaSetDevice(m->device);
-  launch_dpir_matvec(out_dev, m->a.p, b_dev, m->rows, m->cols, variant, m->stream);
+  launch_dpir_matvec(out_dev, m->a.p, b_dev, m->rows, m->cols, m->stream);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -203,7 +199,7 @@ int b200pir_dpir_matvec_packed_rows(b200pir_dpir* m, uint64_t row_begin, uint64_
   std::lock_guard<std::mutex> lk(m->mu);
   cudaSetDevice(m->device);
   B200_CUDA(cudaMemcpyAsync(m->b.p, b, 3 * m->cols * 4, cudaMemcpyHostToDevice, m->stream));
-  launch_dpir_matvec(m->out.p, m->a.p + row_begin * m->cols, m->b.p, row_count, m->cols, 0, m->stream);
+  launch_dpir_matvec(m->out.p, m->a.p + row_begin * m->cols, m->b.p, row_count, m->cols, m->stream);
   B200_CUDA(cudaMemcpyAsync(out, m->out.p, row_count * 4, cudaMemcpyDeviceToHost, m->stream));
   B200_CUDA(cudaStreamSynchronize(m->stream));
   B200_CUDA(cudaGetLastError());

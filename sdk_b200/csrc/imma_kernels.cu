@@ -1,4 +1,6 @@
-// First dimension on the INT8 tensor-core path (batched queries).
+// First dimension on the INT8 tensor-core path (batched queries, database format 1): the query operand in fragment order
+// (k_query_to_frag), the mma.sync products and the z-major product's stage-level read-out (k_zmajor_to_ntt32).  The inverse
+// transform of the z-major product, which formats 1 and 2 share, is k_intt_from_zmajor_tiled in poly_kernels.cu.
 //
 // multiply_reg_by_database (lib/spiral-rs/src/server.rs:155-221) is, for every NTT coordinate z and CRT
 // modulus n, a small integer GEMM  C[ii][(query,row)] = sum_j A[ii][j] * B[j][(query,row)]  mod q_n  with
@@ -275,93 +277,6 @@ k_multiply_imma8(DevParams P, ImmaGeom F, const uint4* __restrict__ dbf, const u
   cp_async_wait<0>();
 }
 
-__constant__ Twiddle c_tw_lo_imma[2][3][64];
-struct TwConstI {
-  int n, dir;
-  __device__ __forceinline__ Twiddle operator()(int i) const { return c_tw_lo_imma[n][dir][i]; }
-  __device__ __forceinline__ void load2(int i, Twiddle (&t)[2]) const { t[0] = (*this)(i); t[1] = (*this)(i + 1); }
-  __device__ __forceinline__ void load4(int i, Twiddle (&t)[4]) const {
-    t[0] = (*this)(i); t[1] = (*this)(i + 1); t[2] = (*this)(i + 2); t[3] = (*this)(i + 3);
-  }
-};
-struct TwGlobalI {
-  const Twiddle* p;
-  __device__ __forceinline__ Twiddle operator()(int i) const {
-    uint2 v = __ldg(reinterpret_cast<const uint2*>(p + i));
-    return Twiddle{v.x, v.y};
-  }
-  __device__ __forceinline__ void load2(int i, Twiddle (&t)[2]) const {
-    uint4 v = __ldg(reinterpret_cast<const uint4*>(p + i));
-    t[0] = Twiddle{v.x, v.y}; t[1] = Twiddle{v.z, v.w};
-  }
-  __device__ __forceinline__ void load4(int i, Twiddle (&t)[4]) const {
-    uint4 v = __ldg(reinterpret_cast<const uint4*>(p + i)), w = __ldg(reinterpret_cast<const uint4*>(p + i) + 1);
-    t[0] = Twiddle{v.x, v.y}; t[1] = Twiddle{v.z, v.w}; t[2] = Twiddle{w.x, w.y}; t[3] = Twiddle{w.z, w.w};
-  }
-};
-struct SyncI {
-  __device__ __forceinline__ void operator()() const { __syncthreads(); }
-};
-
-// inverse NTT of every (ciphertext row, modulus) of the z-major product -> residue-form ciphertexts
-//   out[((query*slices + slice)*rows + ii)][ct_row][n][z]     (server.rs:707-709 without the CRT lift)
-// One CTA handles PP (= 2, 4 or 8) polynomials that are adjacent in the z-major product, so every 32-byte sector it fetches
-// is fully used (one CTA per polynomial would use 4 of every 32 bytes: its z-stride is rows*2 words).  The PP polynomials
-// are transposed through shared memory, then inverse-transformed two at a time.  rows*2 is even, so PP = 2 always fits.
-// grid = (rows*2 / PP, 2 moduli, nq*slices), 256 threads, dynamic smem = PP*2048*4 + 2*NTT_SMEM_WORDS*4
-template <int PP>
-__global__ void __launch_bounds__(256)
-k_intt_from_zmajor_tiled(DevParams P, ImmaGeom F, const uint32_t* __restrict__ in_zm, size_t in_stride,
-                         uint32_t* __restrict__ out, int slices) {
-  extern __shared__ __align__(16) uint32_t tsm[];
-  uint32_t* polybuf = tsm;                               // [PP][2048]
-  uint32_t* sm0 = tsm + PP * POLY;
-  uint32_t* sm1 = sm0 + NTT_SMEM_WORDS;
-  const int tid = threadIdx.x, n = blockIdx.y;
-  const int p0 = blockIdx.x * PP;                        // index into the flattened [row][ct_row] axis
-  const int qs = blockIdx.z, qi = qs / slices, slice = qs % slices;
-  const uint32_t q = n ? P.q[1] : P.q[0];
-  const size_t zstride = (size_t)F.rows * 2;
-  const uint32_t* src = in_zm + (size_t)qi * in_stride + (((size_t)slice * 2 + n) * POLY) * zstride + p0;
-  for (int z = tid; z < POLY; z += 256) {
-    uint32_t v[PP];
-    const uint32_t* s = src + (size_t)z * zstride;
-    if (PP == 8) {
-      uint4 a = __ldg(reinterpret_cast<const uint4*>(s)), b = __ldg(reinterpret_cast<const uint4*>(s) + 1);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4 % PP] = b.x; v[5 % PP] = b.y; v[6 % PP] = b.z; v[7 % PP] = b.w;
-    } else if (PP == 4) {
-      uint4 a = __ldg(reinterpret_cast<const uint4*>(s));
-      v[0] = a.x; v[1] = a.y; v[2 % PP] = a.z; v[3 % PP] = a.w;
-    } else {
-      uint2 a = __ldg(reinterpret_cast<const uint2*>(s));
-      v[0] = a.x; v[1] = a.y;
-    }
-#pragma unroll
-    for (int p = 0; p < PP; p++) polybuf[p * POLY + z] = v[p];
-  }
-  __syncthreads();
-  const TwConstI lo{n, 2};                               // relaxed-range inverse (ntt_core.cuh "lz"): inputs are canonical residues
-  const TwGlobalI hi{n ? P.inv_lz[1] : P.inv_lz[0]};
-#pragma unroll 1
-  for (int p = 0; p < PP; p += 2) {
-    uint32_t x0[8], x1[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      x0[k] = polybuf[p * POLY + tid * 8 + k];
-      x1[k] = polybuf[(p + 1) * POLY + tid * 8 + k];
-    }
-    ntt_inverse_group2_nh(tid, x0, x1, sm0, sm1, lo, hi, q, SyncI());
-    const int f0 = p0 + p, f1 = p0 + p + 1;               // flattened (row, ct_row)
-    uint32_t* d0 = out + ((((size_t)qs * F.rows + (f0 >> 1)) * 2 + (f0 & 1)) * 2 + n) * POLY;
-    uint32_t* d1 = out + ((((size_t)qs * F.rows + (f1 >> 1)) * 2 + (f1 & 1)) * 2 + n) * POLY;
-#pragma unroll
-    for (int a = 0; a < 8; a++) {
-      d0[a * 256 + tid] = x0[a];
-      d1[a * 256 + tid] = x1[a];
-    }
-  }
-}
-
 // z-major product -> the ABI's [ii][r][n][z] NTT-form layout (stage-level entry point only)
 __global__ void k_zmajor_to_ntt32(ImmaGeom F, const uint32_t* __restrict__ in_zm, uint32_t* __restrict__ out, int slice) {
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;      // over rows*4*2048, z fastest
@@ -372,13 +287,8 @@ __global__ void k_zmajor_to_ntt32(ImmaGeom F, const uint32_t* __restrict__ in_zm
   out[idx] = in_zm[((((size_t)slice * 2 + n) * POLY + z) * F.rows + ii) * 2 + r];
 }
 
-inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + block - 1) / block); }
-
 }  // namespace
 
-void upload_imma_constants(const Twiddle* lo, cudaStream_t s) {
-  B200_CUDA(cudaMemcpyToSymbolAsync(c_tw_lo_imma, lo, sizeof(Twiddle) * 2 * 3 * 64, 0, cudaMemcpyHostToDevice, s));
-}
 size_t imma_query_cells(const ImmaGeom& F) { return (size_t)2 * POLY * 4 * F.ks * 4 * 32; }   // up to 4 column tiles
 // 16 queries per pass need the B operand (4 tiles) plus the A rings in one CTA's shared memory
 bool imma_supports_16(const ImmaGeom& F) {
@@ -417,21 +327,6 @@ void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* db
     k_multiply_imma<1><<<dim3(POLY, 2), 256, smem, s>>>(P, F, dbf, qf, out_zm, out_stride, nq, slice_begin, slice_count);
   else
     k_multiply_imma<2><<<dim3(POLY, 2), 256, smem, s>>>(P, F, dbf, qf, out_zm, out_stride, nq, slice_begin, slice_count);
-}
-template <int PP>
-static void launch_intt_tiled(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
-                              int nq, int slices, cudaStream_t s) {
-  const size_t smem = (size_t)(PP * POLY + 2 * NTT_SMEM_WORDS) * 4;
-  opt_in_smem(k_intt_from_zmajor_tiled<PP>, (int)smem);
-  k_intt_from_zmajor_tiled<PP><<<dim3(F.rows * 2 / PP, 2, nq * slices), 256, smem, s>>>(P, F, in_zm, in_stride, out, slices);
-}
-void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
-                             int nq, int slices, cudaStream_t s) {
-  ++g_kernel_launches;
-  const int polys = F.rows * 2;
-  if (polys % 8 == 0) launch_intt_tiled<8>(P, F, in_zm, in_stride, out, nq, slices, s);
-  else if (polys % 4 == 0) launch_intt_tiled<4>(P, F, in_zm, in_stride, out, nq, slices, s);
-  else launch_intt_tiled<2>(P, F, in_zm, in_stride, out, nq, slices, s);
 }
 void launch_zmajor_to_ntt32(const ImmaGeom& F, const uint32_t* in_zm, uint32_t* out, int slice, cudaStream_t s) {
   size_t total = (size_t)F.rows * 4 * POLY;

@@ -1,7 +1,7 @@
 // Where one NTT coordinate z of one database item lives in each device layout, and how it is read back.  Item (slice, local
 // row il, column j) holds, at every z, the residue mod q0 (`lo`) and mod q1 (`hi`) of the packed word lo | hi << 32
-// (loading.rs:34-41 pack_ntt_poly).  The single-item upsert, the batched item writer (k_write_items: raw bytes or the
-// synthetic database) and the import and export kernels (export_kernels.cu) all address the database through these maps, so
+// (loading.rs:34-41 pack_ntt_poly).  The single-item upsert (mul_kernels.cu), the batched item writer (k_write_items in
+// poly_kernels.cu: raw bytes or the synthetic database) and the import and export kernels (export_kernels.cu) all address the database through these maps, so
 // every writer and reader agrees on the layouts; the host sizes the store with db_bytes.  The maps are __host__ __device__
 // and use no CUDA types: tests/cpp/db_layout_inverse.cpp checks on the CPU that place and fetch are mutually inverse, that no
 // two items share a byte and that every byte a writer touches lies inside db_bytes.

@@ -45,22 +45,20 @@ void launch_from_ntt(const DevParams& P, uint64_t* out_raw, const uint32_t* in, 
 // raw u64 coefficients <-> residue form u32 [poly][n][z] (coefficient domain; the CRT lift is poly.rs:658)
 void launch_raw_to_res(const DevParams& P, uint32_t* out, const uint64_t* raw, size_t polys, cudaStream_t s);
 void launch_res_to_raw(const DevParams& P, uint64_t* out, const uint32_t* res, size_t polys, cudaStream_t s);
-// twiddle entries 0..63 of every (modulus, direction) -> constant bank of the poly kernels' module
+// twiddle entries 0..63 of every (modulus, direction) -> the constant bank of poly_kernels.cu, the only module that runs the NTT
 // stream-ordered on s; `lo` must stay valid until s has reached the copy
 void upload_poly_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */, cudaStream_t s);
-void upload_mul_constants(const Twiddle* lo /* [2][3][64]: forward, inverse, relaxed-range inverse */, cudaStream_t s);
 // format converters for the C ABI (u64 [n][z] words < 2^32  <->  ntt32)
 void launch_widen(uint64_t* out, const uint32_t* in, size_t words, cudaStream_t s);
 void launch_narrow(uint32_t* out, const uint64_t* in, size_t words, cudaStream_t s);
 
-// ---- first dimension (K1): server.rs:155-221
+// ---- first dimension (K1) on the IMAD layout (mul_kernels.cu): server.rs:155-221
 // db_dev : uint4 [slice][ii][jp = j/2][z] = {w(2jp).lo, w(2jp).hi, w(2jp+1).lo, w(2jp+1).hi}
 // q_dev  : uint4 [jp][jb][z] = {a[j][r0].lo, a[j][r0].hi, a[j][r1].lo, a[j][r1].hi},  j = 2jp+jb
 // out    : ntt32 [slice][ii][r][n][z]
 // `nq` queries are processed per DB pass (q_dev / out strided by q_stride / out_stride uint4 / u32).
 void launch_multiply(const DevParams& P, const MulGeom& G, const uint4* db_dev, const uint4* q_dev, uint32_t* out,
-                     int slice_begin, int slice_count, int nq, size_t q_stride, size_t out_stride, int variant,
-                     cudaStream_t s);
+                     int slice_begin, int slice_count, int nq, size_t q_stride, size_t out_stride, cudaStream_t s);
 // reference layout v_firstdim u64 [z][j][r]  ->  q_dev
 void launch_query_to_dev(const MulGeom& G, uint4* q_dev, const uint64_t* v_firstdim, cudaStream_t s);
 // Row sharding of the second-dimension index: this GPU holds global rows ii = il*count + index
@@ -71,12 +69,12 @@ struct Shard { int index, count; };
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
 bool imma_supports_16(const ImmaGeom& F);                 // 16 queries per database pass fit one CTA's shared memory
 inline int imma_query_tiles(int nq) { return nq > 8 ? 4 : (nq > 4 ? 2 : 1); }   // column tiles of 4 queries
-void upload_imma_constants(const Twiddle* lo, cudaStream_t s);
 void launch_query_to_frag(const ImmaGeom& F, const uint4* q_dev, size_t q_stride, int nq, uint2* qf, cudaStream_t s);
 // out_zm: u32 [query][slice][n][z][row][ct_row]  (queries out_stride words apart)
 void launch_multiply_imma(const DevParams& P, const ImmaGeom& F, const uint4* dbf, const uint2* qf, uint32_t* out_zm,
                           size_t out_stride, int nq, int slice_begin, int slice_count, cudaStream_t s);
-// inverse NTT of the z-major product -> residue-form ciphertexts [query*slices + slice][row][ct_row][n][z]
+// inverse NTT of the z-major product of formats 1 and 2 -> residue-form ciphertexts [query*slices + slice][row][ct_row][n][z]
+// (poly_kernels.cu)
 void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
                              int nq, int slices, cudaStream_t s);
 // z-major product of one slice -> ntt32 [row][ct_row][n][z]
@@ -95,7 +93,8 @@ void launch_reorient_to_tc5(const Tc5Geom& T, const uint32_t* v, size_t v_stride
 void launch_multiply_tc5(const DevParams& P, const Tc5Geom& T, const uint8_t* dbt, const uint32_t* tile_mask, const uint8_t* qt,
                          uint32_t* out_zm, size_t out_stride, int nq, int slice_begin, int slice_count, int sm_count, cudaStream_t s);
 
-// ---- writes into a database, in any layout (DbLayout, item_place.cuh; mul_kernels.cu)
+// ---- writes into a database, in any layout (DbLayout, item_place.cuh): the upsert in mul_kernels.cu, the item writers in
+// poly_kernels.cu
 // one item poly (2048 packed words, lo|hi<<32) -> its place at (slice, local row il, column j)   (lib/server db/loading.rs:317-359)
 void launch_db_upsert(const DbLayout& L, int slice, int il, int j, const uint64_t* poly, cudaStream_t s);
 // raw item bytes -> database (loading.rs:317-359 update_item_raw, batched)
@@ -177,9 +176,9 @@ void launch_pack(const DevParams& P, uint64_t* out_raw, size_t out_q_stride, con
 void launch_encode(const DevParams& P, uint8_t* out, size_t out_bytes, const uint64_t* packed_raw, size_t packed_q_stride,
                    int nq, int n, int instances, uint64_t q2, int q2_bits, uint64_t q1, int q1_bits, cudaStream_t s);
 
-// ---- DoublePIR packed matvec (K6): lib/doublepir/src/matrix/kernels.rs:14-178
-void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t rows, size_t cols, int variant,
-                        cudaStream_t s);
+// ---- DoublePIR packed matvec (K6, mul_kernels.cu): lib/doublepir/src/matrix/kernels.rs:14-178
+// even cols: k_dpir_matvec_row, odd cols: k_dpir_matvec, rows too wide for `b` in shared memory: k_dpir_matvec_wide
+void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t rows, size_t cols, cudaStream_t s);
 
 // lib/doublepir/src/matrix/kernels.rs:180-278 and matrix/indexing.rs:117-143 (the small tail of answer())
 void launch_dpir_mul_transposed(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t a_rows, size_t a_cols,

@@ -1,8 +1,9 @@
-// First-dimension kernels: multiply_reg_by_database (lib/spiral-rs/src/server.rs:155-221) over an
-// HBM-resident database, the item writers that convert and place items in any of its layouts, and DoublePIR's packed
-// matvec (lib/doublepir/src/matrix/kernels.rs:14-178).  All of these are pure streams of the
-// database: 8 bytes read -> 4 (u32 x u32 -> u64) multiply-adds, so the design goal is coalesced
-// 16-byte loads, many of them in flight per SM, and no shared-memory or shuffle traffic at all.
+// First-dimension kernels on the IMAD layout (format 0): multiply_reg_by_database (lib/spiral-rs/src/server.rs:155-221) over
+// an HBM-resident database and the query operand it reads; the single-item upsert into any layout; and DoublePIR's
+// single-vector packed matvec (lib/doublepir/src/matrix/kernels.rs:14-178) with the small kernels of answer()'s tail.  The
+// item writer (k_write_items) runs the NTT and so lives with the other transforms in poly_kernels.cu.  The products are pure
+// streams of the database: 8 bytes read -> 4 (u32 x u32 -> u64) multiply-adds, so the design goal is coalesced 16-byte loads,
+// many of them in flight per SM, and no shared-memory or shuffle traffic at all.
 //
 // Device layout of one slice (format 0, built from the reference layout at upload, export_kernels.cu; the C ABI accepts
 // the reference layout [z][ii][j], server.rs:263-266):
@@ -19,31 +20,6 @@
 namespace b200pir {
 
 namespace {
-
-__constant__ Twiddle c_tw_lo_mul[2][3][64];
-struct TwConstM {
-  int n, dir;
-  __device__ __forceinline__ Twiddle operator()(int i) const { return c_tw_lo_mul[n][dir][i]; }
-  __device__ __forceinline__ void load2(int i, Twiddle (&t)[2]) const { t[0] = (*this)(i); t[1] = (*this)(i + 1); }
-  __device__ __forceinline__ void load4(int i, Twiddle (&t)[4]) const {
-    t[0] = (*this)(i); t[1] = (*this)(i + 1); t[2] = (*this)(i + 2); t[3] = (*this)(i + 3);
-  }
-};
-struct TwGlobalM {
-  const Twiddle* p;
-  __device__ __forceinline__ Twiddle operator()(int i) const {
-    uint2 v = __ldg(reinterpret_cast<const uint2*>(p + i));
-    return Twiddle{v.x, v.y};
-  }
-  __device__ __forceinline__ void load2(int i, Twiddle (&t)[2]) const {
-    uint4 v = __ldg(reinterpret_cast<const uint4*>(p + i));
-    t[0] = Twiddle{v.x, v.y}; t[1] = Twiddle{v.z, v.w};
-  }
-  __device__ __forceinline__ void load4(int i, Twiddle (&t)[4]) const {
-    uint4 v = __ldg(reinterpret_cast<const uint4*>(p + i)), w = __ldg(reinterpret_cast<const uint4*>(p + i) + 1);
-    t[0] = Twiddle{v.x, v.y}; t[1] = Twiddle{v.z, v.w}; t[2] = Twiddle{w.x, w.y}; t[3] = Twiddle{w.z, w.w};
-  }
-};
 
 template <int R, int NQ, int UNROLL>
 __global__ void __launch_bounds__(512)
@@ -139,68 +115,6 @@ __global__ void k_query_to_dev(MulGeom G, uint4* q_dev, const uint64_t* v) {
       make_uint4((uint32_t)a0, (uint32_t)(a0 >> 32), (uint32_t)a1, (uint32_t)(a1 >> 32));
 }
 
-__device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t index) {
-  uint64_t z = seed + (index + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  return z ^ (z >> 31);
-}
-
-// Plaintext sources of k_write_items: item(b) is the item CTA column b writes (its local row il and column j), coef(it, c, i, pt)
-// coefficient i < 2048 of its chunk c, a value below pt.
-// Raw bytes (lib/server/src/db/loading.rs:317-359 update_item_raw): item b of `items`; chunk c is the bpc bytes at
-// item.off + c * bpc of `bytes`, zero past item.len (the zero padding of update_item_raw), coefficient i = byte i.
-struct ItemBytes {
-  const uint8_t* bytes; const ItemWrite* items; int bpc;
-  struct Item { int il, j; const uint8_t* src; uint32_t len; };
-  __device__ Item item(unsigned b) const { const ItemWrite it = items[b]; return Item{(int)it.il, (int)it.j, bytes + it.off, it.len}; }
-  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t) const {
-    const int begin = c * bpc;
-    return (i < bpc && (uint32_t)(begin + i) < it.len) ? (uint64_t)it.src[begin + i] : 0;
-  }
-};
-// The synthetic database (server.rs:223-275 with a counter PRNG): item b is (il, j) = (b / dim0, b % dim0) of this GPU's rows;
-// coefficient i of slice c is splitmix64_at(seed, (c * num_items + item) * 2048 + i) % pt, item = j * num_per_global + ii.
-struct ItemSynthetic {
-  MulGeom G; Shard sh; uint64_t seed;
-  struct Item { int il, j; uint64_t item; };
-  __device__ Item item(unsigned b) const {
-    const int il = (int)(b / G.dim0), j = (int)(b % G.dim0);
-    return Item{il, j, (uint64_t)j * G.num_per * sh.count + (uint64_t)il * sh.count + sh.index};
-  }
-  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t pt) const {
-    const uint64_t num_items = (uint64_t)G.dim0 * G.num_per * sh.count;
-    return splitmix64_at(seed, ((uint64_t)c * num_items + it.item) * POLY + i) % pt;
-  }
-};
-
-// Many items at once, conversion and placement fused.  CTA = (item, chunk c): the chunk's coefficients from the source,
-// recenter_mod, forward NTT mod both q_n (loading.rs:278-299 convert_pt_to_poly), and the two residues go straight to the
-// item's place in the database of slice c.  512 threads: one 256-thread group per modulus; 2 CTAs per SM (64 registers, no
-// spills on sm_90a).
-template <typename Src>
-__global__ void __launch_bounds__(512, 2)
-k_write_items(DevParams P, DbLayout L, Src src, uint64_t pt) {
-  __shared__ __align__(16) uint32_t ntt_smem[2 * NTT_SMEM_WORDS];
-  __shared__ uint32_t halves[2][POLY];
-  const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
-  const int slice = blockIdx.y;
-  const uint32_t q = n ? P.q[1] : P.q[0];
-  const typename Src::Item it = src.item(blockIdx.x);
-  struct S { __device__ __forceinline__ void operator()() const { __syncthreads(); } };
-  uint32_t x[8];
-#pragma unroll
-  for (int a = 0; a < 8; a++) {
-    const uint64_t v = src.coef(it, slice, a * 256 + tid, pt);
-    x[a] = (v > pt / 2) ? (uint32_t)(q - (uint32_t)(pt - v)) : (uint32_t)v;       // recenter_mod, then mod q_n
-  }
-  ntt_forward_group_lz<NTT_OUT_CANON>(tid, x, ntt_smem + n * NTT_SMEM_WORDS, TwConstM{n, 0}, TwGlobalM{n ? P.fwd[1] : P.fwd[0]}, q, S());   // inputs canonical
-#pragma unroll
-  for (int k = 0; k < 8; k++) halves[n][tid * 8 + k] = x[k];
-  __syncthreads();
-  for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, it.il, it.j, z, halves[0][z], halves[1][z]);
-}
-
 // one item polynomial (2048 packed words lo|hi<<32) into the database, in any layout
 __global__ void k_db_upsert(DbLayout L, int slice, int il, int j, const uint64_t* poly) {
   const int z = blockIdx.x * blockDim.x + threadIdx.x;
@@ -211,12 +125,12 @@ __global__ void k_db_upsert(DbLayout L, int slice, int il, int j, const uint64_t
 
 // ------------------------------------------------------------------ DoublePIR
 // out[i] = sum_k sum_{m<3} ((a[i][k] >> 10m) & 1023) * b[3k+m]   (wrapping u32; kernels.rs:52-93)
-// One warp per ROWS rows; lanes stride over k.  b is staged in shared memory as three planes
-// bm[m][k] so that a lane's two consecutive k read one conflict-free 8-byte word per plane.
-template <int ROWS>
+// Odd column counts, whose rows are not 8-byte aligned: one warp per ROWS rows, lanes stride over k.  b is staged in shared
+// memory as three planes bm[m][k].
 __global__ void __launch_bounds__(256)
 k_dpir_matvec(uint32_t* __restrict__ out, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, size_t rows,
               size_t cols, size_t cols_pad) {
+  constexpr int ROWS = 4;
   extern __shared__ __align__(16) uint32_t bsm[];          // [3][cols_pad]
   for (size_t k = threadIdx.x; k < cols; k += blockDim.x) {
     bsm[k] = b[3 * k];
@@ -225,6 +139,8 @@ k_dpir_matvec(uint32_t* __restrict__ out, const uint32_t* __restrict__ a, const 
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  // launch_dpir_matvec sends even column counts to k_dpir_matvec_row, so vec2 is never true.  The branch stays because without
+  // it the odd-column loop compiles to 40 registers instead of 32 and ran 0.2 % slower at 2^23 x 1365 on H100.
   const bool vec2 = (cols & 1) == 0;
   for (size_t row0 = ((size_t)blockIdx.x * nwarps + warp) * ROWS; row0 < rows; row0 += (size_t)gridDim.x * nwarps * ROWS) {
     uint32_t acc[ROWS];
@@ -268,11 +184,13 @@ k_dpir_matvec(uint32_t* __restrict__ out, const uint32_t* __restrict__ a, const 
   }
 }
 
-// One row per warp; every lane keeps U independent 8-byte streaming loads in flight before it consumes them.
-template <int U>
+// Even column counts: one row per warp; every lane keeps U independent 8-byte streaming loads in flight before it consumes
+// them.  b is staged in shared memory as three planes bm[m][k], so a lane's two consecutive k read one conflict-free 8-byte
+// word per plane.
 __global__ void __launch_bounds__(256)
 k_dpir_matvec_row(uint32_t* __restrict__ out, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, size_t rows,
                   size_t cols, size_t cols_pad) {
+  constexpr int U = 8;
   extern __shared__ __align__(16) uint32_t bsm[];          // [3][cols_pad]
   for (size_t k = threadIdx.x; k < cols_pad; k += blockDim.x) {
     bool in = k < cols;
@@ -375,8 +293,6 @@ __global__ void k_dpir_transpose_expand(uint32_t* __restrict__ out, const uint32
   out[idx] = acc;
 }
 
-inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + block - 1) / block); }
-
 }  // namespace
 
 void launch_dpir_mul_transposed(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t a_rows, size_t a_cols,
@@ -390,21 +306,16 @@ void launch_dpir_transpose_expand(uint32_t* out, const uint32_t* a, size_t rows,
   k_dpir_transpose_expand<<<grid1d(out_rows * out_cols, 256), 256, 0, s>>>(out, a, rows, cols, modulus, delta, concat,
                                                                            out_rows, out_cols);
 }
-void upload_mul_constants(const Twiddle* lo, cudaStream_t s) {
-  B200_CUDA(cudaMemcpyToSymbolAsync(c_tw_lo_mul, lo, sizeof(Twiddle) * 2 * 3 * 64, 0, cudaMemcpyHostToDevice, s));
-}
 void launch_multiply(const DevParams& P, const MulGeom& G, const uint4* db_dev, const uint4* q_dev, uint32_t* out,
-                     int slice_begin, int slice_count, int nq, size_t q_stride, size_t out_stride, int variant,
-                     cudaStream_t s) {
+                     int slice_begin, int slice_count, int nq, size_t q_stride, size_t out_stride, cudaStream_t s) {
   if (G.dim0 < 2 || (G.dim0 & 1)) throw Error(-2, "multiply: dim0 must be even");
   // row tile: the largest of {8,4,2,1} dividing num_per (num_per is a power of two)
-  int R = G.num_per >= 8 ? 8 : G.num_per;
-  if (variant == 1 && R == 8) R = 4;
+  const int R = G.num_per >= 8 ? 8 : G.num_per;
 #define MUL_CASE(RR, QQ, UU, GG)                                                                                     \
   launch_mul_t<RR, QQ, UU>(P, G, db_dev, q_dev, out, slice_begin, slice_count, q_stride, out_stride, GG, s)
   if (nq == 1) {
-    if (R == 8) { if (variant == 2) MUL_CASE(8, 1, 1, 1); else MUL_CASE(8, 1, 1, 2); }
-    else if (R == 4) { if (variant == 3) MUL_CASE(4, 1, 2, 2); else MUL_CASE(4, 1, 2, 4); }
+    if (R == 8) MUL_CASE(8, 1, 1, 2);
+    else if (R == 4) MUL_CASE(4, 1, 2, 4);
     else if (R == 2) MUL_CASE(2, 1, 2, 2);
     else MUL_CASE(1, 1, 2, 1);
   } else if (nq == 2) {
@@ -428,22 +339,7 @@ void launch_db_upsert(const DbLayout& L, int slice, int il, int j, const uint64_
   ++g_kernel_launches;
   k_db_upsert<<<POLY / 256, 256, 0, s>>>(L, slice, il, j, poly);
 }
-void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
-                        int bpc, uint64_t pt_modulus, cudaStream_t s) {
-  if (count == 0) return;
-  if (chunks > 65535) throw Error(-2, "write_items: more than 65535 slices");
-  ++g_kernel_launches;
-  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, ItemBytes{bytes, items, bpc}, pt_modulus);
-}
-void launch_write_synthetic(const DevParams& P, const DbLayout& L, Shard sh, uint64_t seed, uint64_t pt_modulus, cudaStream_t s) {
-  const size_t count = (size_t)L.G.num_per * L.G.dim0;
-  if (count == 0) return;
-  if (count > 0x7fffffffULL || L.G.slices > 65535) throw Error(-2, "write_synthetic: grid too large");
-  ++g_kernel_launches;
-  k_write_items<<<dim3((unsigned)count, (unsigned)L.G.slices), 512, 0, s>>>(P, L, ItemSynthetic{L.G, sh, seed}, pt_modulus);
-}
-void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t rows, size_t cols, int variant,
-                        cudaStream_t s) {
+void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, size_t rows, size_t cols, cudaStream_t s) {
   size_t cols_pad = (cols + 3) & ~(size_t)3;
   size_t smem = 3 * cols_pad * 4;
   if (rows == 0) return;
@@ -453,32 +349,18 @@ void launch_dpir_matvec(uint32_t* out, const uint32_t* a, const uint32_t* b, siz
     k_dpir_matvec_wide<<<(unsigned)rows, 256, 0, s>>>(out, a, b, rows, cols);
     return;
   }
-  if ((cols & 1) == 0 && variant != 1 && variant != 4) {
-    // default: one row per warp, 8 loads in flight per lane (variant 2: 4 loads)
+  if ((cols & 1) == 0) {
     unsigned g = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)132 * 8);
+    cudaFuncSetAttribute(k_dpir_matvec_row, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     ++g_kernel_launches;
-    if (variant == 2) {
-      cudaFuncSetAttribute(k_dpir_matvec_row<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      k_dpir_matvec_row<4><<<g, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
-    } else {
-      cudaFuncSetAttribute(k_dpir_matvec_row<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      k_dpir_matvec_row<8><<<g, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
-    }
+    k_dpir_matvec_row<<<g, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
     return;
   }
-  const int rows_per_warp = variant == 1 ? 2 : 4;
-  size_t warps_needed = (rows + rows_per_warp - 1) / rows_per_warp;
+  size_t warps_needed = (rows + 3) / 4;
   unsigned grid = (unsigned)std::min<size_t>((warps_needed + 7) / 8, (size_t)132 * 8);
-  if (grid == 0) return;
-  if (rows_per_warp == 2) {
-    cudaFuncSetAttribute(k_dpir_matvec<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    ++g_kernel_launches;
-    k_dpir_matvec<2><<<grid, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
-  } else {
-    cudaFuncSetAttribute(k_dpir_matvec<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    ++g_kernel_launches;
-    k_dpir_matvec<4><<<grid, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
-  }
+  cudaFuncSetAttribute(k_dpir_matvec, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  ++g_kernel_launches;
+  k_dpir_matvec<<<grid, 256, smem, s>>>(out, a, b, rows, cols, cols_pad);
 }
 
 }  // namespace b200pir

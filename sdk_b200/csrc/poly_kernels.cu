@@ -1,4 +1,6 @@
-// Ring-arithmetic kernels for the Spiral second dimension, query expansion and packing (sm_90a).
+// Ring-arithmetic kernels for the Spiral second dimension, query expansion and packing (sm_90a), and every other kernel that
+// runs the NTT: the plain transforms, the item writer (convert_pt_to_poly fused with the placement into the database) and the
+// inverse transform of the first dimension's product.
 //
 // Every kernel here runs CTAs of 512 threads = two groups of 256; group g works modulo q_g, so the
 // two CRT halves of a polynomial are transformed side by side and can be CRT-lifted inside the CTA.
@@ -19,7 +21,8 @@ constexpr int HI_TW = NTT_N - 64;       // twiddle table entries 64..2047 (passe
 
 // Table entries 0..63 (passes A and B) of every (modulus, direction) live in the constant bank: the
 // index is thread-uniform (pass A) or warp-uniform (pass B), so they cost no load/store-unit traffic.
-__constant__ Twiddle c_tw_lo[2][3][64];     // [n][0 = forward, 1 = inverse][index]
+// This is the library's only twiddle bank: every kernel that runs the NTT of ntt_core.cuh is in this file.
+__constant__ Twiddle c_tw_lo[2][3][64];     // [n][0 = forward, 1 = inverse, 2 = relaxed-range inverse][index]
 
 struct TwConst {
   int n, dir;
@@ -329,6 +332,61 @@ __global__ void __launch_bounds__(256) k_to_ntt(DevParams P, uint32_t* out, cons
   grp_ntt_fwd<false>(g, x);
   st8(out + ((size_t)blockIdx.x * 2 + g.n) * POLY + g.tid * 8, x);
 }
+
+// Plaintext sources of k_write_items: item(b) is the item CTA column b writes (its local row il and column j), coef(it, c, i, pt)
+// coefficient i < 2048 of its chunk c, a value below pt.
+// Raw bytes (lib/server/src/db/loading.rs:317-359 update_item_raw): item b of `items`; chunk c is the bpc bytes at
+// item.off + c * bpc of `bytes`, zero past item.len (the zero padding of update_item_raw), coefficient i = byte i.
+struct ItemBytes {
+  const uint8_t* bytes; const ItemWrite* items; int bpc;
+  struct Item { int il, j; const uint8_t* src; uint32_t len; };
+  __device__ Item item(unsigned b) const { const ItemWrite it = items[b]; return Item{(int)it.il, (int)it.j, bytes + it.off, it.len}; }
+  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t) const {
+    const int begin = c * bpc;
+    return (i < bpc && (uint32_t)(begin + i) < it.len) ? (uint64_t)it.src[begin + i] : 0;
+  }
+};
+// The synthetic database (server.rs:223-275 with a counter PRNG): item b is (il, j) = (b / dim0, b % dim0) of this GPU's rows;
+// coefficient i of slice c is splitmix64_at(seed, (c * num_items + item) * 2048 + i) % pt, item = j * num_per_global + ii.
+struct ItemSynthetic {
+  MulGeom G; Shard sh; uint64_t seed;
+  struct Item { int il, j; uint64_t item; };
+  __device__ Item item(unsigned b) const {
+    const int il = (int)(b / G.dim0), j = (int)(b % G.dim0);
+    return Item{il, j, (uint64_t)j * G.num_per * sh.count + (uint64_t)il * sh.count + sh.index};
+  }
+  __device__ uint64_t coef(const Item& it, int c, int i, uint64_t pt) const {
+    const uint64_t num_items = (uint64_t)G.dim0 * G.num_per * sh.count;
+    return splitmix64_at(seed, ((uint64_t)c * num_items + it.item) * POLY + i) % pt;
+  }
+};
+
+// Many items at once, conversion and placement fused.  CTA = (item, chunk c): the chunk's coefficients from the source,
+// recenter_mod, forward NTT mod both q_n (loading.rs:278-299 convert_pt_to_poly), and the two residues go straight to the
+// item's place in the database of slice c (item_place.cuh).  512 threads: one 256-thread group per modulus; 2 CTAs per SM (64
+// registers, no spills on sm_90a).  The transform keeps ntt_forward_group_lz's default input contract (canonical inputs), not
+// grp_ntt_fwd's inputs < 4q.
+template <typename Src>
+__global__ void __launch_bounds__(512, 2)
+k_write_items(DevParams P, DbLayout L, Src src, uint64_t pt) {
+  __shared__ __align__(16) uint32_t ntt_smem[2 * NTT_SMEM_WORDS];
+  __shared__ uint32_t halves[2][POLY];
+  const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
+  const int slice = blockIdx.y;
+  const uint32_t q = n ? P.q[1] : P.q[0];
+  const typename Src::Item it = src.item(blockIdx.x);
+  uint32_t x[8];
+#pragma unroll
+  for (int a = 0; a < 8; a++) {
+    const uint64_t v = src.coef(it, slice, a * 256 + tid, pt);
+    x[a] = (v > pt / 2) ? (uint32_t)(q - (uint32_t)(pt - v)) : (uint32_t)v;       // recenter_mod, then mod q_n
+  }
+  ntt_forward_group_lz<NTT_OUT_CANON>(tid, x, ntt_smem + n * NTT_SMEM_WORDS, TwConst{n, 0}, TwGlobal{n ? P.fwd[1] : P.fwd[0]}, q, CtaSync());
+#pragma unroll
+  for (int k = 0; k < 8; k++) halves[n][tid * 8 + k] = x[k];
+  __syncthreads();
+  for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, it.il, it.j, z, halves[0][z], halves[1][z]);
+}
 // raw u64 coefficients -> residue form u32 [poly][n][z] (coefficient domain), and back (CRT lift)
 __global__ void k_raw_to_res(DevParams P, uint32_t* out, const uint64_t* raw, size_t polys) {
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;     // over polys * 2048
@@ -355,6 +413,66 @@ __global__ void __launch_bounds__(CTA) k_from_ntt(DevParams P, uint64_t* out, co
   grp_ntt_inv(g, x);
   uint64_t* dst = out + (size_t)blockIdx.x * POLY;
   crt_lift(x, res, g, P, [&](int z, uint64_t v) { dst[z] = v; });
+}
+
+// from_ntt of the first dimension's z-major product (tc5_kernels.cu, imma_kernels.cu): inverse NTT of every (ciphertext row,
+// modulus) -> residue-form ciphertexts
+//   out[((query*slices + slice)*rows + ii)][ct_row][n][z]     (server.rs:707-709 without the CRT lift)
+// One CTA handles PP (= 2, 4 or 8) polynomials that are adjacent in the z-major product, so every 32-byte sector it fetches
+// is fully used (one CTA per polynomial would use 4 of every 32 bytes: its z-stride is rows*2 words).  The PP polynomials
+// are transposed through shared memory, then inverse-transformed two at a time.  rows*2 is even, so PP = 2 always fits.
+// grid = (rows*2 / PP, 2 moduli, nq*slices), 256 threads, dynamic smem = PP*2048*4 + 2*NTT_SMEM_WORDS*4
+template <int PP>
+__global__ void __launch_bounds__(256)
+k_intt_from_zmajor_tiled(DevParams P, ImmaGeom F, const uint32_t* __restrict__ in_zm, size_t in_stride,
+                         uint32_t* __restrict__ out, int slices) {
+  extern __shared__ __align__(16) uint32_t tsm[];
+  uint32_t* polybuf = tsm;                               // [PP][2048]
+  uint32_t* sm0 = tsm + PP * POLY;
+  uint32_t* sm1 = sm0 + NTT_SMEM_WORDS;
+  const int tid = threadIdx.x, n = blockIdx.y;
+  const int p0 = blockIdx.x * PP;                        // index into the flattened [row][ct_row] axis
+  const int qs = blockIdx.z, qi = qs / slices, slice = qs % slices;
+  const uint32_t q = n ? P.q[1] : P.q[0];
+  const size_t zstride = (size_t)F.rows * 2;
+  const uint32_t* src = in_zm + (size_t)qi * in_stride + (((size_t)slice * 2 + n) * POLY) * zstride + p0;
+  for (int z = tid; z < POLY; z += 256) {
+    uint32_t v[PP];
+    const uint32_t* s = src + (size_t)z * zstride;
+    if (PP == 8) {
+      uint4 a = __ldg(reinterpret_cast<const uint4*>(s)), b = __ldg(reinterpret_cast<const uint4*>(s) + 1);
+      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4 % PP] = b.x; v[5 % PP] = b.y; v[6 % PP] = b.z; v[7 % PP] = b.w;
+    } else if (PP == 4) {
+      uint4 a = __ldg(reinterpret_cast<const uint4*>(s));
+      v[0] = a.x; v[1] = a.y; v[2 % PP] = a.z; v[3 % PP] = a.w;
+    } else {
+      uint2 a = __ldg(reinterpret_cast<const uint2*>(s));
+      v[0] = a.x; v[1] = a.y;
+    }
+#pragma unroll
+    for (int p = 0; p < PP; p++) polybuf[p * POLY + z] = v[p];
+  }
+  __syncthreads();
+  const TwConst lo{n, 2};                                // relaxed-range inverse (ntt_core.cuh "lz"): inputs are canonical residues
+  const TwGlobal hi{n ? P.inv_lz[1] : P.inv_lz[0]};
+#pragma unroll 1
+  for (int p = 0; p < PP; p += 2) {
+    uint32_t x0[8], x1[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      x0[k] = polybuf[p * POLY + tid * 8 + k];
+      x1[k] = polybuf[(p + 1) * POLY + tid * 8 + k];
+    }
+    ntt_inverse_group2_nh(tid, x0, x1, sm0, sm1, lo, hi, q, CtaSync());
+    const int f0 = p0 + p, f1 = p0 + p + 1;               // flattened (row, ct_row)
+    uint32_t* d0 = out + ((((size_t)qs * F.rows + (f0 >> 1)) * 2 + (f0 & 1)) * 2 + n) * POLY;
+    uint32_t* d1 = out + ((((size_t)qs * F.rows + (f1 >> 1)) * 2 + (f1 & 1)) * 2 + n) * POLY;
+#pragma unroll
+    for (int a = 0; a < 8; a++) {
+      d0[a * 256 + tid] = x0[a];
+      d1[a * 256 + tid] = x1[a];
+    }
+  }
 }
 __global__ void k_widen(uint64_t* out, const uint32_t* in, size_t words) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1008,7 +1126,6 @@ __global__ void k_encode(DevParams P, uint64_t* out, size_t out_words, const uin
   out[w] = word;
 }
 
-inline unsigned grid1d(size_t total, int block) { return (unsigned)((total + block - 1) / block); }
 const size_t kDynSmemBig = (size_t)(4 * NTT_SMEM_WORDS + 2 * POLY) * 4 + (size_t)2 * POLY * 8 + (size_t)2 * HI_TW * 8;
 const size_t kDynSmemFold = (size_t)(2 * NTT_SMEM_WORDS) * 4 + (size_t)HI_TW * 8;
 
@@ -1033,6 +1150,20 @@ void launch_to_ntt_strided(const DevParams& P, uint32_t* out, size_t out_stride,
                            size_t count, int batches, cudaStream_t s) {
   if (count && batches)
     ++g_kernel_launches, k_to_ntt<<<dim3((unsigned)count, 2, (unsigned)batches), 256, 0, s>>>(P, out, raw, out_stride, raw_stride);
+}
+void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
+                        int bpc, uint64_t pt_modulus, cudaStream_t s) {
+  if (count == 0) return;
+  if (chunks > 65535) throw Error(-2, "write_items: more than 65535 slices");
+  ++g_kernel_launches;
+  k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, ItemBytes{bytes, items, bpc}, pt_modulus);
+}
+void launch_write_synthetic(const DevParams& P, const DbLayout& L, Shard sh, uint64_t seed, uint64_t pt_modulus, cudaStream_t s) {
+  const size_t count = (size_t)L.G.num_per * L.G.dim0;
+  if (count == 0) return;
+  if (count > 0x7fffffffULL || L.G.slices > 65535) throw Error(-2, "write_synthetic: grid too large");
+  ++g_kernel_launches;
+  k_write_items<<<dim3((unsigned)count, (unsigned)L.G.slices), 512, 0, s>>>(P, L, ItemSynthetic{L.G, sh, seed}, pt_modulus);
 }
 void launch_raw_to_res(const DevParams& P, uint32_t* out, const uint64_t* raw, size_t polys, cudaStream_t s) {
   if (polys) ++g_kernel_launches, k_raw_to_res<<<grid1d(polys * POLY, 256), 256, 0, s>>>(P, out, raw, polys);
@@ -1062,6 +1193,21 @@ void launch_fold_res(const DevParams& P, const uint32_t* in, uint32_t* out, size
 }
 void launch_from_ntt(const DevParams& P, uint64_t* out_raw, const uint32_t* in, size_t count, cudaStream_t s) {
   if (count) ++g_kernel_launches, k_from_ntt<<<(unsigned)count, CTA, 0, s>>>(P, out_raw, in);
+}
+template <int PP>
+static void launch_intt_tiled(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
+                              int nq, int slices, cudaStream_t s) {
+  const size_t smem = (size_t)(PP * POLY + 2 * NTT_SMEM_WORDS) * 4;
+  opt_in_smem(k_intt_from_zmajor_tiled<PP>, (int)smem);
+  k_intt_from_zmajor_tiled<PP><<<dim3(F.rows * 2 / PP, 2, nq * slices), 256, smem, s>>>(P, F, in_zm, in_stride, out, slices);
+}
+void launch_intt_from_zmajor(const DevParams& P, const ImmaGeom& F, const uint32_t* in_zm, size_t in_stride, uint32_t* out,
+                             int nq, int slices, cudaStream_t s) {
+  ++g_kernel_launches;
+  const int polys = F.rows * 2;
+  if (polys % 8 == 0) launch_intt_tiled<8>(P, F, in_zm, in_stride, out, nq, slices, s);
+  else if (polys % 4 == 0) launch_intt_tiled<4>(P, F, in_zm, in_stride, out, nq, slices, s);
+  else launch_intt_tiled<2>(P, F, in_zm, in_stride, out, nq, slices, s);
 }
 void launch_widen(uint64_t* out, const uint32_t* in, size_t words, cudaStream_t s) {
   if (words) ++g_kernel_launches, k_widen<<<grid1d(words, 256), 256, 0, s>>>(out, in, words);

@@ -183,8 +183,9 @@ def test_dpir_gpu_chunked_answers_add_up_and_decode():
 
 # ------------------------------------------------------------------ matvec dispatch (launch_dpir_matvec) against numpy
 # `b` is staged in shared memory up to 17064 packed words a row (3 * 17064 * 4 bytes = 200 KiB), wider rows take the wide
-# kernel.  Even cols: row<8> (variants 0, 3), row<4> (variant 2); odd cols or variant 4: matvec<4>; variant 1: matvec<2>.
-# A grid-stride pass covers 8448 rows in the row kernels, 16896 in matvec<2> and 33792 in matvec<4>.
+# kernel (17065, 17066).  Below that, even cols run k_dpir_matvec_row and odd cols (1, 3, 5, ...) k_dpir_matvec.  A grid-stride
+# pass covers 8448 rows in k_dpir_matvec_row and 33792 in k_dpir_matvec.  Variants 1, 2 and 4 are retired tilings: accepted,
+# and they must give the same bytes.
 MATVEC_SHAPES = ([(r, c) for r in (1, 7, 8, 9) for c in (1, 2, 3, 4, 5)]
                  + [(9, c) for c in (17062, 17063, 17064, 17065, 17066)]
                  + [(16899, 2), (67589, 3), (67589, 4)])

@@ -487,7 +487,7 @@ def test_a_dpir_matvec_packed_dev_on_callers_stream(delay, streams):
         out = torch.zeros(rows, dtype=torch.int32, device="cuda")
         out_copy = torch.zeros_like(out)
         torch.cuda.synchronize()
-        for variant in (0, 1, 2, 4):
+        for variant in (0, 1, 2, 4):                           # 1, 2 and 4 are retired tilings: accepted, and they select nothing
             call = lambda: check(LIB.b200pir_dpir_matvec_packed_dev(m._h, b_dev.data_ptr(), out.data_ptr(), variant))
             ms = delay.device_ms(stream, call)                 # out now holds the decoy vector's product
             delay.ordered(stream, ms, lambda: b_dev.copy_(real), call, lambda: (out_copy.copy_(out), b_dev.copy_(decoy)))
