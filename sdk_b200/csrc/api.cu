@@ -1,28 +1,14 @@
-// C-ABI implementation (include/b200pir.h): contexts, HBM-resident handles and the host-side
-// orchestration of spiral_rs::server::process_query (lib/spiral-rs/src/server.rs:650-741) as a
-// stream of sm_90a kernel launches.  No CPU fallback exists anywhere on this path: every entry
-// point either runs on the GPU or returns an error.
-#include "api_internal.hpp"
+// C-ABI implementation (include/b200pir.h): contexts, public parameters and the host-side orchestration of
+// spiral_rs::server::process_query (lib/spiral-rs/src/server.rs:650-741) as a stream of sm_90a kernel launches; the database
+// handle is in db_api.cu.  No CPU fallback exists anywhere on this path: every entry point either runs on the GPU or returns
+// an error.
+#include "spiral_api.hpp"
 #include "ntt_tables.hpp"
-#include "update_body.hpp"
 #include "gadget.hpp"
-#include <cstdio>
-#include <cerrno>
-#include <fcntl.h>
-#include <unistd.h>
-#include <algorithm>
 #include <cmath>
 #include <memory>
-#include <cstring>
-#include <condition_variable>
-#include <chrono>
-#include <deque>
-#include <mutex>
 #include <set>
 #include <utility>
-#include <vector>
-
-using namespace b200pir;
 
 namespace b200pir {
 thread_local unsigned long long g_kernel_launches = 0;
@@ -60,235 +46,7 @@ const uint64_t kQ2Values[37] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 12289U
                                 2013265921ULL, 4293918721ULL, 8588886017ULL, 17175674881ULL, 34359214081ULL,
                                 68718428161ULL};   // params.rs:8-46
 
-enum Stage { ST_EXPAND = 0, ST_MUL, ST_FROMNTT, ST_FOLD, ST_PACK, ST_ENCODE, ST_QIMG /* query operand re-tiling */, ST_COUNT };
-
 }  // namespace
-
-struct b200pir_ctx {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = true;
-  std::recursive_mutex mu;
-  b200pir_params hp;
-  // derived (params.rs:116-200)
-  int dim0, num_per, slices, trials, g, stop_round, num_packing;
-  int bits_gsw, bits_conv, bits_left, bits_right;
-  int live_gsw, live_conv, live_left, live_right;     // live_digits() of each gadget
-  bool has_right;
-  uint64_t q2, q1, setup_bytes, query_bytes, response_bytes;
-  int q1_bits;
-  DevParams dp;
-  DevBuf<Twiddle> d_tw;      // fwd0, inv0, fwd1, inv1, inv_lz0, inv_lz1
-  DevBuf<Twiddle> d_tw4k;    // fwd0, inv0, fwd1, inv1 for poly_len 4096 (config #5 sweep)
-  DevBuf<uint32_t> d_neg1;   // [11][2][2048] ntt32 (params.rs:98-107)
-  // options
-  int max_group = 16, profile = 0;  // max_group: queries per database pass (IMAD path: <= 4)
-  int sparse_fold = 0;           // 1: lib/server's fold (all-zero ciphertext shortcut, compute/fold.rs:37-43); 0: spiral-rs dense fold
-  int db_format = -1;            // format given to databases created from now on: -1 = automatic (2 where the wgmma kernel
-                                 // supports the geometry, else 1), 0 = IMAD layout, 1 = mma.sync fragments, 2 = wgmma tile images
-  DevBuf<uint2> w_qf;            // B operand of the IMMA path (one group of <= 16 queries)
-  DevBuf<uint8_t> w_qt;          // B operand of the wgmma path (tile images, 16 queries)
-  int sm_count = 0;
-  // workspace, sized for `ws_queries` queries
-  size_t ws_queries = 0, ws_rows = 0;
-  DevBuf<uint64_t> w_query;      // [Q][2][2048] raw
-  DevBuf<uint32_t> w_v;          // [Q][2^g][2][2][2048]
-  DevBuf<uint32_t> w_zflags;     // all-zero flags of the current fold round's ciphertexts ("sparse_fold")
-  DevBuf<uint32_t> w_xr;         // [Q][num_in][2][2048] residues of row 0 (expansion rounds)
-  DevBuf<uint4> w_qdev;          // [Q][dim0][2048]
-  DevBuf<uint32_t> w_vfold, w_vfold_neg;   // [Q][nu_2][2][2t][2][2048]
-  DevBuf<uint32_t> w_mult;       // [Q][slices][rows][2][2][2048]  NTT form, then residue form in place
-  DevBuf<uint32_t> w_cts;        // ping-pong partner of w_mult for the fold rounds (same size)
-  const uint32_t* folded = nullptr;   // where the last fold left its survivors
-  size_t folded_stride = 0;           // u32 words between consecutive (query, slice) survivors
-  DevBuf<uint64_t> w_packed;     // [Q][inst][n+1][n][2048]
-  DevBuf<uint8_t> w_resp;        // [Q][response_bytes]
-  // database writers (update_item_raw, update_many_items, load_raw_file): raw item bytes and their item descriptors, one group
-  // of whole items at a time; sized on the first write, so later writes neither allocate nor free device memory
-  static constexpr size_t kWriteStageBytes = (size_t)64 << 20;
-  static constexpr size_t kWriteStageItems = 65536;
-  DevBuf<uint8_t> w_wbytes;
-  DevBuf<ItemWrite> w_witems;
-  // database exports (download, save_file): chunks are un-tiled into w_wbytes and copied to one of two pinned buffers, one
-  // event each; allocated on the first export, freed in b200pir_ctx_destroy.  Exports share them, so export_mu serialises
-  // exports with each other; queries only contend for `mu`, which an export holds per chunk.
-  std::mutex export_mu;
-  uint8_t* h_export[2] = {nullptr, nullptr};
-  size_t h_export_bytes = 0;
-  cudaEvent_t export_done[2] = {nullptr, nullptr};
-  void ensure_export_staging(size_t bytes) {
-    w_wbytes.ensure(std::max(kWriteStageBytes, bytes));
-    if (!export_done[0])
-      for (auto& e : export_done) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming | cudaEventBlockingSync));
-    if (bytes <= h_export_bytes) return;
-    release_export_pinned();
-    const size_t n = std::max(kWriteStageBytes, bytes);
-    for (auto& h : h_export) B200_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h), n, cudaHostAllocDefault));
-    h_export_bytes = n;
-  }
-  void release_export_pinned() {
-    for (auto& h : h_export) { if (h) cudaFreeHost(h); h = nullptr; }
-    h_export_bytes = 0;
-  }
-  // Coalescing of concurrent callers ("coalesce", default on): lib/server takes a READ lock around process_query
-  // (bin/server.rs:102), so actix workers call it concurrently.  Requests arriving while a batch runs queue up here; the
-  // thread that finds no batch in flight becomes the leader and serves everything queued (up to kCoalesceMax) in ONE
-  // database pass.  A lone caller is served immediately.  Two refinements for sustained load: a batch larger than one
-  // database pass (16 queries) is trimmed to whole passes, the remainder joining the next batch (it would have finished no
-  // earlier inside this one); and a leader that follows a multi-query batch by less than 1 ms gives the callers of that batch
-  // up to "coalesce_window_us" (default 200) to come back before it starts, so closed-loop clients do not alternate between
-  // full and near-empty passes.
-  struct Pending {
-    b200pir_db* db; b200pir_pp* pp; const uint64_t* query_ct; const uint8_t* query_bytes; uint8_t* out;
-    int rc = 0; std::string err; bool done = false;
-  };
-  static constexpr size_t kCoalesceMax = 32;
-  static constexpr size_t kPassQueries = 16;
-  int coalesce = 1;
-  int coalesce_window_us = 200;
-  size_t last_batch = 0;
-  std::chrono::steady_clock::time_point last_batch_end{};
-  std::mutex qmu;
-  std::condition_variable qcv;
-  std::deque<Pending*> pending;
-  bool leader_active = false;
-  unsigned long long coalesced_batches = 0, coalesced_queries = 0;
-  // per-query public parameters (PpTable, kernels.h): device arrays [4][pptab_cap] of base pointers; `multi_pps` (host array, one
-  // handle per query of the call in flight) is set by the multi-client entry points, otherwise one handle serves every query
-  DevBuf<const uint32_t*> d_pptab;
-  size_t pptab_cap = 0;
-  std::vector<const uint32_t*> h_pptab;          // what d_pptab holds (skip the upload when unchanged)
-  b200pir_pp* const* multi_pps = nullptr;
-  PpTable pp_table(b200pir_pp* pp, size_t count);
-  // profiling
-  struct Span { int stage; cudaEvent_t a, b; };
-  std::vector<Span> spans;
-  std::vector<cudaEvent_t> event_pool;
-  size_t event_next = 0;
-  int mul_launches = 0;
-  double last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // expand, multiply, from_ntt, fold, pack, encode, total, multiply launches, query image
-
-  size_t v_words() const { return ((size_t)1 << g) * 4 * POLY; }
-  size_t fold_words() const { return (size_t)hp.nu_2 * 2 * 2 * hp.t_gsw * 2 * POLY; }
-  MulGeom geom(int rows) const { return MulGeom{dim0, rows, slices}; }
-
-  cudaEvent_t get_event() {
-    if (event_next == event_pool.size()) {
-      cudaEvent_t e;
-      B200_CUDA(cudaEventCreate(&e));
-      event_pool.push_back(e);
-    }
-    return event_pool[event_next++];
-  }
-  struct Scope {
-    b200pir_ctx* c; int stage; cudaEvent_t a = nullptr;
-    Scope(b200pir_ctx* ctx, int st) : c(ctx), stage(st) {
-      if (c->profile) { a = c->get_event(); cudaEventRecord(a, c->stream); }
-    }
-    ~Scope() {
-      if (c->profile) { cudaEvent_t b = c->get_event(); cudaEventRecord(b, c->stream); c->spans.push_back({stage, a, b}); }
-    }
-  };
-  // profile == 1: per call; profile == 2: accumulate over calls until the option is set again
-  void prof_reset() { if (profile == 2) return; spans.clear(); event_next = 0; mul_launches = 0; }
-  void prof_collect() {
-    if (!profile) return;
-    B200_CUDA(cudaStreamSynchronize(stream));
-    for (int i = 0; i < 9; i++) last_ms[i] = 0;
-    for (auto& s : spans) {
-      float ms = 0;
-      cudaEventElapsedTime(&ms, s.a, s.b);
-      last_ms[s.stage == ST_QIMG ? 8 : s.stage] += ms;
-      last_ms[6] += ms;
-    }
-    last_ms[7] = mul_launches;
-  }
-  // buffers of the first dimension / fold / pack only (queries expanded elsewhere)
-  void ensure_workspace_lite(size_t queries, size_t rows) {
-    w_mult.ensure(queries * slices * rows * 4 * POLY);
-    w_cts.ensure(queries * slices * rows * 4 * POLY);
-    w_packed.ensure(queries * hp.instances * (hp.n + 1) * hp.n * POLY);
-  }
-  void ensure_workspace(size_t queries, size_t rows) {
-    if (queries <= ws_queries && rows <= ws_rows) return;
-    queries = std::max(queries, ws_queries);
-    rows = std::max(rows, ws_rows);
-    w_query.ensure(queries * 2 * POLY);
-    if (hp.expand_queries) w_v.ensure(queries * v_words());
-    w_qdev.ensure(queries * (size_t)dim0 * POLY);
-    w_vfold.ensure(queries * std::max<size_t>(fold_words(), 1));
-    w_vfold_neg.ensure(queries * std::max<size_t>(fold_words(), 1));
-    w_mult.ensure(queries * slices * rows * 4 * POLY);
-    w_cts.ensure(queries * slices * rows * 4 * POLY);
-    w_packed.ensure(queries * hp.instances * (hp.n + 1) * hp.n * POLY);
-    w_resp.ensure(queries * response_bytes);
-    ws_queries = queries;
-    ws_rows = rows;
-  }
-};
-
-struct b200pir_db {
-  b200pir_ctx* ctx;
-  Shard shard;
-  int rows;                 // local second-dimension rows
-  DbLayout layout;          // format (0: IMAD cells, 1: mma.sync fragments, 2: wgmma tile images), geometries, store.p
-  DevBuf<uint8_t> store;    // db_bytes(layout, slices) bytes
-  // The first dimension's product is z-major (formats 1 and 2: u32 [query][slice][n][z][row][ct_row]) or ntt32 (format 0)
-  bool zmajor_product() const { return layout.format != 0; }
-  // Presence (lib/server's SparseDb, db/sparse_db.rs:5-47: an item exists once it has been written).  Storage stays dense in HBM
-  // (absent = zero polynomial, so every sum is unchanged); what the map buys is COST: on the wgmma path whole 32-row x 32-j
-  // tiles without a present item are neither fetched nor multiplied (tile_mask, one bit per tile, kept on the device).
-  std::vector<uint64_t> present;          // bit ((slice * rows + il) * dim0 + j)
-  uint64_t present_count = 0;
-  std::vector<uint32_t> h_tile_mask;      // [slice][mt], bit ks
-  DevBuf<uint32_t> tile_mask;
-  uint64_t capacity() const { return (uint64_t)ctx->slices * rows * ctx->dim0; }
-  void presence_init() {
-    present.assign((capacity() + 63) / 64, 0);
-    present_count = 0;
-    h_tile_mask.assign((size_t)ctx->slices * layout.T.mt, 0u);
-    tile_mask.alloc(h_tile_mask.size());
-    // on the context's stream: a cudaMemset would queue on the legacy default stream, behind whatever the caller has there,
-    // and could land after the first writer's mask upload on the context's stream
-    B200_CUDA(cudaMemsetAsync(tile_mask.p, 0, h_tile_mask.size() * 4, ctx->stream));
-  }
-  // one item written, host side only: returns true when its tile-mask word changed (the device copy is then stale)
-  bool mark_host(int slice, int il, int j) {
-    const uint64_t bit = ((uint64_t)slice * rows + il) * ctx->dim0 + j;
-    if (!((present[bit >> 6] >> (bit & 63)) & 1)) { present[bit >> 6] |= 1ull << (bit & 63); present_count++; }
-    const size_t w = (size_t)slice * layout.T.mt + (il >> 5);
-    const uint32_t nv = h_tile_mask[w] | (1u << (j >> 5));
-    if (nv == h_tile_mask[w]) return false;
-    h_tile_mask[w] = nv;
-    return true;
-  }
-  // one item written (stream-ordered update of the device mask word)
-  void mark(int slice, int il, int j, cudaStream_t s) {
-    if (mark_host(slice, il, j)) {
-      const size_t w = (size_t)slice * layout.T.mt + (il >> 5);
-      B200_CUDA(cudaMemcpyAsync(tile_mask.p + w, &h_tile_mask[w], 4, cudaMemcpyHostToDevice, s));
-    }
-  }
-  // every item of every slice of `items` written: one upload of the whole mask when any word changed
-  void mark_items(const ItemWrite* items, size_t count, cudaStream_t s) {
-    bool changed = false;
-    for (size_t k = 0; k < count; k++)
-      for (int sl = 0; sl < ctx->slices; sl++) changed |= mark_host(sl, (int)items[k].il, (int)items[k].j);
-    if (changed)
-      B200_CUDA(cudaMemcpyAsync(tile_mask.p, h_tile_mask.data(), h_tile_mask.size() * 4, cudaMemcpyHostToDevice, s));
-  }
-  // a whole slice written at once (bulk upload, file load, synthetic fill): every item of it exists from now on
-  void mark_slice(int slice, cudaStream_t s) {
-    const uint64_t lo = (uint64_t)slice * rows * ctx->dim0, hi = lo + (uint64_t)rows * ctx->dim0;
-    for (uint64_t b = lo; b < hi; b++)
-      if (!((present[b >> 6] >> (b & 63)) & 1)) { present[b >> 6] |= 1ull << (b & 63); present_count++; }
-    const Tc5Geom& T = layout.T;
-    const uint32_t full = T.ks >= 32 ? 0xffffffffu : ((1u << T.ks) - 1u);
-    for (int m = 0; m < T.mt; m++) h_tile_mask[(size_t)slice * T.mt + m] = full;
-    B200_CUDA(cudaMemcpyAsync(tile_mask.p + (size_t)slice * T.mt, &h_tile_mask[(size_t)slice * T.mt], (size_t)T.mt * 4,
-                              cudaMemcpyHostToDevice, s));
-  }
-};
 
 struct b200pir_pp {
   b200pir_ctx* ctx;
@@ -317,11 +75,6 @@ PpTable b200pir_ctx::pp_table(b200pir_pp* pp, size_t count) {
 }
 
 namespace {
-
-struct Guard {
-  std::lock_guard<std::recursive_mutex> lk;
-  explicit Guard(b200pir_ctx* c) : lk(c->mu) { cudaSetDevice(c->device); }
-};
 
 // `words` u64 host words of NTT form (each < 2^32) into the ntt32 device words `dst`, on the context's stream, staged through
 // `wide`, which must live until the caller has synchronised
@@ -544,14 +297,6 @@ void run_pack_encode(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* folded, siz
   }
 }
 
-// handles may be used from any context with identical parameters on the same device (one context per host
-// thread / CUDA stream sharing one HBM-resident database)
-bool same_params(const b200pir_ctx* a, const b200pir_ctx* b) {
-  return a == b || (a->device == b->device && std::memcmp(&a->hp, &b->hp, sizeof(b200pir_params)) == 0);
-}
-void check_db(b200pir_ctx* c, b200pir_db* db) {
-  if (!db || !same_params(db->ctx, c)) throw Error(B200PIR_E_BADARG, "db handle was created for different parameters / device");
-}
 void check_pp(b200pir_ctx* c, b200pir_pp* pp) {
   if (!pp || !same_params(pp->ctx, c)) throw Error(B200PIR_E_BADARG, "pp handle was created for different parameters / device");
 }
@@ -591,6 +336,8 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   c->num_per = 1 << hp.nu_2;
   c->trials = (int)(hp.n * hp.n);
   c->slices = (int)(hp.instances * c->trials);
+  c->slice_words = (size_t)c->dim0 * c->num_per * POLY;
+  c->bytes_per_chunk = (hp.db_item_size + c->slices - 1) / c->slices;
   c->g = (int)log2_ceil_u64(hp.t_gsw * hp.nu_2 + c->dim0);
   c->stop_round = hp.nu_2 ? (int)log2_ceil_u64(hp.t_gsw * hp.nu_2) : 0;
   if (c->g > 11) throw Error(B200PIR_E_UNSUPPORTED, "expansion needs more than 2048 slots");
@@ -759,397 +506,6 @@ int b200pir_ctx_sizes(b200pir_ctx* c, uint64_t* setup_bytes, uint64_t* query_byt
   API_END
 }
 
-// ---------------------------------------------------------------- database
-int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, b200pir_db** out) {
-  API_BEGIN
-  if (!c || !out) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  if (shard_count == 0) { shard_count = 1; shard_index = 0; }
-  if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)c->num_per % shard_count)
-    throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
-  std::unique_ptr<b200pir_db> db(new b200pir_db());
-  db->ctx = c;
-  db->shard = Shard{(int)shard_index, (int)shard_count};
-  db->rows = c->num_per / (int)shard_count;
-  DbLayout& L = db->layout;
-  L.G = c->geom(db->rows);
-  L.F = make_imma_geom(c->dim0, db->rows);
-  L.T = make_tc5_geom(c->dim0, db->rows);
-  L.format = c->db_format >= 0 ? c->db_format : (tc5_supported(L.T) ? 2 : 1);
-  db->presence_init();
-  if (L.format == 2 && !tc5_supported(L.T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
-  db->store.alloc(db_bytes(L, c->slices));
-  L.base = db->store.p;
-  B200_CUDA(cudaMemsetAsync(db->store.p, 0, db->store.n, c->stream));
-  B200_CUDA(cudaStreamSynchronize(c->stream));
-  *out = db.release();
-  API_END
-}
-void b200pir_db_destroy(b200pir_db* db) {
-  if (!db) return;
-  cudaSetDevice(db->ctx->device);
-  delete db;
-}
-extern "C++" {
-namespace {
-// One slice in the reference's z-major layout, delivered chunk by chunk: fetch(word_offset, n_words) returns a host pointer
-// to that range of the slice (valid until the next call).
-template <typename Fetch>
-void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fetch) {
-  // reference layout is z-major: stage a range of z at a time in the writers' staging (w_wbytes, at least 64 MiB).  An export
-  // may still be copying its last chunk out of it; that copy is queued on the context's stream, ahead of this upload's copies.
-  const size_t per_z = (size_t)c->dim0 * c->num_per;
-  int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
-  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, per_z * zc * 8));
-  uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
-  for (int z0 = 0; z0 < POLY; z0 += zc) {
-    int cur = std::min(zc, POLY - z0);
-    const uint64_t* src = fetch((size_t)z0 * per_z, per_z * cur);
-    B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, c->stream));
-    launch_db_import(db->layout, db->shard, (int)slice, stage, z0, cur, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  db->mark_slice((int)slice, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));
-  B200_CUDA(cudaGetLastError());
-}
-
-// Stage `span` raw bytes from host memory `host` and write the `count` items that lie in them (ItemWrite offsets are relative
-// to `host`): one conversion-and-placement launch over (item, slice).  Presence is the caller's.  Stream-ordered: the staging
-// buffers are only overwritten by the next group's copies, which run after this launch.
-void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
-  if (count == 0) return;
-  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
-  c->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, count));
-  if (span) B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, host, span, cudaMemcpyHostToDevice, c->stream));
-  B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
-  const size_t chunks = (size_t)c->slices;
-  const size_t bpc = (c->hp.db_item_size + chunks - 1) / chunks;             // params.bytes_per_chunk()
-  launch_write_items(c->dp, db->layout, c->w_wbytes.p, c->w_witems.p, (int)count, (int)chunks, (int)bpc, c->hp.p, c->stream);
-}
-
-// Database export, shared by b200pir_db_download(_slice) and b200pir_db_save_file.  A chunk is one slice and a range of z of
-// the local rows, at most the writers' 64 MiB device staging (w_wbytes).  Under the context lock one launch un-tiles it into
-// [zc][rows][dim0] u64 there and the chunk is queued for a copy to one of the two pinned buffers; the lock is then released and
-// `sink(slice, z0, zc, words)` consumes the previous chunk once its copy has landed, while the GPU un-tiles and copies this
-// one.  Everything is ordered on the context's stream, so a chunk's un-tiling never overwrites staging its copy still reads.
-template <typename Sink>
-void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
-  std::lock_guard<std::mutex> ex(c->export_mu);
-  const size_t per_z = (size_t)db->rows * c->dim0;
-  const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
-  struct Chunk { int slice, z0, zc; };
-  std::vector<Chunk> chunks;
-  for (int s = slice_begin; s < slice_end; s++)
-    for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
-  {
-    Guard gd(c);
-    c->ensure_export_staging(per_z * zc * 8);
-  }
-  auto consume = [&](size_t k) {
-    const int b = (int)(k & 1);
-    B200_CUDA(cudaEventSynchronize(c->export_done[b]));
-    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<const uint64_t*>(c->h_export[b]));
-  };
-  try {
-    for (size_t k = 0; k < chunks.size(); k++) {
-      {
-        Guard gd(c);
-        uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
-        launch_db_export(db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
-        B200_CUDA(cudaMemcpyAsync(c->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, c->stream));
-        B200_CUDA(cudaEventRecord(c->export_done[k & 1], c->stream));
-      }
-      if (k > 0) consume(k - 1);
-    }
-    if (!chunks.empty()) consume(chunks.size() - 1);
-  } catch (...) {
-    for (auto e : c->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
-    throw;
-  }
-  B200_CUDA(cudaGetLastError());
-}
-
-// the local rows of slices [slice_begin, slice_end) into `words` (the reference layout of those slices): ii = il * G + index
-void download_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, uint64_t* words) {
-  const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per, rows = (size_t)db->rows;
-  const size_t G = (size_t)db->shard.count, gi = (size_t)db->shard.index;
-  const size_t slice_words = d0 * npg * POLY;
-  export_impl(c, db, slice_begin, slice_end, [&](int s, int z0, int zc, const uint64_t* src) {
-    uint64_t* dst = words + (size_t)(s - slice_begin) * slice_words + (size_t)z0 * npg * d0;
-    if (G == 1) { std::memcpy(dst, src, (size_t)zc * rows * d0 * 8); return; }
-    for (size_t zl = 0; zl < (size_t)zc; zl++)
-      for (size_t il = 0; il < rows; il++)
-        std::memcpy(dst + (zl * npg + il * G + gi) * d0, src + (zl * rows + il) * d0, d0 * 8);
-  });
-}
-}  // namespace
-}  // extern "C++"
-
-int b200pir_db_upload_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, const uint64_t* words, size_t n_words) {
-  API_BEGIN
-  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  const size_t slice_words = (size_t)c->dim0 * c->num_per * POLY;
-  if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
-  if (n_words != slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
-  upload_slice_impl(c, db, slice, [&](size_t off, size_t) { return words + off; });
-  API_END
-}
-// load_preprocessed_db_from_file (lib/spiral-rs/src/server.rs:373-386, lib/server/src/db/loading.rs:263-276): the file is the
-// native-endian u64 stream of the whole `db: &[u64]`; it is streamed through a 64 MiB staging buffer, never held in RAM.
-int b200pir_db_load_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
-  API_BEGIN
-  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  const size_t slice_words = (size_t)c->dim0 * c->num_per * POLY;
-  struct Closer { FILE* f; ~Closer() { if (f) fclose(f); } } file{fopen(path, "rb")};
-  if (!file.f) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
-  if (fseeko(file.f, 0, SEEK_END)) throw Error(B200PIR_E_BADARG, "cannot seek in the database file");
-  const off_t bytes = ftello(file.f);
-  if (bytes < 0 || (uint64_t)bytes != (uint64_t)slice_words * c->slices * 8)
-    throw Error(B200PIR_E_SHAPE, "database file must hold slices*dim0*num_per*2048 u64 words");
-  std::vector<uint64_t> buf;
-  for (int s = 0; s < c->slices; s++) {
-    upload_slice_impl(c, db, (uint64_t)s, [&](size_t off, size_t n) -> const uint64_t* {
-      buf.resize(n);
-      if (fseeko(file.f, (off_t)(((size_t)s * slice_words + off) * 8), SEEK_SET) || fread(buf.data(), 8, n, file.f) != n)
-        throw Error(B200PIR_E_SHAPE, "short read from the database file");
-      return buf.data();
-    });
-  }
-  API_END
-}
-int b200pir_db_upload(b200pir_ctx* c, b200pir_db* db, const uint64_t* words, size_t n_words) {
-  if (!c) { g_last_error = "null ctx"; return B200PIR_E_BADARG; }
-  const size_t slice_words = (size_t)c->dim0 * c->num_per * POLY;
-  if (n_words != slice_words * c->slices) { g_last_error = "db must hold slices*dim0*num_per*2048 words"; return B200PIR_E_SHAPE; }
-  for (int s = 0; s < c->slices; s++) {
-    int rc = b200pir_db_upload_slice(c, db, s, words + (size_t)s * slice_words, slice_words);
-    if (rc) return rc;
-  }
-  return 0;
-}
-int b200pir_db_download_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t* words, size_t n_words) {
-  API_BEGIN
-  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
-  check_db(c, db);
-  const size_t slice_words = (size_t)c->dim0 * c->num_per * POLY;
-  if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
-  if (n_words != slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
-  download_impl(c, db, (int)slice, (int)slice + 1, words);
-  API_END
-}
-int b200pir_db_download(b200pir_ctx* c, b200pir_db* db, uint64_t* words, size_t n_words) {
-  API_BEGIN
-  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
-  check_db(c, db);
-  if (n_words != (size_t)c->dim0 * c->num_per * POLY * c->slices) throw Error(B200PIR_E_SHAPE, "db must hold slices*dim0*num_per*2048 words");
-  download_impl(c, db, 0, c->slices, words);
-  API_END
-}
-// The file b200pir_db_load_file reads, written atomically: a temporary file in the target's directory is written chunk by
-// chunk (an unsharded chunk is a contiguous run of the file), flushed to disk and renamed over `path`; on any failure it is
-// removed, so `path` holds either its earlier content or the complete new snapshot.
-int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
-  API_BEGIN
-  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
-  check_db(c, db);
-  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
-  const std::string target(path);
-  std::string tmp = target + ".tmp.XXXXXX";
-  const int fd = mkstemp(&tmp[0]);
-  if (fd < 0) throw Error(B200PIR_E_BADARG, "cannot create a temporary file next to " + target + ": " + std::strerror(errno));
-  FILE* f = fdopen(fd, "wb");
-  if (!f) close(fd);
-  // drop the temporary file and report `why`: `path` is left as it was
-  auto discard = [&](const std::string& why, int code) {
-    if (f) fclose(f);
-    f = nullptr;
-    unlink(tmp.c_str());
-    throw Error(code, code == B200PIR_E_BADARG ? "cannot write " + target + ": " + why : why);
-  };
-  if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
-  try {
-    export_impl(c, db, 0, c->slices, [&](int, int, int zc, const uint64_t* src) {
-      const size_t n = (size_t)zc * db->rows * c->dim0;
-      if (fwrite(src, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
-    });
-  } catch (const Error& e) {
-    discard(e.what(), e.code);
-  } catch (const std::exception& e) {
-    discard(e.what(), B200PIR_E_CUDA);
-  }
-  if (fflush(f) != 0 || fsync(fileno(f)) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  const int closed = fclose(f);
-  f = nullptr;
-  if (closed != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  if (rename(tmp.c_str(), target.c_str()) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  // make the rename itself durable
-  const size_t slash = target.find_last_of('/');
-  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : target.substr(0, slash));
-  const int dfd = open(dir.c_str(), O_RDONLY);
-  if (dfd >= 0) { fsync(dfd); close(dfd); }
-  API_END
-}
-int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
-  API_BEGIN
-  if (!c || !poly) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  if (slice >= (uint64_t)c->slices || item_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "index out of range");
-  int ii = (int)(item_idx % c->num_per), j = (int)(item_idx / c->num_per);
-  if (ii % db->shard.count != db->shard.index) return 0;           // row lives on another GPU
-  DevBuf<uint64_t> tmp(POLY);
-  B200_CUDA(cudaMemcpyAsync(tmp.p, poly, POLY * 8, cudaMemcpyHostToDevice, c->stream));
-  launch_db_upsert(db->layout, (int)slice, ii / db->shard.count, j, tmp.p, c->stream);
-  db->mark((int)slice, ii / db->shard.count, j, c->stream);
-  // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
-  B200_CUDA(cudaStreamSynchronize(c->stream));
-  API_END
-}
-int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, const uint8_t* data, size_t len) {
-  API_BEGIN
-  if (!c || (!data && len)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  const auto& hp = c->hp;
-  if (hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
-  const size_t chunks = (size_t)c->slices;
-  const size_t pt_len = (hp.db_item_size + chunks - 1) / chunks;            // params.bytes_per_chunk()
-  if (pt_len > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
-  if (len > chunks * pt_len) throw Error(B200PIR_E_SHAPE, "update longer than instances*n^2*bytes_per_chunk");   // loading.rs:308-310
-  if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
-  const int ii = (int)(db_idx % c->num_per), j = (int)(db_idx / c->num_per);
-  if (ii % db->shard.count != db->shard.index) return 0;                      // row lives on another GPU
-  const ItemWrite item{0, (uint32_t)len, (uint32_t)(ii / db->shard.count), (uint32_t)j};
-  write_items(c, db, data, len, &item, 1);
-  db->mark_items(&item, 1, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
-  B200_CUDA(cudaGetLastError());
-  API_END
-}
-
-// lib/server/src/db/loading.rs:361-377 update_many_items (the /update-row body).  The whole body is parsed on the host first
-// (update_body.hpp); the valid prefix is applied and the error of the first bad entry, if any, returned afterwards, which is
-// the database state the reference's entry-by-entry loop leaves.  Only the last occurrence of each db_idx is written, so how
-// the entries are split into staging groups cannot change the result.  Every shard checks every entry and writes its own rows.
-int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update) {
-  API_BEGIN
-  if (!c || (!body && len)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  const auto& hp = c->hp;
-  const size_t chunks = (size_t)c->slices;
-  const size_t pt_len = (hp.db_item_size + chunks - 1) / chunks;            // params.bytes_per_chunk()
-  const BodyParse parsed = parse_update_body(body, len, 4 + chunks * pt_len, (uint64_t)c->dim0 * c->num_per);
-  // the reference reaches convert_pt_to_poly, which asserts logp == 8 (loading.rs:291), at the first well-formed entry
-  if (hp.p != 256 && !parsed.entries.empty()) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
-  if (pt_len > (size_t)POLY && !parsed.entries.empty()) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
-  const std::vector<BodyEntry> kept = keep_last_occurrence(parsed.entries);
-  std::vector<ItemWrite> all, group;
-  for (size_t k = 0; k < kept.size();) {
-    // one staging group: whole entries in body order, their bytes (dropped duplicates in between included) within the budget
-    const size_t k0 = k, base = kept[k].data_pos();
-    size_t end = base;
-    group.clear();
-    for (; k < kept.size() && group.size() < b200pir_ctx::kWriteStageItems; k++) {
-      const size_t e = kept[k].data_pos() + kept[k].data_len();
-      if (k > k0 && e - base > b200pir_ctx::kWriteStageBytes) break;
-      end = e;
-      const int ii = (int)(kept[k].db_idx % c->num_per), j = (int)(kept[k].db_idx / c->num_per);
-      if (ii % db->shard.count != db->shard.index) continue;                   // row lives on another GPU
-      group.push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)(ii / db->shard.count), (uint32_t)j});
-    }
-    write_items(c, db, body + base, end - base, group.data(), group.size());
-    all.insert(all.end(), group.begin(), group.end());
-  }
-  db->mark_items(all.data(), all.size(), c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
-  B200_CUDA(cudaGetLastError());
-  if (parsed.error) throw Error(parsed.error, parsed.message);
-  if (largest_update) *largest_update = parsed.largest_update;
-  API_END
-}
-
-// load_db_from_seek (lib/spiral-rs/src/server.rs:277-357; lib/server/src/db/loading.rs:192-247): `path` is the raw database,
-// item i at byte i * db_item_size.  Chunk c of item i is the bytes_per_chunk bytes at i * db_item_size + c * bytes_per_chunk,
-// clipped at the end of the FILE (as the reference's read does), each byte one plaintext coefficient; items past the end
-// of the file are zero polynomials.  The file is read in groups of whole items (one read and one conversion-and-placement
-// launch per group, within the writers' staging budget); an item's bytes may overlap the next item's, as its chunks do.
-int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
-  API_BEGIN
-  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  const auto& hp = c->hp;
-  if (hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "load_item_from_seek is restated for logp == 8 only");
-  const size_t chunks = (size_t)c->slices;
-  const size_t bpc = (hp.db_item_size + chunks - 1) / chunks;                // params.bytes_per_chunk()
-  if (bpc > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");     // server.rs:292
-  struct Closer { FILE* f; ~Closer() { if (f) fclose(f); } } file{fopen(path, "rb")};
-  if (!file.f) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
-  if (fseeko(file.f, 0, SEEK_END)) throw Error(B200PIR_E_BADARG, "cannot seek in the database file");
-  const off_t fbytes = ftello(file.f);
-  if (fbytes < 0) throw Error(B200PIR_E_BADARG, "cannot size the database file");
-  const size_t flen = (size_t)fbytes;
-  const size_t num_items = (size_t)c->dim0 * c->num_per;
-  const size_t item_span = chunks * bpc, isz = hp.db_item_size;
-  const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems,
-                                                    b200pir_ctx::kWriteStageBytes / std::max<size_t>(1, std::max(isz, item_span))));
-  std::vector<uint8_t> host;
-  std::vector<ItemWrite> items;
-  for (size_t i0 = 0; i0 < num_items; i0 += group) {
-    const size_t cnt = std::min(group, num_items - i0);
-    const size_t lo = i0 * isz, hi = std::min(flen, (i0 + cnt - 1) * isz + item_span);
-    const size_t span = hi > lo ? hi - lo : 0;
-    host.resize(span);
-    if (span && (fseeko(file.f, (off_t)lo, SEEK_SET) || fread(host.data(), 1, span, file.f) != span))
-      throw Error(B200PIR_E_SHAPE, "short read from the database file");
-    items.clear();
-    for (size_t k = 0; k < cnt; k++) {
-      const size_t idx = i0 + k, pos = idx * isz;
-      const int ii = (int)(idx % c->num_per), j = (int)(idx / c->num_per);
-      if (ii % db->shard.count != db->shard.index) continue;                  // row lives on another GPU
-      const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0;   // clipped at the end of the file
-      items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)(ii / db->shard.count), (uint32_t)j});
-    }
-    write_items(c, db, host.data(), span, items.data(), items.size());        // pageable `host`: staged before the call returns
-  }
-  for (int s = 0; s < c->slices; s++) db->mark_slice(s, c->stream);            // load_db_from_seek builds a dense database
-  B200_CUDA(cudaStreamSynchronize(c->stream));
-  B200_CUDA(cudaGetLastError());
-  API_END
-}
-
-int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity) {
-  API_BEGIN
-  if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  if (items) *items = db->present_count;
-  if (capacity) *capacity = db->capacity();
-  API_END
-}
-int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes) {
-  API_BEGIN
-  if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  if (format) *format = db->layout.format;
-  if (local_rows) *local_rows = (uint64_t)db->rows;
-  if (hbm_bytes) *hbm_bytes = (uint64_t)db->store.n;
-  API_END
-}
-int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
-  API_BEGIN
-  if (!c) throw Error(B200PIR_E_BADARG, "null ctx");
-  Guard gd(c);
-  check_db(c, db);
-  launch_write_synthetic(c->dp, db->layout, db->shard, seed, c->hp.p, c->stream);
-  for (int s0 = 0; s0 < c->slices; s0++) db->mark_slice(s0, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));
-  B200_CUDA(cudaGetLastError());
-  API_END
-}
 
 // ---------------------------------------------------------------- public parameters
 int b200pir_pp_create(b200pir_ctx* c, const uint64_t* v_packing, const uint64_t* left, const uint64_t* right,

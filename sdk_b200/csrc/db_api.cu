@@ -1,0 +1,428 @@
+// C-ABI implementation of the HBM-resident database handle (include/b200pir.h): creation, bulk uploads and file loads,
+// exports, the item writers and the presence map.  Every writer places items through the same three decisions: which GPU owns
+// an item (Shard::local_item), the context's write staging (w_wbytes) and the presence update (mark_items / mark_slices).
+#include "spiral_api.hpp"
+#include "update_body.hpp"
+#include <cstdio>
+#include <cerrno>
+#include <fcntl.h>
+#include <unistd.h>
+#include <memory>
+#include <utility>
+
+// ---------------------------------------------------------------- presence
+// every item of `items` written in slices [slice_begin, slice_end): one upload of the whole mask when any word changed
+void b200pir_db::mark_items(const ItemWrite* items, size_t count, int slice_begin, int slice_end, cudaStream_t s) {
+  bool changed = false;
+  for (size_t k = 0; k < count; k++)
+    for (int sl = slice_begin; sl < slice_end; sl++) {
+      const uint64_t bit = ((uint64_t)sl * rows + items[k].il) * ctx->dim0 + items[k].j;
+      if (!((present[bit >> 6] >> (bit & 63)) & 1)) { present[bit >> 6] |= 1ull << (bit & 63); present_count++; }
+      uint32_t& w = h_tile_mask[(size_t)sl * layout.T.mt + (items[k].il >> 5)];
+      const uint32_t nv = w | (1u << (items[k].j >> 5));
+      changed |= nv != w;
+      w = nv;
+    }
+  if (changed)
+    B200_CUDA(cudaMemcpyAsync(tile_mask.p, h_tile_mask.data(), h_tile_mask.size() * 4, cudaMemcpyHostToDevice, s));
+}
+// whole slices [slice_begin, slice_end) written at once (bulk upload, file load, synthetic fill): every item of them exists
+// from now on
+void b200pir_db::mark_slices(int slice_begin, int slice_end, cudaStream_t s) {
+  const uint64_t lo = (uint64_t)slice_begin * rows * ctx->dim0, hi = (uint64_t)slice_end * rows * ctx->dim0;
+  for (uint64_t b = lo; b < hi; b++)
+    if (!((present[b >> 6] >> (b & 63)) & 1)) { present[b >> 6] |= 1ull << (b & 63); present_count++; }
+  const Tc5Geom& T = layout.T;
+  const uint32_t full = T.ks >= 32 ? 0xffffffffu : ((1u << T.ks) - 1u);
+  const size_t w0 = (size_t)slice_begin * T.mt, w1 = (size_t)slice_end * T.mt;
+  for (size_t w = w0; w < w1; w++) h_tile_mask[w] = full;
+  B200_CUDA(cudaMemcpyAsync(tile_mask.p + w0, &h_tile_mask[w0], (w1 - w0) * 4, cudaMemcpyHostToDevice, s));
+}
+
+namespace {
+
+// One slice in the reference's z-major layout, delivered chunk by chunk: fetch(word_offset, n_words) returns a host pointer
+// to that range of the slice (valid until the next call).
+template <typename Fetch>
+void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fetch) {
+  // reference layout is z-major: stage a range of z at a time in the writers' staging (w_wbytes, at least 64 MiB).  An export
+  // may still be copying its last chunk out of it; that copy is queued on the context's stream, ahead of this upload's copies.
+  const size_t per_z = (size_t)c->dim0 * c->num_per;
+  int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
+  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, per_z * zc * 8));
+  uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
+  for (int z0 = 0; z0 < POLY; z0 += zc) {
+    int cur = std::min(zc, POLY - z0);
+    const uint64_t* src = fetch((size_t)z0 * per_z, per_z * cur);
+    B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, c->stream));
+    launch_db_import(db->layout, db->shard, (int)slice, stage, z0, cur, c->stream);
+    B200_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  db->mark_slices((int)slice, (int)slice + 1, c->stream);
+  B200_CUDA(cudaStreamSynchronize(c->stream));
+  B200_CUDA(cudaGetLastError());
+}
+
+// Stage `span` raw bytes from host memory `host` and write the `count` items that lie in them (ItemWrite offsets are relative
+// to `host`): one conversion-and-placement launch over (item, slice).  Presence is the caller's.  Stream-ordered: the staging
+// buffers are only overwritten by the next group's copies, which run after this launch.
+void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
+  if (count == 0) return;
+  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
+  c->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, count));
+  if (span) B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, host, span, cudaMemcpyHostToDevice, c->stream));
+  B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
+  launch_write_items(c->dp, db->layout, c->w_wbytes.p, c->w_witems.p, (int)count, c->slices, (int)c->bytes_per_chunk, c->hp.p, c->stream);
+}
+
+// Database export, shared by b200pir_db_download(_slice) and b200pir_db_save_file.  A chunk is one slice and a range of z of
+// the local rows, at most the writers' 64 MiB device staging (w_wbytes).  Under the context lock one launch un-tiles it into
+// [zc][rows][dim0] u64 there and the chunk is queued for a copy to one of the two pinned buffers; the lock is then released and
+// `sink(slice, z0, zc, words)` consumes the previous chunk once its copy has landed, while the GPU un-tiles and copies this
+// one.  Everything is ordered on the context's stream, so a chunk's un-tiling never overwrites staging its copy still reads.
+template <typename Sink>
+void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
+  std::lock_guard<std::mutex> ex(c->export_mu);
+  const size_t per_z = (size_t)db->rows * c->dim0;
+  const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
+  struct Chunk { int slice, z0, zc; };
+  std::vector<Chunk> chunks;
+  for (int s = slice_begin; s < slice_end; s++)
+    for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
+  {
+    Guard gd(c);
+    c->ensure_export_staging(per_z * zc * 8);
+  }
+  auto consume = [&](size_t k) {
+    const int b = (int)(k & 1);
+    B200_CUDA(cudaEventSynchronize(c->export_done[b]));
+    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<const uint64_t*>(c->h_export[b]));
+  };
+  try {
+    for (size_t k = 0; k < chunks.size(); k++) {
+      {
+        Guard gd(c);
+        uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
+        launch_db_export(db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
+        B200_CUDA(cudaMemcpyAsync(c->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, c->stream));
+        B200_CUDA(cudaEventRecord(c->export_done[k & 1], c->stream));
+      }
+      if (k > 0) consume(k - 1);
+    }
+    if (!chunks.empty()) consume(chunks.size() - 1);
+  } catch (...) {
+    for (auto e : c->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
+    throw;
+  }
+  B200_CUDA(cudaGetLastError());
+}
+
+// the local rows of slices [slice_begin, slice_end) into `words` (the reference layout of those slices)
+void download_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, uint64_t* words) {
+  const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per, rows = (size_t)db->rows;
+  export_impl(c, db, slice_begin, slice_end, [&](int s, int z0, int zc, const uint64_t* src) {
+    uint64_t* dst = words + (size_t)(s - slice_begin) * c->slice_words + (size_t)z0 * npg * d0;
+    if (db->shard.count == 1) { std::memcpy(dst, src, (size_t)zc * rows * d0 * 8); return; }
+    for (size_t zl = 0; zl < (size_t)zc; zl++)
+      for (size_t il = 0; il < rows; il++)
+        std::memcpy(dst + (zl * npg + db->shard.global_row(il)) * d0, src + (zl * rows + il) * d0, d0 * 8);
+  });
+}
+
+// `path` opened for reading, and its size (ftello: negative when it cannot be told)
+std::pair<std::unique_ptr<FILE, int (*)(FILE*)>, off_t> open_sized(const char* path) {
+  std::unique_ptr<FILE, int (*)(FILE*)> f(fopen(path, "rb"), fclose);
+  if (!f) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
+  if (fseeko(f.get(), 0, SEEK_END)) throw Error(B200PIR_E_BADARG, "cannot seek in the database file");
+  const off_t bytes = ftello(f.get());
+  return {std::move(f), bytes};
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, b200pir_db** out) {
+  API_BEGIN
+  if (!c || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  if (shard_count == 0) { shard_count = 1; shard_index = 0; }
+  if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)c->num_per % shard_count)
+    throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+  std::unique_ptr<b200pir_db> db(new b200pir_db());
+  db->ctx = c;
+  db->shard = Shard{(int)shard_index, (int)shard_count};
+  db->rows = c->num_per / (int)shard_count;
+  DbLayout& L = db->layout;
+  L.G = c->geom(db->rows);
+  L.F = make_imma_geom(c->dim0, db->rows);
+  L.T = make_tc5_geom(c->dim0, db->rows);
+  L.format = c->db_format >= 0 ? c->db_format : (tc5_supported(L.T) ? 2 : 1);
+  db->present.assign((db->capacity() + 63) / 64, 0);
+  db->h_tile_mask.assign((size_t)c->slices * L.T.mt, 0u);
+  db->tile_mask.alloc(db->h_tile_mask.size());
+  // on the context's stream: a cudaMemset would queue on the legacy default stream, behind whatever the caller has there,
+  // and could land after the first writer's mask upload on the context's stream
+  B200_CUDA(cudaMemsetAsync(db->tile_mask.p, 0, db->h_tile_mask.size() * 4, c->stream));
+  if (L.format == 2 && !tc5_supported(L.T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
+  db->store.alloc(db_bytes(L, c->slices));
+  L.base = db->store.p;
+  B200_CUDA(cudaMemsetAsync(db->store.p, 0, db->store.n, c->stream));
+  B200_CUDA(cudaStreamSynchronize(c->stream));
+  *out = db.release();
+  API_END
+}
+void b200pir_db_destroy(b200pir_db* db) {
+  if (!db) return;
+  cudaSetDevice(db->ctx->device);
+  delete db;
+}
+
+int b200pir_db_upload_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, const uint64_t* words, size_t n_words) {
+  API_BEGIN
+  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
+  if (n_words != c->slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
+  upload_slice_impl(c, db, slice, [&](size_t off, size_t) { return words + off; });
+  API_END
+}
+// load_preprocessed_db_from_file (lib/spiral-rs/src/server.rs:373-386, lib/server/src/db/loading.rs:263-276): the file is the
+// native-endian u64 stream of the whole `db: &[u64]`; it is streamed through a 64 MiB staging buffer, never held in RAM.
+int b200pir_db_load_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
+  API_BEGIN
+  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  const auto [file, bytes] = open_sized(path);
+  if (bytes < 0 || (uint64_t)bytes != (uint64_t)c->slice_words * c->slices * 8)
+    throw Error(B200PIR_E_SHAPE, "database file must hold slices*dim0*num_per*2048 u64 words");
+  std::vector<uint64_t> buf;
+  for (int s = 0; s < c->slices; s++) {
+    upload_slice_impl(c, db, (uint64_t)s, [&, f = file.get()](size_t off, size_t n) -> const uint64_t* {
+      buf.resize(n);
+      if (fseeko(f, (off_t)(((size_t)s * c->slice_words + off) * 8), SEEK_SET) || fread(buf.data(), 8, n, f) != n)
+        throw Error(B200PIR_E_SHAPE, "short read from the database file");
+      return buf.data();
+    });
+  }
+  API_END
+}
+int b200pir_db_upload(b200pir_ctx* c, b200pir_db* db, const uint64_t* words, size_t n_words) {
+  if (!c) { g_last_error = "null ctx"; return B200PIR_E_BADARG; }
+  if (n_words != c->slice_words * c->slices) { g_last_error = "db must hold slices*dim0*num_per*2048 words"; return B200PIR_E_SHAPE; }
+  for (int s = 0; s < c->slices; s++) {
+    int rc = b200pir_db_upload_slice(c, db, s, words + (size_t)s * c->slice_words, c->slice_words);
+    if (rc) return rc;
+  }
+  return 0;
+}
+int b200pir_db_download_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t* words, size_t n_words) {
+  API_BEGIN
+  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
+  if (n_words != c->slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
+  download_impl(c, db, (int)slice, (int)slice + 1, words);
+  API_END
+}
+int b200pir_db_download(b200pir_ctx* c, b200pir_db* db, uint64_t* words, size_t n_words) {
+  API_BEGIN
+  if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  if (n_words != c->slice_words * c->slices) throw Error(B200PIR_E_SHAPE, "db must hold slices*dim0*num_per*2048 words");
+  download_impl(c, db, 0, c->slices, words);
+  API_END
+}
+// The file b200pir_db_load_file reads, written atomically: a temporary file in the target's directory is written chunk by
+// chunk (an unsharded chunk is a contiguous run of the file), flushed to disk and renamed over `path`; on any failure it is
+// removed, so `path` holds either its earlier content or the complete new snapshot.
+int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
+  API_BEGIN
+  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
+  const std::string target(path);
+  std::string tmp = target + ".tmp.XXXXXX";
+  const int fd = mkstemp(&tmp[0]);
+  if (fd < 0) throw Error(B200PIR_E_BADARG, "cannot create a temporary file next to " + target + ": " + std::strerror(errno));
+  FILE* f = fdopen(fd, "wb");
+  if (!f) close(fd);
+  // drop the temporary file and report `why`: `path` is left as it was
+  auto discard = [&](const std::string& why, int code) {
+    if (f) fclose(f);
+    f = nullptr;
+    unlink(tmp.c_str());
+    throw Error(code, code == B200PIR_E_BADARG ? "cannot write " + target + ": " + why : why);
+  };
+  if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
+  try {
+    export_impl(c, db, 0, c->slices, [&](int, int, int zc, const uint64_t* src) {
+      const size_t n = (size_t)zc * db->rows * c->dim0;
+      if (fwrite(src, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
+    });
+  } catch (const Error& e) {
+    discard(e.what(), e.code);
+  } catch (const std::exception& e) {
+    discard(e.what(), B200PIR_E_CUDA);
+  }
+  if (fflush(f) != 0 || fsync(fileno(f)) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  const int closed = fclose(f);
+  f = nullptr;
+  if (closed != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  if (rename(tmp.c_str(), target.c_str()) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  // make the rename itself durable
+  const size_t slash = target.find_last_of('/');
+  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : target.substr(0, slash));
+  const int dfd = open(dir.c_str(), O_RDONLY);
+  if (dfd >= 0) { fsync(dfd); close(dfd); }
+  API_END
+}
+int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
+  API_BEGIN
+  if (!c || !poly) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  if (slice >= (uint64_t)c->slices || item_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "index out of range");
+  int il, j;
+  if (!db->shard.local_item(item_idx, c->num_per, il, j)) return 0;       // row lives on another GPU
+  c->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like write_items
+  B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, poly, POLY * 8, cudaMemcpyHostToDevice, c->stream));
+  launch_db_upsert(db->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(c->w_wbytes.p), c->stream);
+  const ItemWrite item{0, 0, (uint32_t)il, (uint32_t)j};
+  db->mark_items(&item, 1, (int)slice, (int)slice + 1, c->stream);
+  // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
+  B200_CUDA(cudaStreamSynchronize(c->stream));
+  API_END
+}
+int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, const uint8_t* data, size_t len) {
+  API_BEGIN
+  if (!c || (!data && len)) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
+  if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
+  if (len > (size_t)c->slices * c->bytes_per_chunk) throw Error(B200PIR_E_SHAPE, "update longer than instances*n^2*bytes_per_chunk");   // loading.rs:308-310
+  if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
+  int il, j;
+  if (!db->shard.local_item(db_idx, c->num_per, il, j)) return 0;         // row lives on another GPU
+  const ItemWrite item{0, (uint32_t)len, (uint32_t)il, (uint32_t)j};
+  write_items(c, db, data, len, &item, 1);
+  db->mark_items(&item, 1, 0, c->slices, c->stream);
+  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+// lib/server/src/db/loading.rs:361-377 update_many_items (the /update-row body).  The whole body is parsed on the host first
+// (update_body.hpp); the valid prefix is applied and the error of the first bad entry, if any, returned afterwards, which is
+// the database state the reference's entry-by-entry loop leaves.  Only the last occurrence of each db_idx is written, so how
+// the entries are split into staging groups cannot change the result.  Every shard checks every entry and writes its own rows.
+int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update) {
+  API_BEGIN
+  if (!c || (!body && len)) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  const BodyParse parsed = parse_update_body(body, len, 4 + (size_t)c->slices * c->bytes_per_chunk, (uint64_t)c->dim0 * c->num_per);
+  // the reference reaches convert_pt_to_poly, which asserts logp == 8 (loading.rs:291), at the first well-formed entry
+  if (c->hp.p != 256 && !parsed.entries.empty()) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
+  if (c->bytes_per_chunk > (size_t)POLY && !parsed.entries.empty()) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
+  const std::vector<BodyEntry> kept = keep_last_occurrence(parsed.entries);
+  std::vector<ItemWrite> all, group;
+  for (size_t k = 0; k < kept.size();) {
+    // one staging group: whole entries in body order, their bytes (dropped duplicates in between included) within the budget
+    const size_t k0 = k, base = kept[k].data_pos();
+    size_t end = base;
+    group.clear();
+    for (; k < kept.size() && group.size() < b200pir_ctx::kWriteStageItems; k++) {
+      const size_t e = kept[k].data_pos() + kept[k].data_len();
+      if (k > k0 && e - base > b200pir_ctx::kWriteStageBytes) break;
+      end = e;
+      int il, j;
+      if (!db->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
+      group.push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)il, (uint32_t)j});
+    }
+    write_items(c, db, body + base, end - base, group.data(), group.size());
+    all.insert(all.end(), group.begin(), group.end());
+  }
+  db->mark_items(all.data(), all.size(), 0, c->slices, c->stream);
+  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
+  B200_CUDA(cudaGetLastError());
+  if (parsed.error) throw Error(parsed.error, parsed.message);
+  if (largest_update) *largest_update = parsed.largest_update;
+  API_END
+}
+
+// load_db_from_seek (lib/spiral-rs/src/server.rs:277-357; lib/server/src/db/loading.rs:192-247): `path` is the raw database,
+// item i at byte i * db_item_size.  Chunk c of item i is the bytes_per_chunk bytes at i * db_item_size + c * bytes_per_chunk,
+// clipped at the end of the FILE (as the reference's read does), each byte one plaintext coefficient; items past the end
+// of the file are zero polynomials.  The file is read in groups of whole items (one read and one conversion-and-placement
+// launch per group, within the writers' staging budget); an item's bytes may overlap the next item's, as its chunks do.
+int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
+  API_BEGIN
+  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  check_db(c, db);
+  if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "load_item_from_seek is restated for logp == 8 only");
+  if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");     // server.rs:292
+  const auto [file, fbytes] = open_sized(path);
+  if (fbytes < 0) throw Error(B200PIR_E_BADARG, "cannot size the database file");
+  const size_t flen = (size_t)fbytes;
+  const size_t num_items = (size_t)c->dim0 * c->num_per;
+  const size_t item_span = (size_t)c->slices * c->bytes_per_chunk, isz = c->hp.db_item_size;
+  const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems,
+                                                    b200pir_ctx::kWriteStageBytes / std::max<size_t>(1, std::max(isz, item_span))));
+  std::vector<uint8_t> host;
+  std::vector<ItemWrite> items;
+  for (size_t i0 = 0; i0 < num_items; i0 += group) {
+    const size_t cnt = std::min(group, num_items - i0);
+    const size_t lo = i0 * isz, hi = std::min(flen, (i0 + cnt - 1) * isz + item_span);
+    const size_t span = hi > lo ? hi - lo : 0;
+    host.resize(span);
+    if (span && (fseeko(file.get(), (off_t)lo, SEEK_SET) || fread(host.data(), 1, span, file.get()) != span))
+      throw Error(B200PIR_E_SHAPE, "short read from the database file");
+    items.clear();
+    for (size_t k = 0; k < cnt; k++) {
+      const size_t idx = i0 + k, pos = idx * isz;
+      int il, j;
+      if (!db->shard.local_item(idx, c->num_per, il, j)) continue;           // row lives on another GPU
+      const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0;   // clipped at the end of the file
+      items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)il, (uint32_t)j});
+    }
+    write_items(c, db, host.data(), span, items.data(), items.size());        // pageable `host`: staged before the call returns
+  }
+  db->mark_slices(0, c->slices, c->stream);                                   // load_db_from_seek builds a dense database
+  B200_CUDA(cudaStreamSynchronize(c->stream));
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity) {
+  API_BEGIN
+  if (!db) throw Error(B200PIR_E_BADARG, "null db");
+  if (items) *items = db->present_count;
+  if (capacity) *capacity = db->capacity();
+  API_END
+}
+int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes) {
+  API_BEGIN
+  if (!db) throw Error(B200PIR_E_BADARG, "null db");
+  if (format) *format = db->layout.format;
+  if (local_rows) *local_rows = (uint64_t)db->rows;
+  if (hbm_bytes) *hbm_bytes = (uint64_t)db->store.n;
+  API_END
+}
+int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
+  API_BEGIN
+  if (!c) throw Error(B200PIR_E_BADARG, "null ctx");
+  Guard gd(c);
+  check_db(c, db);
+  launch_write_synthetic(c->dp, db->layout, db->shard, seed, c->hp.p, c->stream);
+  db->mark_slices(0, c->slices, c->stream);
+  B200_CUDA(cudaStreamSynchronize(c->stream));
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+}  // extern "C"

@@ -63,7 +63,17 @@ void launch_multiply(const DevParams& P, const MulGeom& G, const uint4* db_dev, 
 void launch_query_to_dev(const MulGeom& G, uint4* q_dev, const uint64_t* v_firstdim, cudaStream_t s);
 // Row sharding of the second-dimension index: this GPU holds global rows ii = il*count + index
 // (il = local row, G.num_per local rows).  index=0,count=1 is the whole database.
-struct Shard { int index, count; };
+struct Shard {
+  int index, count;
+  // global item idx = j * num_per_global + ii -> this GPU's local row il and column j; false when row ii lives on another GPU
+  bool local_item(uint64_t idx, int num_per_global, int& il, int& j) const {
+    const int ii = (int)(idx % num_per_global);
+    il = ii / count;
+    j = (int)(idx / num_per_global);
+    return ii % count == index;
+  }
+  size_t global_row(size_t il) const { return il * count + index; }      // the inverse: local row il -> global row ii
+};
 
 // ---- first dimension on INT8 tensor cores (imma_kernels.cu): database in MMA fragment order
 size_t imma_query_cells(const ImmaGeom& F);               // uint2 cells of the B operand (up to 16 queries)
