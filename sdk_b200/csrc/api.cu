@@ -53,28 +53,52 @@ struct b200pir_pp {
   DevBuf<uint32_t> pack, left, right, conv;    // ntt32
 };
 
-PpTable b200pir_ctx::pp_table(b200pir_pp* pp, size_t count) {
-  if (count > pptab_cap) {
-    pptab_cap = std::max<size_t>(count, 16);
-    d_pptab.alloc(4 * pptab_cap);
-    h_pptab.clear();
+namespace {
+
+// The public parameters of a call's queries: `each[i]` for query i (a multi-client batch) or, where `each` is null, `one` for
+// every query
+struct Keys {
+  b200pir_pp* one = nullptr;
+  b200pir_pp* const* each = nullptr;
+  b200pir_pp* operator[](size_t i) const { return each ? each[i] : one; }
+};
+
+// The context's per-query parameter table for queries [0, count) of `keys`; uploaded only when its contents change
+PpTable pp_table(b200pir_ctx* c, Keys keys, size_t count) {
+  size_t& cap = c->pptab_cap;
+  if (count > cap) {
+    cap = std::max<size_t>(count, 16);
+    c->d_pptab.alloc(4 * cap);
+    c->h_pptab.clear();
   }
-  std::vector<const uint32_t*> h(4 * pptab_cap, nullptr);
+  std::vector<const uint32_t*> h(4 * cap, nullptr);
   for (size_t i = 0; i < count; i++) {
-    const b200pir_pp* p = multi_pps ? multi_pps[i] : pp;
-    h[0 * pptab_cap + i] = p->pack.p;
-    h[1 * pptab_cap + i] = p->left.p;
-    h[2 * pptab_cap + i] = p->right.p ? p->right.p : p->left.p;     // unwrap_or(v_w_left), server.rs:549
-    h[3 * pptab_cap + i] = p->conv.p;
+    const b200pir_pp* p = keys[i];
+    h[0 * cap + i] = p->pack.p;
+    h[1 * cap + i] = p->left.p;
+    h[2 * cap + i] = p->right.p ? p->right.p : p->left.p;     // unwrap_or(v_w_left), server.rs:549
+    h[3 * cap + i] = p->conv.p;
   }
-  if (h != h_pptab) {
-    B200_CUDA(cudaMemcpyAsync(d_pptab.p, h.data(), h.size() * sizeof(const uint32_t*), cudaMemcpyHostToDevice, stream));
-    h_pptab = h;
+  if (h != c->h_pptab) {
+    B200_CUDA(cudaMemcpyAsync(c->d_pptab.p, h.data(), h.size() * sizeof(const uint32_t*), cudaMemcpyHostToDevice, c->stream));
+    c->h_pptab = h;
   }
-  return PpTable{d_pptab.p, d_pptab.p + pptab_cap, d_pptab.p + 2 * pptab_cap, d_pptab.p + 3 * pptab_cap};
+  const uint32_t* const* d = c->d_pptab.p;
+  return PpTable{d, d + cap, d + 2 * cap, d + 3 * cap};
 }
 
-namespace {
+// Where a fold left its survivors: the residue-form ciphertext of (query qi, slice t) at p + (qi * slices + t) * stride
+struct Survivors {
+  const uint32_t* p;
+  size_t stride;
+};
+
+// The first-dimension operand as tile images (format-2 databases): image g holds queries [g * per_group, (g + 1) * per_group),
+// per_group <= 16.  p == nullptr: no images, the operand is q_dev.
+struct Images {
+  const uint8_t* p;
+  size_t per_group;
+};
 
 // `words` u64 host words of NTT form (each < 2^32) into the ntt32 device words `dst`, on the context's stream, staged through
 // `wide`, which must live until the caller has synchronised
@@ -101,13 +125,13 @@ void upload_ntt32(b200pir_ctx* c, DevBuf<uint32_t>& dst, const uint64_t* host, s
 // ---- pipeline pieces (all stream-ordered, device pointers)
 
 // server.rs:19-121 over `nq` queries at once (v: [nq][2^g][4][2048], v_stride words apart)
-void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size_t v_stride, int nq, bool all_slots) {
+void run_coefficient_expansion(b200pir_ctx* c, Keys keys, uint32_t* v, size_t v_stride, int nq, bool all_slots) {
   const auto& hp = c->hp;
   cudaStream_t s = c->stream;
   const int g = c->g;
   const int stop_round = hp.nu_2 > 0 ? c->stop_round : 0;
   const int max_right = hp.nu_2 > 0 ? (int)(hp.t_gsw * hp.nu_2) : 0;
-  const PpTable T = c->pp_table(pp, (size_t)nq);
+  const PpTable T = pp_table(c, keys, (size_t)nq);
   for (int r = 0; r < g; r++) {
     const int num_in = 1 << r;
     ExpandRound R;
@@ -134,13 +158,13 @@ void run_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint32_t* v, size
 // server.rs:525-591 for `nq` queries.  v: [nq][2^g][4][2048]; writes v_fold of every query and the first-dimension operand:
 // q_dev (uint4 [query][dim0][2048], reorient_reg_ciphertexts util.rs:323-355) or, when `images` is given (format-2 databases),
 // the operand tile images of groups of 16 queries directly (image g = queries 16g .., tc5_query_bytes apart): no intermediate.
-void run_expand_query(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_raw, uint32_t* v, uint4* q_dev,
-                      uint32_t* v_fold, int nq, uint8_t* images = nullptr) {
+void run_expand_query(b200pir_ctx* c, Keys keys, const uint64_t* query_raw, uint32_t* v, uint4* q_dev, uint32_t* v_fold,
+                      int nq, uint8_t* images) {
   const auto& hp = c->hp;
   cudaStream_t s = c->stream;
   // no clear of v: every slot the query path reads (even slots < 2 dim0, odd slots < 2 t_gsw nu_2) is written by the rounds
   launch_to_ntt_strided(c->dp, v, c->v_words(), query_raw, (size_t)2 * POLY, 2, nq, s);   // v[0] = query.ct.ntt()
-  run_coefficient_expansion(c, pp, v, c->v_words(), nq, false);
+  run_coefficient_expansion(c, keys, v, c->v_words(), nq, false);
   const int factor = hp.nu_2 > 0 ? 2 : 1;
   if (images) {
     const Tc5Geom T = make_tc5_geom(c->dim0, 32);
@@ -151,7 +175,7 @@ void run_expand_query(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_raw,
     launch_reorient(c->geom(c->num_per), q_dev, (size_t)c->dim0 * POLY, v, c->v_words(), nq, factor, s);
   }
   if (hp.nu_2 > 0)
-    launch_regev_to_gsw(c->dp, v_fold, c->fold_words(), v, c->v_words(), nq, (int)hp.nu_2, 2, 1, c->pp_table(pp, (size_t)nq).conv,
+    launch_regev_to_gsw(c->dp, v_fold, c->fold_words(), v, c->v_words(), nq, (int)hp.nu_2, 2, 1, pp_table(c, keys, (size_t)nq).conv,
                         (int)hp.t_gsw, (int)hp.t_conv, c->bits_conv, c->live_conv, s);
 }
 
@@ -188,19 +212,19 @@ const uint32_t* run_fold_res(b200pir_ctx* c, uint32_t* a, uint32_t* b, size_t ba
 }
 
 // expansion (or direct upload) for `count` queries already in w_query / w_qdev,w_vfold
-void run_prepare(b200pir_ctx* c, b200pir_pp* pp, size_t count, bool images = false) {
+// (`images`: the expansion writes the first-dimension operand to w_qt as tile images, for a format-2 database)
+void run_prepare(b200pir_ctx* c, Keys keys, size_t count, bool images) {
   b200pir_ctx::Scope sc(c, ST_EXPAND);
   if (images) c->w_qt.ensure((count + 15) / 16 * tc5_query_bytes(make_tc5_geom(c->dim0, 32)));
   if (c->hp.expand_queries)
-    run_expand_query(c, pp, c->w_query.p, c->w_v.p, c->w_qdev.p, c->w_vfold.p, (int)count, images ? c->w_qt.p : nullptr);
+    run_expand_query(c, keys, c->w_query.p, c->w_v.p, c->w_qdev.p, c->w_vfold.p, (int)count, images ? c->w_qt.p : nullptr);
   // v_folding_neg (server.rs:680) is not materialised: the fold fast path uses G - C_k implicitly.
 }
 
-// The first-dimension product of `count` queries (operands qdev + qi * dim0 * POLY) over slices [slice_begin, slice_begin +
-// slice_count), into `out` (queries slices * rows * 4 * POLY words apart) in the form db->zmajor_product() names.
-// `images`: the operand already sits as tile images (format 2; groups of `per_group` <= 16 queries, one image each).
-void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, uint32_t* out, int slice_begin,
-                   int slice_count, const uint8_t* images = nullptr, size_t per_group = 16) {
+// The first-dimension product of `count` queries (operands qdev + qi * dim0 * POLY, or `images`) over slices [slice_begin,
+// slice_begin + slice_count), into `out` (queries slices * rows * 4 * POLY words apart) in the form db->zmajor_product() names.
+void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, Images images, uint32_t* out,
+                   int slice_begin, int slice_count) {
   const DbLayout& L = db->layout;
   const size_t q_stride = (size_t)c->dim0 * POLY;
   const size_t out_stride = (size_t)c->slices * db->rows * 4 * POLY;
@@ -219,12 +243,12 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
     }
   } else if (L.format == 2) {
     // wgmma path: same z-major product as the mma.sync path, 16 queries per database pass
-    if (!images) c->w_qt.ensure(tc5_query_bytes(L.T));
-    const size_t step = images ? per_group : 16;
+    if (!images.p) c->w_qt.ensure(tc5_query_bytes(L.T));
+    const size_t step = images.p ? images.per_group : 16;
     for (size_t qi = 0, g = 0; qi < count; qi += step, g++) {
       const int nq = (int)std::min<size_t>(step, count - qi);
-      const uint8_t* qt = images ? images + g * tc5_query_bytes(L.T) : c->w_qt.p;
-      if (!images) {
+      const uint8_t* qt = images.p ? images.p + g * tc5_query_bytes(L.T) : c->w_qt.p;
+      if (!images.p) {
         b200pir_ctx::Scope sq(c, ST_QIMG);
         launch_query_to_tc5(L.T, qdev + qi * q_stride, q_stride, nq, c->w_qt.p, c->stream);
       }
@@ -253,41 +277,34 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
   }
 }
 
-// first dimension + from_ntt + local fold.  Leaves survivors at w_cts[(qi*slices + slice)*rows*2*POLY].
-// `images`: the first-dimension operand already sits as tile images (groups of `per_group` <= 16 queries, one image each)
-void run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev = nullptr,
-                            const uint32_t* vfold = nullptr, const uint8_t* images = nullptr, size_t per_group = 16) {
-  if (!qdev) qdev = c->w_qdev.p;
-  if (!vfold) vfold = c->w_vfold.p;
+// first dimension (operand qdev or `images`) + from_ntt + local fold with the folding matrices vfold; returns the survivors
+// (in w_mult or w_cts), one per (query, slice)
+Survivors run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, Images images,
+                                 const uint32_t* vfold) {
   const int rows = db->rows;
   const size_t out_stride = (size_t)c->slices * rows * 4 * POLY;
   // server.rs:707-709 from_ntt, minus the CRT lift, into w_mult in residue form: a z-major product goes to w_cts (free until
   // the fold starts) and is inverse-transformed from there; an ntt32 product is inverse-transformed in place
   const bool zmajor = db->zmajor_product();
-  run_first_dim(c, db, count, qdev, zmajor ? c->w_cts.p : c->w_mult.p, 0, c->slices, images, per_group);
+  run_first_dim(c, db, count, qdev, images, zmajor ? c->w_cts.p : c->w_mult.p, 0, c->slices);
   {
     b200pir_ctx::Scope sc(c, ST_FROMNTT);
     if (zmajor) launch_intt_from_zmajor(c->dp, db->layout.F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
     else launch_ntt32(c->dp, c->w_mult.p, count * c->slices * rows * 2, true, c->stream);
   }
-  {
-    b200pir_ctx::Scope sc(c, ST_FOLD);
-    c->folded = c->w_mult.p;
-    c->folded_stride = (size_t)rows * 4 * POLY;
-    if (rows > 1)
-      c->folded = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, (size_t)rows * 4 * POLY, rows,
-                               (int)c->hp.nu_2 - 1, vfold, c->slices);
-  }
+  b200pir_ctx::Scope sc(c, ST_FOLD);
+  Survivors s{c->w_mult.p, (size_t)rows * 4 * POLY};
+  if (rows > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, rows, (int)c->hp.nu_2 - 1, vfold, c->slices);
+  return s;
 }
 
-// pack + encode for `count` queries whose folded ciphertexts sit at folded + ((qi*slices)+t)*ct_stride
-void run_pack_encode(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* folded, size_t ct_stride, size_t count,
-                     uint8_t* out_dev) {
+// pack + encode for `count` queries
+void run_pack_encode(b200pir_ctx* c, Keys keys, Survivors s, size_t count, uint8_t* out_dev) {
   const auto& hp = c->hp;
   const size_t packed_words = (size_t)hp.instances * (hp.n + 1) * hp.n * POLY;
   {
     b200pir_ctx::Scope sc(c, ST_PACK);
-    launch_pack(c->dp, c->w_packed.p, packed_words, folded, ct_stride, (size_t)c->slices * ct_stride, (int)count, c->pp_table(pp, count).pack,
+    launch_pack(c->dp, c->w_packed.p, packed_words, s.p, s.stride, (size_t)c->slices * s.stride, (int)count, pp_table(c, keys, count).pack,
                 (int)hp.n, (int)hp.instances, (int)hp.t_conv, c->bits_conv, c->live_conv, (int)hp.version, c->stream);
   }
   {
@@ -719,7 +736,7 @@ int b200pir_multiply_reg_by_database(b200pir_ctx* c, b200pir_db* db, uint64_t sl
   DevBuf<uint32_t> o((size_t)c->slices * rows * 4 * POLY), zm(zmajor ? o.n : 0);
   B200_CUDA(cudaMemcpyAsync(vq.p, v_firstdim, vq.n * 8, cudaMemcpyHostToDevice, c->stream));
   launch_query_to_dev(db->layout.G, qd.p, vq.p, c->stream);
-  run_first_dim(c, db, 1, qd.p, zmajor ? zm.p : o.p, (int)slice, 1);
+  run_first_dim(c, db, 1, qd.p, Images{}, zmajor ? zm.p : o.p, (int)slice, 1);
   uint32_t* o_slice = o.p + (size_t)slice * rows * 4 * POLY;          // ntt32 [row][ct_row][n][z] of this slice
   if (zmajor) launch_zmajor_to_ntt32(db->layout.F, zm.p, o_slice, (int)slice, c->stream);
   download_widen(c, out, o_slice, (size_t)rows * 4 * POLY);
@@ -801,7 +818,7 @@ int b200pir_coefficient_expansion(b200pir_ctx* c, b200pir_pp* pp, uint64_t* v) {
   DevBuf<uint64_t> wide;
   DevBuf<uint32_t> dv(words);
   upload_narrow(c, dv.p, wide, v, words);
-  run_coefficient_expansion(c, pp, dv.p, words, 1, true);
+  run_coefficient_expansion(c, Keys{pp}, dv.p, words, 1, true);
   download_widen(c, v, dv.p, words);
   B200_CUDA(cudaGetLastError());
   API_END
@@ -816,7 +833,7 @@ int b200pir_expand_query(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_c
   if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "context was created with expand_queries = 0");
   c->ensure_workspace(1, 1);
   B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_ct, 2 * POLY * 8, cudaMemcpyHostToDevice, c->stream));
-  run_expand_query(c, pp, c->w_query.p, c->w_v.p, c->w_qdev.p, c->w_vfold.p, 1);
+  run_expand_query(c, Keys{pp}, c->w_query.p, c->w_v.p, c->w_qdev.p, c->w_vfold.p, 1, nullptr);
   // q_dev -> reference layout [z][j][r]
   const size_t qwords = (size_t)c->dim0 * 2 * POLY;
   std::vector<uint32_t> hq(qwords * 2);
@@ -844,7 +861,7 @@ int b200pir_pack(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* v_ct, uint64_t*
   DevBuf<uint32_t> o(outp * 2 * POLY), res(nn * 4 * POLY);
   B200_CUDA(cudaMemcpyAsync(cts.p, v_ct, cts.n * 8, cudaMemcpyHostToDevice, c->stream));
   launch_raw_to_res(c->dp, res.p, cts.p, nn * 2, c->stream);
-  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, c->pp_table(pp, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, c->live_conv, (int)hp.version, c->stream,
+  launch_pack(c->dp, raw.p, 0, res.p, 4 * POLY, 0, 1, pp_table(c, Keys{pp}, 1).pack, (int)hp.n, 1, (int)hp.t_conv, c->bits_conv, c->live_conv, (int)hp.version, c->stream,
               cts.p);
   // the reference's pack returns the NTT-form matrix (server.rs:467); the kernel already applied .raw()
   launch_to_ntt(c->dp, o.p, raw.p, outp, c->stream);
@@ -884,35 +901,30 @@ struct Responses {
 };
 
 // One single-GPU query call on `count` queries: the checks, stage(), which puts the queries into the workspace (w_query, or
-// w_qdev and w_vfold for direct upload), one database pass and the responses.  `pps`: one handle per query (a multi-client
-// batch, whose workspace is sized once for a full coalesced batch: batch sizes vary from call to call, the buffers do not), or
-// null, and `pp` serves every query.  `needs_expand`: the queries are ciphertexts, which only an expanding context takes.
+// w_qdev and w_vfold for direct upload), one database pass and the responses.  `keys.each`: a multi-client batch, whose
+// workspace is sized once for a full coalesced batch (batch sizes vary from call to call, the buffers do not).
+// `needs_expand`: the queries are ciphertexts, which only an expanding context takes.
 template <typename Stage>
-void run_queries(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, b200pir_pp* const* pps, size_t count, bool needs_expand,
-                 Stage stage, const Responses& out) {
+void run_queries(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, bool needs_expand, Stage stage,
+                 const Responses& out) {
   Guard gd(c);
   check_db(c, db);
-  if (pps)
-    for (size_t i = 0; i < count; i++) check_pp(c, pps[i]);
+  if (keys.each)
+    for (size_t i = 0; i < count; i++) check_pp(c, keys.each[i]);
   else
-    check_pp(c, pp);
+    check_pp(c, keys.one);
   if (db->shard.count != 1) throw Error(B200PIR_E_BADARG, "sharded database: use the stage_a / stage_b entry points");
   if (needs_expand && !c->hp.expand_queries)
-    throw Error(B200PIR_E_BADARG, pps ? "multi-client batches need expand_queries" : "batch entry point needs expand_queries");
+    throw Error(B200PIR_E_BADARG, keys.each ? "multi-client batches need expand_queries" : "batch entry point needs expand_queries");
   if (count == 0) return;
-  c->ensure_workspace(pps && c->coalesce ? std::max(count, b200pir_ctx::kCoalesceMax) : count, db->rows);
+  c->ensure_workspace(keys.each && c->coalesce ? std::max(count, b200pir_ctx::kCoalesceMax) : count, db->rows);
   c->prof_reset();
   stage();
   // format-2 databases get their operand as tile images straight from the expansion
   const bool images = db->layout.format == 2 && c->hp.expand_queries;
-  if (pps) pp = pps[0];            // pp_table takes the handles from multi_pps
-  c->multi_pps = pps;
-  try {
-    run_prepare(c, pp, count, images);
-    run_first_dim_and_fold(c, db, count, nullptr, nullptr, images ? c->w_qt.p : nullptr, 16);
-    run_pack_encode(c, pp, c->folded, c->folded_stride, count, out.dev ? out.dev : c->w_resp.p);
-  } catch (...) { c->multi_pps = nullptr; throw; }
-  c->multi_pps = nullptr;
+  run_prepare(c, keys, count, images);
+  const Survivors s = run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{images ? c->w_qt.p : nullptr, 16}, c->w_vfold.p);
+  run_pack_encode(c, keys, s, count, out.dev ? out.dev : c->w_resp.p);
   if (!out.dev) {
     const size_t rb = c->response_bytes;
     if (out.each)
@@ -942,7 +954,7 @@ int b200pir_process_query_batch_dev(b200pir_ctx* c, b200pir_db* db, b200pir_pp* 
                                     size_t count, uint8_t* out_dev) {
   API_BEGIN
   if (!c || !out_dev || !query_cts_dev) throw Error(B200PIR_E_BADARG, "null argument");
-  run_queries(c, db, pp, nullptr, count, true, [&] {
+  run_queries(c, db, Keys{pp}, count, true, [&] {
     B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_cts_dev, count * 2 * POLY * 8, cudaMemcpyDeviceToDevice, c->stream));
   }, Responses{out_dev});
   API_END
@@ -952,7 +964,7 @@ int b200pir_process_query_batch(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, 
                                 uint8_t* out, size_t* out_len_each) {
   API_BEGIN
   if (!c || !out || !query_cts) throw Error(B200PIR_E_BADARG, "null argument");
-  run_queries(c, db, pp, nullptr, count, true, [&] {
+  run_queries(c, db, Keys{pp}, count, true, [&] {
     B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_cts, count * 2 * POLY * 8, cudaMemcpyHostToDevice, c->stream));
   }, Responses{nullptr, out, nullptr, out_len_each});
   API_END
@@ -993,7 +1005,7 @@ int coalesced_query(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, const uint64
     try {
       std::vector<b200pir_pp*> pps; std::vector<const uint64_t*> cts; std::vector<const uint8_t*> bys; std::vector<uint8_t*> outs;
       for (auto* p : batch) { pps.push_back(p->pp); cts.push_back(p->query_ct); bys.push_back(p->query_bytes); outs.push_back(p->out); }
-      run_queries(c, bdb, nullptr, pps.data(), batch.size(), true, [&] { stage_each(c, cts.data(), bys.data(), batch.size()); },
+      run_queries(c, bdb, Keys{nullptr, pps.data()}, batch.size(), true, [&] { stage_each(c, cts.data(), bys.data(), batch.size()); },
                   Responses{nullptr, nullptr, outs.data()});
     } catch (const std::exception& e) { rc = fail(e); err = e.what(); }
     lk.lock();
@@ -1016,7 +1028,7 @@ int b200pir_process_queries(b200pir_ctx* c, b200pir_db* db, b200pir_pp* const* p
   for (size_t i = 0; i < count; i++)
     if (!pps[i] || !query_cts[i] || !outs[i]) throw Error(B200PIR_E_BADARG, "null entry");
   if (count == 0) return 0;
-  run_queries(c, db, nullptr, pps, count, true, [&] { stage_each(c, query_cts, nullptr, count); }, Responses{nullptr, nullptr, outs});
+  run_queries(c, db, Keys{nullptr, pps}, count, true, [&] { stage_each(c, query_cts, nullptr, count); }, Responses{nullptr, nullptr, outs});
   API_END
 }
 int b200pir_coalesce_stats(b200pir_ctx* c, uint64_t* batches, uint64_t* queries) {
@@ -1039,7 +1051,7 @@ int b200pir_process_query_bytes(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, 
     if (rc == 0 && out_len_each) *out_len_each = c->response_bytes;
     return rc;
   }
-  run_queries(c, db, pp, nullptr, count, false, [&] {
+  run_queries(c, db, Keys{pp}, count, false, [&] {
     if (c->hp.expand_queries) {
       deserialize_queries(c, queries, count, c->w_query.p);
     } else {
@@ -1064,7 +1076,7 @@ int b200pir_process_query(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, const 
   API_BEGIN
   if (!v_buf || (!v_ct && c->hp.nu_2) || !out) throw Error(B200PIR_E_BADARG, "null argument");
   DevBuf<uint64_t> vq, raw;        // staging, in use until the call's final synchronise
-  run_queries(c, db, pp, nullptr, 1, false, [&] {
+  run_queries(c, db, Keys{pp}, 1, false, [&] {
     // server.rs:666-678: v_reg_reoriented = query.v_buf ; v_folding = v_ct.map(ntt)
     vq.alloc((size_t)c->dim0 * 2 * POLY);
     B200_CUDA(cudaMemcpyAsync(vq.p, v_buf, vq.n * 8, cudaMemcpyHostToDevice, c->stream));
@@ -1082,15 +1094,15 @@ int b200pir_process_query(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, const 
 // ---- multi-GPU building blocks: the three phases with caller-owned device buffers in between, so the host can put a
 // collective between them (bench.py: queries are expanded by the rank that received them, everything is all-gathered)
 namespace {
-// the survivors of the last fold, [count][slices], into partial_dev as a dense buffer of residue-form ciphertexts
-void gather_survivors(b200pir_ctx* c, size_t count, uint32_t* partial_dev) {
-  B200_CUDA(cudaMemcpy2DAsync(partial_dev, 4 * POLY * 4, c->folded, c->folded_stride * 4, 4 * POLY * 4, count * c->slices,
+// the survivors `s`, [count][slices], into partial_dev as a dense buffer of residue-form ciphertexts
+void gather_survivors(b200pir_ctx* c, Survivors s, size_t count, uint32_t* partial_dev) {
+  B200_CUDA(cudaMemcpy2DAsync(partial_dev, 4 * POLY * 4, s.p, s.stride * 4, 4 * POLY * 4, count * c->slices,
                               cudaMemcpyDeviceToDevice, c->stream));
 }
 
 // The last phase for queries [first, first + count) of the `total_count` whose partial survivors `world` ranks gathered: their
 // fold across the ranks with the folding matrices v_folding, then pack and encode into out_dev
-void run_finish(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* gathered_dev, size_t world, size_t total_count, size_t first,
+void run_finish(b200pir_ctx* c, Keys keys, const uint32_t* gathered_dev, size_t world, size_t total_count, size_t first,
                 size_t count, const uint32_t* v_folding, uint8_t* out_dev) {
   // gathered: [world][total_count][slices][ct]  ->  w_mult as [count][slices][world][ct]   (ct = 4*2048 u32)
   const size_t ct = 4 * POLY;
@@ -1099,83 +1111,79 @@ void run_finish(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* gathered_dev, si
                                 ct * 4, ct * 4, count * c->slices, cudaMemcpyDeviceToDevice, c->stream));
   int dims = 0;
   while (((size_t)1 << dims) < world) dims++;
+  Survivors s{c->w_mult.p, world * ct};
   {
     b200pir_ctx::Scope sc(c, ST_FOLD);
-    c->folded = c->w_mult.p;
-    c->folded_stride = world * ct;
-    if (world > 1)
-      c->folded = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, world * ct, world, dims - 1, v_folding, c->slices);
+    if (world > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, world, dims - 1, v_folding, c->slices);
   }
-  run_pack_encode(c, pp, c->folded, c->folded_stride, count, out_dev);
+  run_pack_encode(c, keys, s, count, out_dev);
 }
-}  // namespace
 
-int b200pir_expand_queries_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count,
-                               void* q_expanded_dev, uint32_t* v_folding_dev) {
+// The expansion phase of `count` queries into the caller's buffers: the first-dimension operand as q_dev or, with `images`, as
+// the tile images of one group of 1..16 queries; the folding matrices into v_folding_dev
+int expand_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count, void* operand_dev,
+               uint32_t* v_folding_dev, bool images) {
   API_BEGIN
-  if (!c || !query_cts_dev || !q_expanded_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
+  if (!c || !query_cts_dev || !operand_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_pp(c, pp);
   if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "needs expand_queries");
+  if (images) {
+    if (count == 0 || count > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
+    if (!tc5_supported(make_tc5_geom(c->dim0, 32))) throw Error(B200PIR_E_UNSUPPORTED, "dim0 too large for the wgmma kernel");
+  }
   if (count == 0) return 0;
   c->w_v.ensure(count * c->v_words());
   c->prof_reset();
   {
     b200pir_ctx::Scope sc(c, ST_EXPAND);
-    run_expand_query(c, pp, query_cts_dev, c->w_v.p, (uint4*)q_expanded_dev, v_folding_dev, (int)count);
+    run_expand_query(c, Keys{pp}, query_cts_dev, c->w_v.p, images ? nullptr : (uint4*)operand_dev, v_folding_dev, (int)count,
+                     images ? (uint8_t*)operand_dev : nullptr);
   }
   B200_CUDA(cudaGetLastError());
   API_END
 }
-int b200pir_first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* q_expanded_dev, const uint32_t* v_folding_dev,
-                               size_t count, uint32_t* partial_dev) {
+
+// The first dimension and local fold of `count` queries, their survivors into partial_dev: the operand as q_dev or, with
+// `images`, as tile images of per_group queries each (format-2 databases)
+int first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* operand_dev, size_t count, bool images, size_t per_group,
+                       const uint32_t* v_folding_dev, uint32_t* partial_dev) {
   API_BEGIN
-  if (!c || !q_expanded_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
+  if (!c || !operand_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
+  if (images) {
+    if (db->layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
+    if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
+  }
   if (count == 0) return 0;
   c->ensure_workspace_lite(count, db->rows);
-  run_first_dim_and_fold(c, db, count, (const uint4*)q_expanded_dev, v_folding_dev);
-  gather_survivors(c, count, partial_dev);
+  const uint4* qdev = images ? nullptr : (const uint4*)operand_dev;
+  const Images im{images ? (const uint8_t*)operand_dev : nullptr, per_group};
+  gather_survivors(c, run_first_dim_and_fold(c, db, count, qdev, im, v_folding_dev), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
+}
+}  // namespace
+
+int b200pir_expand_queries_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count,
+                               void* q_expanded_dev, uint32_t* v_folding_dev) {
+  return expand_dev(c, pp, query_cts_dev, count, q_expanded_dev, v_folding_dev, false);
+}
+int b200pir_first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* q_expanded_dev, const uint32_t* v_folding_dev,
+                               size_t count, uint32_t* partial_dev) {
+  return first_dim_fold_dev(c, db, q_expanded_dev, count, false, 0, v_folding_dev, partial_dev);
 }
 // The same two phases with the first-dimension operand exchanged as operand tile images (format-2 databases): the rank that expands a
 // group of <= 16 queries also re-tiles it, once; the receivers multiply straight from the image.
 size_t b200pir_query_image_bytes(b200pir_ctx* c) { return c ? tc5_query_bytes(make_tc5_geom(c->dim0, 32)) : 0; }
 int b200pir_expand_queries_images_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count, void* image_dev,
                                       uint32_t* v_folding_dev) {
-  API_BEGIN
-  if (!c || !query_cts_dev || !image_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_pp(c, pp);
-  if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "needs expand_queries");
-  if (count == 0 || count > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
-  if (!tc5_supported(make_tc5_geom(c->dim0, 32))) throw Error(B200PIR_E_UNSUPPORTED, "dim0 too large for the wgmma kernel");
-  c->w_v.ensure(count * c->v_words());
-  c->prof_reset();
-  {
-    b200pir_ctx::Scope sc(c, ST_EXPAND);
-    run_expand_query(c, pp, query_cts_dev, c->w_v.p, nullptr, v_folding_dev, (int)count, (uint8_t*)image_dev);
-  }
-  B200_CUDA(cudaGetLastError());
-  API_END
+  return expand_dev(c, pp, query_cts_dev, count, image_dev, v_folding_dev, true);
 }
 int b200pir_first_dim_fold_images_dev(b200pir_ctx* c, b200pir_db* db, const void* images_dev, size_t groups, size_t per_group,
                                       const uint32_t* v_folding_dev, uint32_t* partial_dev) {
-  API_BEGIN
-  if (!c || !images_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  check_db(c, db);
-  if (db->layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
-  if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
-  const size_t count = groups * per_group;
-  if (count == 0) return 0;
-  c->ensure_workspace_lite(count, db->rows);
-  run_first_dim_and_fold(c, db, count, nullptr, v_folding_dev, (const uint8_t*)images_dev, per_group);
-  gather_survivors(c, count, partial_dev);
-  B200_CUDA(cudaGetLastError());
-  API_END
+  return first_dim_fold_dev(c, db, images_dev, groups * per_group, true, per_group, v_folding_dev, partial_dev);
 }
 int b200pir_finish_queries_dev(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* gathered_dev, size_t world, size_t total_count,
                                size_t first, size_t count, const uint32_t* v_folding_dev, uint8_t* out_dev) {
@@ -1187,7 +1195,7 @@ int b200pir_finish_queries_dev(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* g
   if (first + count > total_count) throw Error(B200PIR_E_SHAPE, "query range out of bounds");
   if (count == 0) return 0;
   c->ensure_workspace_lite(count, world);
-  run_finish(c, pp, gathered_dev, world, total_count, first, count, v_folding_dev, out_dev);
+  run_finish(c, Keys{pp}, gathered_dev, world, total_count, first, count, v_folding_dev, out_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -1203,9 +1211,8 @@ int b200pir_query_stage_a_dev(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, co
   c->ensure_workspace(count, db->rows);
   c->prof_reset();
   B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_cts_dev, count * 2 * POLY * 8, cudaMemcpyDeviceToDevice, c->stream));
-  run_prepare(c, pp, count);
-  run_first_dim_and_fold(c, db, count);
-  gather_survivors(c, count, partial_dev);
+  run_prepare(c, Keys{pp}, count, false);
+  gather_survivors(c, run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{}, c->w_vfold.p), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -1218,7 +1225,7 @@ int b200pir_query_stage_b_dev(b200pir_ctx* c, b200pir_pp* pp, const uint32_t* ga
   check_pp(c, pp);
   if (world == 0 || (world & (world - 1)) || world > (size_t)c->num_per) throw Error(B200PIR_E_SHAPE, "bad world size");
   c->ensure_workspace(count, world);
-  run_finish(c, pp, gathered_dev, world, count, 0, count, c->w_vfold.p, out_dev);
+  run_finish(c, Keys{pp}, gathered_dev, world, count, 0, count, c->w_vfold.p, out_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }

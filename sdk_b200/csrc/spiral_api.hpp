@@ -48,11 +48,9 @@ struct b200pir_ctx {
   DevBuf<uint32_t> w_zflags;     // all-zero flags of the current fold round's ciphertexts ("sparse_fold")
   DevBuf<uint32_t> w_xr;         // [Q][num_in][2][2048] residues of row 0 (expansion rounds)
   DevBuf<uint4> w_qdev;          // [Q][dim0][2048]
-  DevBuf<uint32_t> w_vfold, w_vfold_neg;   // [Q][nu_2][2][2t][2][2048]
+  DevBuf<uint32_t> w_vfold;      // [Q][nu_2][2][2t][2][2048]
   DevBuf<uint32_t> w_mult;       // [Q][slices][rows][2][2][2048]  NTT form, then residue form in place
   DevBuf<uint32_t> w_cts;        // ping-pong partner of w_mult for the fold rounds (same size)
-  const uint32_t* folded = nullptr;   // where the last fold left its survivors
-  size_t folded_stride = 0;           // u32 words between consecutive (query, slice) survivors
   DevBuf<uint64_t> w_packed;     // [Q][inst][n+1][n][2048]
   DevBuf<uint8_t> w_resp;        // [Q][response_bytes]
   // database writers (upsert, update_item_raw, update_many_items, load_raw_file, uploads): raw item bytes and their item
@@ -106,13 +104,10 @@ struct b200pir_ctx {
   std::deque<Pending*> pending;
   bool leader_active = false;
   unsigned long long coalesced_batches = 0, coalesced_queries = 0;
-  // per-query public parameters (PpTable, kernels.h): device arrays [4][pptab_cap] of base pointers; `multi_pps` (host array, one
-  // handle per query of the call in flight) is set by the multi-client entry points, otherwise one handle serves every query
+  // per-query public parameters (PpTable, kernels.h): device arrays [4][pptab_cap] of base pointers, filled by pp_table (api.cu)
   DevBuf<const uint32_t*> d_pptab;
   size_t pptab_cap = 0;
   std::vector<const uint32_t*> h_pptab;          // what d_pptab holds (skip the upload when unchanged)
-  b200pir_pp* const* multi_pps = nullptr;
-  PpTable pp_table(b200pir_pp* pp, size_t count);
   // profiling
   struct Span { int stage; cudaEvent_t a, b; };
   std::vector<Span> spans;
@@ -170,7 +165,6 @@ struct b200pir_ctx {
     if (hp.expand_queries) w_v.ensure(queries * v_words());
     w_qdev.ensure(queries * (size_t)dim0 * POLY);
     w_vfold.ensure(queries * std::max<size_t>(fold_words(), 1));
-    w_vfold_neg.ensure(queries * std::max<size_t>(fold_words(), 1));
     w_mult.ensure(queries * slices * rows * 4 * POLY);
     w_cts.ensure(queries * slices * rows * 4 * POLY);
     w_packed.ensure(queries * hp.instances * (hp.n + 1) * hp.n * POLY);
