@@ -7,10 +7,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libb200pir.so")
-SOURCES = ["api.cu", "db_api.cu", "dpir_api.cu", "poly_kernels.cu", "mul_kernels.cu", "imma_kernels.cu", "wire_kernels.cu", "tc5_kernels.cu", "dpir_gemm.cu",
+SOURCES = ["api.cu", "db_api.cu", "dpir_api.cu", "dpir_server_api.cu", "poly_kernels.cu", "mul_kernels.cu", "imma_kernels.cu", "wire_kernels.cu", "tc5_kernels.cu", "dpir_gemm.cu",
            "export_kernels.cu", "dpir_load.cu", "dpir_serve.cu", "dpir_tc.cu",
            "dpir_update.cu"]
-HEADERS = ["api_internal.hpp", "spiral_api.hpp", "common.cuh", "kernels.h", "ntt_core.cuh", "tc5_layout.cuh", "tc5_ptx.cuh", "ntt_core4096.cuh", "ntt_tables.hpp",
+HEADERS = ["api_internal.hpp", "spiral_api.hpp", "dpir_api.hpp", "dpir_kernels.h", "common.cuh", "kernels.h", "ntt_core.cuh", "tc5_layout.cuh", "tc5_ptx.cuh", "ntt_core4096.cuh", "ntt_tables.hpp",
            "item_place.cuh", "update_body.hpp", "dpir_wire.hpp", "dpir_tc_layout.cuh", "dpir_aes.cuh", "gadget.hpp", os.path.join("..", "..", "include", "b200pir.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"]

@@ -1,5 +1,5 @@
-// What the C-ABI translation units (api.cu and db_api.cu: Spiral, dpir_api.cu: DoublePIR) share: device buffers, the error
-// plumbing of the entry points and the device check.
+// What the C-ABI translation units (api.cu and db_api.cu: Spiral, dpir_api.cu and dpir_server_api.cu: DoublePIR) share:
+// device buffers, the error plumbing of the entry points and the device check.
 #pragma once
 #include "../../include/b200pir.h"
 #include "kernels.h"

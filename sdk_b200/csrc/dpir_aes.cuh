@@ -4,7 +4,7 @@
 // data-dependent, so this is NOT constant-time: that is fine here, because the key and the output are public (the reference
 // derives public matrices only, matrix.rs:120-124) and nothing secret ever passes through it.
 #pragma once
-#include "kernels.h"
+#include "dpir_kernels.h"
 
 namespace b200pir {
 

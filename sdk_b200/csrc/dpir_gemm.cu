@@ -15,7 +15,7 @@
 // and 64..127 (four 64 x 32 accumulators = 64 registers a thread: wider tiles push ptxas into spilling accumulators of
 // in-flight MMAs), warp 8 = producer (ring of k-steps: 2 A tiles + 4 B quarter tiles = 12 KiB per stage).  This is an offline step; the kernel is written for exactness and clarity, not tuned beyond
 // keeping the tensor pipe fed.
-#include "kernels.h"
+#include "dpir_kernels.h"
 #include "tc5_ptx.cuh"
 
 namespace b200pir {

@@ -9,8 +9,10 @@
 //
 // k_dpir_layout: Db::load_data / load_data_fast (database/database.rs:168-247) as a gather, one thread per word of one band of
 // rows of the l x m matrix, then "Map DB elems to [-p/2; p/2]" (the wrapping subtraction of p/2 from every word, touched or
-// not).  A band's entries are one contiguous range of the input, so only that range needs to be on the device (api.cu stages
-// the input band by band).
+// not).  A band's entries are one contiguous range of the input, so only that range needs to be on the device (dpir_api.cu
+// stages the input band by band).
+//
+// k_dpir_synth: the words of b200pir_dpir_create_synthetic's matrix, a counter PRNG (splitmix64) of the word index.
 #include "dpir_aes.cuh"
 
 namespace b200pir {
@@ -113,6 +115,12 @@ __global__ void k_dpir_layout(uint32_t* __restrict__ band, const uint8_t* __rest
   if (bad || wide) atomicOr(out_of_range, (bad ? 1 : 0) | (wide ? 2 : 0));
 }
 
+__global__ void k_dpir_synth(uint32_t* a, size_t words, uint64_t seed, size_t index0) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= words) return;
+  a[i] = (uint32_t)splitmix64_at(seed, index0 + i) & 0x3FFFFFFFu;
+}
+
 unsigned grid_for(size_t items, int block) {
   const size_t need = (items + block - 1) / block;
   return (unsigned)std::min<size_t>(need ? need : 1, 132 * 32);
@@ -146,6 +154,13 @@ DpirAesKey dpir_aes_key(const uint8_t key[16]) {
 void launch_dpir_derive(uint32_t* out, size_t words, const DpirAesKey& key, cudaStream_t s) {
   ++g_kernel_launches;
   k_dpir_derive<<<grid_for((words + 3) / 4, 256), 256, 0, s>>>(out, words, key);
+}
+
+void launch_dpir_synth(uint32_t* a, size_t words, uint64_t seed, cudaStream_t s) {
+  for (size_t off = 0, cur; off < words; off += cur) {      // 2^30 words a launch
+    cur = std::min<size_t>((size_t)1 << 30, words - off);
+    k_dpir_synth<<<(unsigned)((cur + 255) / 256), 256, 0, s>>>(a + off, cur, seed, off);
+  }
 }
 
 void launch_dpir_layout(uint32_t* band, const uint8_t* data, uint64_t base, uint64_t count, bool bits_format, uint64_t r0,

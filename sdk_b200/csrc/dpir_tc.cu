@@ -13,7 +13,7 @@
 // Copies run DTC_DIST chunks ahead through a ring of DTC_STAGES stages; two barriers a chunk order the copies, the unpacking and
 // the MMAs (a stage is refilled only after every warpgroup's wgmma_wait has retired the MMAs that read it).  Partial sums of a
 // split k range are added with atomicAdd into zeroed outputs (exact modulo 2^32; not with big-endian outputs).
-#include "kernels.h"
+#include "dpir_kernels.h"
 #include "tc5_ptx.cuh"
 #include "dpir_tc_layout.cuh"
 

@@ -689,6 +689,17 @@ def test_c_dpir_create_and_answer_many_beside_a_busy_legacy_stream(delay, stream
     reqs = [pool[:1], pool[1:3], pool[3:]]
     wires = [D.serialize_request(q) for q in reqs]
     want = [TS.wire(E.run_answer(st, prm, info, delta, q), prm, info, delta) for q in reqs]
+    # the one-shot ops: matmul, matrix_mul_transposed_packed and transpose_expand_concat_cols_squish
+    mm_a = (rng.integers(0, 65536, (300, 70)).astype(np.int64) - 32768).astype(np.uint32)
+    mm_b = rng.integers(0, 2**32, (70, 130), dtype=np.uint64).astype(np.uint32)
+    mm_ref = ((mm_a.astype(np.uint64) @ mm_b.astype(np.uint64)) & np.uint64(0xFFFFFFFF)).astype(np.uint32)
+    t_rows, t_cols, t_brows = 40, 150, 24
+    t_a = rng.integers(0, 2**32, t_rows * t_cols, dtype=np.uint64).astype(np.uint32)
+    t_b = rng.integers(0, 2**32, t_brows * 3 * t_cols, dtype=np.uint64).astype(np.uint32)
+    t_ref = E.np_matrix_mul_transposed_packed(t_a, t_b, t_rows, t_cols, t_brows, 3 * t_cols)
+    x_rows, x_cols, x_mod, x_delta, x_concat = 4 * 65, 3, 991, 4, 4
+    x_a = rng.integers(0, 2**32, x_rows * x_cols, dtype=np.uint64).astype(np.uint32)
+    x_ref = E.np_transpose_expand_concat_cols_squish(x_a, x_rows, x_cols, x_mod, x_delta, x_concat)
 
     def sequence():
         m = D.PackedMatrix(a, rows, cols)
@@ -702,17 +713,27 @@ def test_c_dpir_create_and_answer_many_beside_a_busy_legacy_stream(delay, stream
         finally:
             srv.close()
             dbm.close()
-        return mv, many
+        ops = (D.matmul(mm_a, mm_b), D.matrix_mul_transposed_packed(t_a, t_rows, t_cols, t_b, t_brows, 3 * t_cols),
+               D.transpose_expand_concat_cols_squish(x_a, x_rows, x_cols, x_mod, x_delta, x_concat))
+        return mv, many, ops
+
+    def check_ops(ops):
+        mm, mt, (x, xr, xc) = ops
+        assert np.array_equal(mm, mm_ref)
+        assert np.array_equal(mt, t_ref)
+        assert (xr, xc) == x_ref[1:] and np.array_equal(x, x_ref[0])
 
     t0 = time.perf_counter()
-    mv, many = sequence()
+    mv, many, ops = sequence()
     idle_ms = (time.perf_counter() - t0) * 1e3
     assert np.array_equal(mv, ref) and many == want
+    check_ops(ops)
     delay.sleep(streams[2], 3 * idle_ms + 50)
-    mv, many = sequence()
+    mv, many, ops = sequence()
     torch.cuda.synchronize()
     assert np.array_equal(mv, ref)
     assert many == want
+    check_ops(ops)
 
 
 # ------------------------------------------------------------------------------------------------ D: switching streams, profiling
