@@ -454,6 +454,48 @@ int b200pir_dpir_server_update(b200pir_dpir_server* s, const uint64_t* indices, 
  * .state).  Null pointers -> B200PIR_E_BADARG. */
 int b200pir_dpir_server_state(b200pir_dpir_server* s, uint32_t* h1_squished);
 
+/* ---- DoublePIR over several GPUs: a database split by rows, driven by one process (DESIGN §4.5) ----------------------------
+ * The split rule: the l layout rows fall into U = ceil(l / 3x) units of 3x rows (x from the DbInfo shape), the last one
+ * clipped at l, and shard g of G takes the next floor(U / G) units, one more when g < U mod G.  Every contraction of setup()
+ * and answer() that crosses rows is a wrapping u32 sum over l/x, and edges on multiples of 3x keep each packed column of h_1,
+ * a_1' and a_2^T inside one shard, so the sum of the shards' partials mod 2^32 is bit for bit the one-GPU result.
+ * Shard `index` of `shards`: its first row and row count.  Host only.  Errors: those of the db info (bits_per_entry up to 64);
+ * l not a multiple of x, shards == 0, or more shards than units -> B200PIR_E_SHAPE; null pointers or index >= shards ->
+ * B200PIR_E_BADARG. */
+int b200pir_dpir_shard_rows(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, size_t shards,
+                            size_t index, uint64_t* row_begin, uint64_t* rows);
+/* The load of b200pir_dpir_load_banded, split into `shards` row shards by the rule above: dbs_out[g] is a handle on devices[g]
+ * holding the squished store rows of shard g (a device may appear more than once).  h1_squished, a2_t and h2 are the whole host
+ * matrices, byte for byte b200pir_dpir_load_banded's.  Distinct devices load at once, one host thread each; shards that share a
+ * device load one after another.  scratch_bytes bounds each shard's band scratch.  Errors as b200pir_dpir_load_banded, and a
+ * shard count the rule refuses -> B200PIR_E_SHAPE; on any error no handle is returned and no device memory stays allocated. */
+int b200pir_dpir_load_sharded(const int* devices, size_t shards, const b200pir_dpir_params* params, uint64_t num_entries,
+                              uint64_t bits_per_entry, const uint8_t* data, uint64_t len, int entry_format, uint64_t scratch_bytes,
+                              b200pir_dpir** dbs_out, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2);
+/* The same with the raw bytes read from the file at `path` (pread, each shard its own byte range); errors as
+ * b200pir_dpir_load_file. */
+int b200pir_dpir_load_file_sharded(const int* devices, size_t shards, const b200pir_dpir_params* params, uint64_t num_entries,
+                                   uint64_t bits_per_entry, const char* path, int entry_format, uint64_t scratch_bytes,
+                                   b200pir_dpir** dbs_out, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2);
+/* A shard from host words: rows x cols packed words that are the layout rows [row_begin, row_begin + rows) of a database (rows
+ * of a saved `.dbp`, say).  Errors as b200pir_dpir_create. */
+int b200pir_dpir_create_shard(int device, const uint32_t* a, uint64_t row_begin, uint64_t rows, uint64_t cols, b200pir_dpir** out);
+/* What a handle holds: its first layout row (0 for the handles of the unsharded creators and loads), rows, packed columns and
+ * device.  Null pointers -> B200PIR_E_BADARG. */
+int b200pir_dpir_shard_info(b200pir_dpir* m, uint64_t* row_begin, uint64_t* rows, uint64_t* cols, int* device);
+/* A server over the row shards dbs[0 .. shards) of one database (borrowed; they must outlive the server), each shard on its
+ * handle's device, the first one's device being where responses are summed.  Each shard uploads its column band of
+ * h1_squished and of a2_t (the last band with the padding column).  The shards must tile [0, l) in order with every inner edge
+ * a multiple of 3x, and have ceil(m/3) packed columns; otherwise B200PIR_E_SHAPE.  Other errors as b200pir_dpir_server_create.
+ * The server is an ordinary b200pir_dpir_server: answer_size, answer (unchunked), answer_many, server_update, server_state and
+ * server_destroy keep their meaning, byte for byte the one-GPU results.  Each shard runs the passes of answer() over its rows on
+ * its device; the shards' partial responses go to the first shard's device (cudaMemcpyPeerAsync) and one kernel adds them.
+ * An update splits its changes by owning shard, and h2 passes through each shard's hint patch in turn; server_state gathers the
+ * whole h1_squished.  answer with chunk_idx >= 0 -> B200PIR_E_UNSUPPORTED (a sharded server holds every row). */
+int b200pir_dpir_server_create_sharded(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                                       b200pir_dpir* const* dbs, size_t shards, const uint32_t* h1_squished, const uint32_t* a2_t,
+                                       size_t max_queries, b200pir_dpir_server** out);
+
 #ifdef __cplusplus
 }
 #endif

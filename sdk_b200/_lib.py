@@ -134,6 +134,17 @@ def _load():
                                                C.POINTER(C.c_size_t)]),
         "b200pir_dpir_server_update": (C.c_int, [vp, u64p, u8p, C.c_size_t, u32p]),
         "b200pir_dpir_server_state": (C.c_int, [vp, u32p]),
+        "b200pir_dpir_shard_rows": (C.c_int, [C.POINTER(DpirParams), C.c_uint64, C.c_uint64, C.c_size_t, C.c_size_t,
+                                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+        "b200pir_dpir_load_sharded": (C.c_int, [C.POINTER(C.c_int), C.c_size_t, C.POINTER(DpirParams), C.c_uint64, C.c_uint64, u8p,
+                                                C.c_uint64, C.c_int, C.c_uint64, C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_load_file_sharded": (C.c_int, [C.POINTER(C.c_int), C.c_size_t, C.POINTER(DpirParams), C.c_uint64, C.c_uint64,
+                                                     C.c_char_p, C.c_int, C.c_uint64, C.POINTER(vp), u32p, u32p, u32p]),
+        "b200pir_dpir_create_shard": (C.c_int, [C.c_int, u32p, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(vp)]),
+        "b200pir_dpir_shard_info": (C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                              C.POINTER(C.c_int)]),
+        "b200pir_dpir_server_create_sharded": (C.c_int, [C.POINTER(DpirParams), C.c_uint64, C.c_uint64, C.POINTER(vp), C.c_size_t,
+                                                         u32p, u32p, C.c_size_t, C.POINTER(vp)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # raises AttributeError if the .so does not export a declared symbol

@@ -38,6 +38,16 @@ b200pir_dpir_info b200pir::dpir_info(const b200pir_dpir_params* prm, uint64_t nu
   return o;
 }
 
+b200pir::DpirShardRows b200pir::dpir_shard_rows(uint64_t l, uint64_t x, size_t shards, size_t index) {
+  const uint64_t unit = 3 * x, units = (l + unit - 1) / unit;
+  if (shards == 0 || shards > units)
+    throw Error(B200PIR_E_SHAPE, "cannot split " + std::to_string(units) + " units of 3x rows over " + std::to_string(shards) + " shards");
+  const uint64_t per = units / shards, extra = units % shards;
+  const uint64_t u0 = index * per + std::min<uint64_t>(index, extra), u1 = u0 + per + (index < extra ? 1 : 0);
+  const uint64_t r0 = u0 * unit, r1 = std::min(l, u1 * unit);
+  return DpirShardRows{r0, r1 - r0};
+}
+
 extern "C" {
 
 namespace {
@@ -86,19 +96,21 @@ void dpir_setup_rows(const uint32_t* d_band, uint64_t r0, uint64_t rows, uint64_
   launch_dpir_gemm_rows(d_h + r0 * n, a_img, d_band, rows, m, a1_img, n, s);                // h_1 = db.data * a_1
   launch_dpir_add_squish(d_dbsq + r0 * ((m + 2) / 3), d_band, rows, m, p / 2, s);         // db.data += p/2; db.squish()
 }
-// The tail, on the whole h_1 (l x n, device) and a2 (l/x x n, device): transpose / expand / concat, h_2 = h_1 * a_2, h_1 += p/2
-// and squish, a_2_copy.  h1_squished, a2_t and h2 are host buffers.  Synchronises s.
-void dpir_setup_tail(const uint32_t* d_h, const uint32_t* d_a2, uint64_t l, uint64_t n, uint32_t p, uint64_t delta, uint64_t x,
-                     uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2, cudaStream_t s) {
-  const size_t lx = l / x, rows1 = n * delta * x, lx3 = lx + (3 - lx % 3) % 3;
-  DevBuf<uint32_t> d_hc(rows1 * lx), d_h2(rows1 * n);
-  DevBuf<uint32_t> d_h1sq(rows1 * ((lx + 2) / 3)), d_a2t(n * lx3);
-  launch_dpir_transpose_expand_concat(d_hc.p, d_h, l, n, p, (int)delta, x, s);          // transpose, expand, concat_cols
-  launch_dpir_gemm(d_h2.p, d_hc.p, d_a2, rows1, lx, n, s);                               // h_2 = h_1 * a_2
-  launch_dpir_add_squish(d_h1sq.p, d_hc.p, rows1, lx, p / 2, s);                         // h_1 += p/2; squish
-  launch_dpir_pad_transpose(d_a2t.p, d_a2, lx, n, lx3, s);                               // a_2_copy
-  B200_CUDA(cudaMemcpyAsync(h1_squished, d_h1sq.p, d_h1sq.n * 4, cudaMemcpyDeviceToHost, s));
-  B200_CUDA(cudaMemcpyAsync(a2_t, d_a2t.p, d_a2t.n * 4, cudaMemcpyDeviceToHost, s));
+// The tail, on the h_1 rows [r0, r0 + rows) of an l-row database (rows x n, device; r0 a multiple of 3x, rows of x) and the
+// whole a2 (l/x x n, device): transpose / expand / concat, h_2 = h_1 * a_2 over the range's columns, h_1 += p/2 and squish,
+// a_2_copy.  Host buffers: the range's squished columns [r0 / 3x, ..) of h1_squished ((n delta x) x ceil(l/3x)); h2, the
+// range's partial of h_2 (all of it for the range [0, l)); a2_t, skipped when null.  Synchronises s.
+void dpir_setup_tail(const uint32_t* d_h, const uint32_t* d_a2, uint64_t l, uint64_t r0, uint64_t rows, uint64_t n, uint32_t p,
+                     uint64_t delta, uint64_t x, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2, cudaStream_t s) {
+  const size_t lx = l / x, rows1 = n * delta * x, lx3 = lx + (3 - lx % 3) % 3, lxg = rows / x, c1 = (lx + 2) / 3, c1g = (lxg + 2) / 3;
+  DevBuf<uint32_t> d_hc(rows1 * lxg), d_h2(rows1 * n);
+  DevBuf<uint32_t> d_h1sq(rows1 * c1g), d_a2t(a2_t ? n * lx3 : 0);
+  launch_dpir_transpose_expand_concat(d_hc.p, d_h, rows, n, p, (int)delta, x, s);       // transpose, expand, concat_cols
+  launch_dpir_gemm(d_h2.p, d_hc.p, d_a2 + r0 / x * n, rows1, lxg, n, s);                // h_2 = h_1 * a_2
+  launch_dpir_add_squish(d_h1sq.p, d_hc.p, rows1, lxg, p / 2, s);                        // h_1 += p/2; squish
+  if (a2_t) launch_dpir_pad_transpose(d_a2t.p, d_a2, lx, n, lx3, s);                     // a_2_copy
+  B200_CUDA(cudaMemcpy2DAsync(h1_squished + r0 / (3 * x), c1 * 4, d_h1sq.p, c1g * 4, c1g * 4, rows1, cudaMemcpyDeviceToHost, s));
+  if (a2_t) B200_CUDA(cudaMemcpyAsync(a2_t, d_a2t.p, d_a2t.n * 4, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaMemcpyAsync(h2, d_h2.p, d_h2.n * 4, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
   B200_CUDA(cudaGetLastError());
@@ -124,7 +136,7 @@ int b200pir_dpir_setup(int device, const uint32_t* db, uint64_t l, uint64_t m, c
   B200_CUDA(cudaMemcpyAsync(d_a2.p, a2, lx * n * 4, cudaMemcpyHostToDevice, s));
   launch_dpir_gemm_b_image(a1_img.p, d_a1.p, m, n, s);
   dpir_setup_rows(d_db.p, 0, l, m, n, p, a1_img.p, a_img.p, d_h.p, d_dbsq.p, s);        // every row as one band
-  dpir_setup_tail(d_h.p, d_a2.p, l, n, p, delta, x, h1_squished, a2_t, h2, s);
+  dpir_setup_tail(d_h.p, d_a2.p, l, 0, l, n, p, delta, x, h1_squished, a2_t, h2, s);
   B200_CUDA(cudaMemcpyAsync(db_squished, d_dbsq.p, d_dbsq.n * 4, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
   B200_CUDA(cudaGetLastError());
@@ -360,24 +372,40 @@ struct DpirStaging {
   }
 };
 
-// DoublePirServer::new + load_data / load_data_fast + setup() (server.rs:160-165, 201-229), band by band: for each band of
-// layout rows the band's input bytes are staged and uploaded, laid out, multiplied into h_1's rows and squished into the
-// resident store; setup()'s tail then runs on the whole h_1.  The band scratch is allocated once, sized by scratch_bytes.
-b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
-                              uint64_t len, int entry_format, uint64_t scratch_bytes, const DpirFill& fill, uint32_t* h1_squished,
-                              uint32_t* a2_t, uint32_t* h2) {
+// What every load checks before it touches a device: the DbInfo shape, the entry format, and that the entries fit l x m
+struct DpirLoadShape {
+  b200pir_dpir_info info;
+  DpirBandGeom G;
+};
+DpirLoadShape dpir_load_shape(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, uint64_t len,
+                              int entry_format) {
   const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry);
   const DpirBandGeom G = dpir_band_geom(params, info, entry_format, len);
-  const uint64_t l = params->l, m = params->m, n = params->n, x = info.x, count = G.count;
-  const uint32_t p = (uint32_t)params->p;
+  const uint64_t l = params->l, m = params->m, count = G.count;
   // where load_data would index past the matrix (and panic): the last packed element, or the last digit row of the last entry
   if (info.packing ? (count + info.packing - 1) / info.packing > l * m : (count && ((count - 1) / m + 1) > l / info.ne))
     throw Error(B200PIR_E_SHAPE, "the entries do not fit the l x m database");
-  if (l % x) throw Error(B200PIR_E_SHAPE, "l must be a multiple of x (concat_cols)");
-  std::unique_ptr<b200pir_dpir, DpirDeleter> h(dpir_new(device, l, (m + 2) / 3));
+  if (l % info.x) throw Error(B200PIR_E_SHAPE, "l must be a multiple of x (concat_cols)");
+  return DpirLoadShape{info, G};
+}
+
+// DoublePirServer::new + load_data / load_data_fast + setup() (server.rs:160-165, 201-229) for the layout rows [r0, r1) on one
+// device, band by band: for each band of rows the band's input bytes are staged and uploaded, laid out, multiplied into the
+// range's rows of h_1 and squished into the resident store; setup()'s tail then runs on the range's h_1 (dpir_setup_tail: its
+// columns of h1_squished, its partial of h2, and a2_t unless null).  The band scratch is allocated once, sized by scratch_bytes.
+// The whole database is the range [0, l); a shard's range has r0 a multiple of 3x (dpir_shard_rows).
+b200pir_dpir* dpir_load_range(int device, const b200pir_dpir_params* params, const DpirLoadShape& S, uint64_t num_entries,
+                              uint64_t bits_per_entry, int entry_format, uint64_t scratch_bytes, const DpirFill& fill, uint64_t r0,
+                              uint64_t r1, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
+  const b200pir_dpir_info& info = S.info;
+  const DpirBandGeom& G = S.G;
+  const uint64_t l = params->l, m = params->m, n = params->n, x = info.x, count = G.count, rows_g = r1 - r0;
+  const uint32_t p = (uint32_t)params->p;
+  std::unique_ptr<b200pir_dpir, DpirDeleter> h(dpir_new(device, rows_g, (m + 2) / 3));
+  h->row_begin = r0;
   cudaStream_t s = h->stream;
-  const uint64_t band = G.band_rows(scratch_bytes ? scratch_bytes : kDpirDefaultScratch);
-  DevBuf<uint32_t> d_h(l * n), d_a2((l / x) * n);
+  const uint64_t band = std::min(G.band_rows(scratch_bytes ? scratch_bytes : kDpirDefaultScratch), rows_g);
+  DevBuf<uint32_t> d_h(rows_g * n), d_a2((l / x) * n);
   {
     DevBuf<uint8_t> a1_img(dpir_gemm_b_bytes(m, n));
     {
@@ -392,15 +420,15 @@ b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uin
     DevBuf<int> d_flag(1);
     B200_CUDA(cudaMemsetAsync(d_flag.p, 0, sizeof(int), s));
     DpirStaging stage(s, (size_t)std::min<uint64_t>(kDpirStagePiece, G.raw_bytes(band)));
-    for (uint64_t r0 = 0; r0 < l; r0 += band) {
-      const uint64_t rows = std::min(band, l - r0);
+    for (uint64_t b = r0; b < r1; b += band) {
+      const uint64_t rows = std::min(band, r1 - b);
       // the band's entries [e0, e1) are bytes [b0, b1) of the input (bits: the band may start and end mid-byte)
-      const uint64_t e0 = std::min(G.first_entry(r0), count), e1 = std::min(G.first_entry(r0 + rows), count);
+      const uint64_t e0 = std::min(G.first_entry(b), count), e1 = std::min(G.first_entry(b + rows), count);
       const uint64_t b0 = G.bits_format ? e0 / 8 : e0, b1 = G.bits_format ? (e1 + 7) / 8 : e1;
       stage.upload(fill, d_raw.p, b0, b1 - b0);
-      launch_dpir_layout(d_band.p, d_raw.p, G.bits_format ? 8 * b0 : b0, count, G.bits_format, r0, rows, m, (uint32_t)info.packing,
+      launch_dpir_layout(d_band.p, d_raw.p, G.bits_format ? 8 * b0 : b0, count, G.bits_format, b, rows, m, (uint32_t)info.packing,
                          (uint32_t)bits_per_entry, (uint32_t)info.ne, p, d_flag.p, s);
-      dpir_setup_rows(d_band.p, r0, rows, m, n, p, a1_img.p, a_img.p, d_h.p, h->a.p, s);
+      dpir_setup_rows(d_band.p, b - r0, rows, m, n, p, a1_img.p, a_img.p, d_h.p, h->a.p, s);
     }
     B200_CUDA(cudaGetLastError());
     int flag = 0;
@@ -409,7 +437,7 @@ b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uin
     if (flag & 1) throw Error(B200PIR_E_UNSUPPORTED, "load: a packed database word lies outside [-2^15, 2^15) (entries far wider than bits_per_entry)");
     h->fields_exact = !(flag & 2);
   }
-  dpir_setup_tail(d_h.p, d_a2.p, l, n, p, info.delta, x, h1_squished, a2_t, h2, s);
+  dpir_setup_tail(d_h.p, d_a2.p, l, r0, rows_g, n, p, info.delta, x, h1_squished, a2_t, h2, s);
   h->from_load = true;
   h->entry_format = entry_format;
   h->load_count = count;
@@ -417,6 +445,98 @@ b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uin
   h->bits_per_entry = bits_per_entry;
   h->params = *params;
   return h.release();
+}
+
+b200pir_dpir* dpir_load_bands(int device, const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry,
+                              uint64_t len, int entry_format, uint64_t scratch_bytes, const DpirFill& fill, uint32_t* h1_squished,
+                              uint32_t* a2_t, uint32_t* h2) {
+  const DpirLoadShape S = dpir_load_shape(params, num_entries, bits_per_entry, len, entry_format);
+  return dpir_load_range(device, params, S, num_entries, bits_per_entry, entry_format, scratch_bytes, fill, 0, params->l,
+                         h1_squished, a2_t, h2);
+}
+
+// The load over `shards` row shards (dpir_shard_rows), shard g on devices[g]: one host thread a distinct device, each loading
+// its shards one after another, so distinct devices read their byte ranges and load at once.  Every range writes its own columns
+// of h1_squished; shard 0 writes a2_t; h2 is the sum of the ranges' partials mod 2^32.  On any error every handle is destroyed.
+void dpir_load_sharded(const int* devices, size_t shards, const b200pir_dpir_params* params, uint64_t num_entries,
+                       uint64_t bits_per_entry, uint64_t len, int entry_format, uint64_t scratch_bytes, const DpirFill& fill,
+                       b200pir_dpir** dbs_out, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
+  const DpirLoadShape S = dpir_load_shape(params, num_entries, bits_per_entry, len, entry_format);
+  if (shards == 0) throw Error(B200PIR_E_SHAPE, "no shards");
+  std::vector<DpirShardRows> R(shards);
+  for (size_t g = 0; g < shards; g++) R[g] = dpir_shard_rows(params->l, S.info.x, shards, g);
+  for (size_t g = 0; g < shards; g++) use_device(devices[g]);
+  const size_t h2_words = (size_t)params->n * S.info.delta * S.info.x * params->n;
+  std::vector<std::vector<uint32_t>> part(shards, std::vector<uint32_t>(h2_words));
+  std::vector<std::unique_ptr<b200pir_dpir, DpirDeleter>> out(shards);
+  std::vector<std::exception_ptr> err(shards);
+  std::vector<int> distinct;
+  for (size_t g = 0; g < shards; g++)
+    if (std::find(distinct.begin(), distinct.end(), devices[g]) == distinct.end()) distinct.push_back(devices[g]);
+  // g_kernel_launches is per thread: each worker reports what it launched, and the caller's count takes it in after the join
+  std::vector<unsigned long long> launched(distinct.size(), 0);
+  std::vector<std::thread> th;
+  for (size_t t = 0; t < distinct.size(); t++)
+    th.emplace_back([&, t] {
+      const int dev = distinct[t];
+      const unsigned long long k0 = g_kernel_launches;
+      for (size_t g = 0; g < shards; g++) {
+        if (devices[g] != dev) continue;
+        try {
+          out[g].reset(dpir_load_range(dev, params, S, num_entries, bits_per_entry, entry_format, scratch_bytes, fill, R[g].begin,
+                                       R[g].begin + R[g].rows, h1_squished, g == 0 ? a2_t : nullptr, part[g].data()));
+        } catch (...) {
+          err[g] = std::current_exception();
+          break;                                         // this device's later shards are not loaded: the call fails anyway
+        }
+      }
+      launched[t] = g_kernel_launches - k0;
+    });
+  for (auto& t : th) t.join();
+  for (unsigned long long k : launched) g_kernel_launches += k;
+  for (auto& e : err)
+    if (e) std::rethrow_exception(e);                    // `out` destroys every handle that was made
+  for (size_t i = 0; i < h2_words; i++) {
+    uint32_t v = 0;
+    for (size_t g = 0; g < shards; g++) v += part[g][i];
+    h2[i] = v;
+  }
+  for (size_t g = 0; g < shards; g++) dbs_out[g] = out[g].release();
+}
+
+// pread of bytes [off, off + n) of an open file, as the file loads read it
+DpirFill dpir_file_fill(int fd) {
+  return [fd](uint8_t* dst, uint64_t off, size_t n) {
+    while (n) {
+      const ssize_t r = pread(fd, dst, n, (off_t)off);
+      if (r < 0 && errno == EINTR) continue;
+      if (r <= 0) throw Error(B200PIR_E_SHAPE, "short read from the database file");
+      dst += r; off += (uint64_t)r; n -= (size_t)r;
+    }
+  };
+}
+
+// The database file at `path`, open, with its size
+struct DpirFile {
+  int fd = -1;
+  uint64_t size = 0;
+  explicit DpirFile(const char* path) {
+    fd = open(path, O_RDONLY | O_CLOEXEC);
+    if (fd < 0) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
+    struct stat st;
+    if (fstat(fd, &st)) throw Error(B200PIR_E_BADARG, std::string("cannot stat ") + path);
+    // the entry count comes from the file size, as load_data_fast's takes it from the bytes it is given; a directory or a
+    // device has no such size, and reading it fails
+    if (!S_ISREG(st.st_mode)) throw Error(B200PIR_E_SHAPE, "short read from the database file (not a regular file)");
+    size = (uint64_t)st.st_size;
+  }
+  ~DpirFile() { if (fd >= 0) close(fd); }
+  DpirFile(const DpirFile&) = delete;
+  DpirFile& operator=(const DpirFile&) = delete;
+};
+
+DpirFill dpir_memory_fill(const uint8_t* data) {
+  return [data](uint8_t* dst, uint64_t off, size_t n) { std::memcpy(dst, data + off, n); };
 }
 }  // namespace
 
@@ -432,8 +552,8 @@ int b200pir_dpir_load_banded(int device, const b200pir_dpir_params* params, uint
                              uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
   API_BEGIN
   if (!params || !data || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
-  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, len, entry_format, scratch_bytes,
-                            [data](uint8_t* dst, uint64_t off, size_t n) { std::memcpy(dst, data + off, n); }, h1_squished, a2_t, h2);
+  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, len, entry_format, scratch_bytes, dpir_memory_fill(data),
+                            h1_squished, a2_t, h2);
   API_END
 }
 
@@ -442,24 +562,63 @@ int b200pir_dpir_load_file(int device, const b200pir_dpir_params* params, uint64
                            uint32_t* a2_t, uint32_t* h2) {
   API_BEGIN
   if (!params || !path || !db_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
-  struct Closer { int fd; ~Closer() { if (fd >= 0) close(fd); } } file{open(path, O_RDONLY | O_CLOEXEC)};
-  if (file.fd < 0) throw Error(B200PIR_E_BADARG, std::string("cannot open ") + path);
-  struct stat st;
-  if (fstat(file.fd, &st)) throw Error(B200PIR_E_BADARG, std::string("cannot stat ") + path);
-  // the entry count comes from the file size, as load_data_fast's takes it from the bytes it is given; a directory or a
-  // device has no such size, and reading it fails
-  if (!S_ISREG(st.st_mode)) throw Error(B200PIR_E_SHAPE, "short read from the database file (not a regular file)");
-  const int fd = file.fd;
-  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, (uint64_t)st.st_size, entry_format, scratch_bytes,
-                            [fd](uint8_t* dst, uint64_t off, size_t n) {
-                              while (n) {
-                                const ssize_t r = pread(fd, dst, n, (off_t)off);
-                                if (r < 0 && errno == EINTR) continue;
-                                if (r <= 0) throw Error(B200PIR_E_SHAPE, "short read from the database file");
-                                dst += r; off += (uint64_t)r; n -= (size_t)r;
-                              }
-                            },
-                            h1_squished, a2_t, h2);
+  DpirFile file(path);
+  *db_out = dpir_load_bands(device, params, num_entries, bits_per_entry, file.size, entry_format, scratch_bytes,
+                            dpir_file_fill(file.fd), h1_squished, a2_t, h2);
+  API_END
+}
+
+int b200pir_dpir_shard_rows(const b200pir_dpir_params* params, uint64_t num_entries, uint64_t bits_per_entry, size_t shards,
+                            size_t index, uint64_t* row_begin, uint64_t* rows) {
+  API_BEGIN
+  if (!row_begin || !rows) throw Error(B200PIR_E_BADARG, "null argument");
+  const b200pir_dpir_info info = dpir_info(params, num_entries, bits_per_entry, 64);
+  if (params->l % info.x) throw Error(B200PIR_E_SHAPE, "l must be a multiple of x (concat_cols)");
+  if (shards && index >= shards) throw Error(B200PIR_E_BADARG, "shard index >= the shard count");
+  const DpirShardRows r = dpir_shard_rows(params->l, info.x, shards, index);
+  *row_begin = r.begin;
+  *rows = r.rows;
+  API_END
+}
+
+int b200pir_dpir_load_sharded(const int* devices, size_t shards, const b200pir_dpir_params* params, uint64_t num_entries,
+                              uint64_t bits_per_entry, const uint8_t* data, uint64_t len, int entry_format, uint64_t scratch_bytes,
+                              b200pir_dpir** dbs_out, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
+  API_BEGIN
+  if (!devices || !params || !data || !dbs_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+  dpir_load_sharded(devices, shards, params, num_entries, bits_per_entry, len, entry_format, scratch_bytes, dpir_memory_fill(data),
+                    dbs_out, h1_squished, a2_t, h2);
+  API_END
+}
+
+int b200pir_dpir_load_file_sharded(const int* devices, size_t shards, const b200pir_dpir_params* params, uint64_t num_entries,
+                                   uint64_t bits_per_entry, const char* path, int entry_format, uint64_t scratch_bytes,
+                                   b200pir_dpir** dbs_out, uint32_t* h1_squished, uint32_t* a2_t, uint32_t* h2) {
+  API_BEGIN
+  if (!devices || !params || !path || !dbs_out || !h1_squished || !a2_t || !h2) throw Error(B200PIR_E_BADARG, "null argument");
+  DpirFile file(path);
+  dpir_load_sharded(devices, shards, params, num_entries, bits_per_entry, file.size, entry_format, scratch_bytes,
+                    dpir_file_fill(file.fd), dbs_out, h1_squished, a2_t, h2);
+  API_END
+}
+
+int b200pir_dpir_create_shard(int device, const uint32_t* a, uint64_t row_begin, uint64_t rows, uint64_t cols, b200pir_dpir** out) {
+  API_BEGIN
+  if (!out) throw Error(B200PIR_E_BADARG, "null argument");
+  b200pir_dpir* m = nullptr;
+  if (int rc = b200pir_dpir_create(device, a, rows, cols, &m)) return rc;
+  m->row_begin = row_begin;
+  *out = m;
+  API_END
+}
+
+int b200pir_dpir_shard_info(b200pir_dpir* m, uint64_t* row_begin, uint64_t* rows, uint64_t* cols, int* device) {
+  API_BEGIN
+  if (!m || !row_begin || !rows || !cols || !device) throw Error(B200PIR_E_BADARG, "null argument");
+  *row_begin = m->row_begin;
+  *rows = m->rows;
+  *cols = m->cols;
+  *device = m->device;
   API_END
 }
 

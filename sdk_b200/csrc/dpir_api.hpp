@@ -17,6 +17,7 @@ struct b200pir_dpir {
   cudaStream_t stream = nullptr;
   bool own_stream = true;
   uint64_t rows, cols;
+  uint64_t row_begin = 0;   // the layout row of row 0: nonzero for a row shard (b200pir_dpir_load*_sharded, b200pir_dpir_create_shard)
   DevBuf<uint32_t> a;
   DevBuf<uint32_t> b, out;
   // what b200pir_dpir_load* laid out in `a`, for b200pir_dpir_server_update; from_load stays false for b200pir_dpir_create*
@@ -47,6 +48,13 @@ const uint8_t kDpirSeedA1[16] = B200PIR_DPIR_SEED_A1;
 b200pir_dpir_info dpir_info(const b200pir_dpir_params* prm, uint64_t num_entries, uint64_t bits, uint64_t max_bits = 63);
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// The row split of a sharded database (b200pir_dpir_shard_rows): the l rows fall into units of 3x rows, the last one clipped at
+// l, and shard g of G takes the next floor(U / G) units, one more when g < U mod G.  Edges on multiples of 3x keep every packed
+// column of h_1', a_1' and a_2^T (three l/x positions a word) inside one shard.  {row_begin, rows}; throws B200PIR_E_SHAPE for
+// G = 0 or more shards than units.
+struct DpirShardRows { uint64_t begin, rows; };
+DpirShardRows dpir_shard_rows(uint64_t l, uint64_t x, size_t shards, size_t index);
 
 // One pass of packed matrix x vectors: on the tensor cores (tc: tasks of DTC_ROWS rows and up to DTC_VECS vectors, whose b are
 // query images) or on k_dpir_matvec_multi (kDpirMvRows rows, up to kDpirMvMaxVecs vectors); its tasks are [t0, t1) of its plan

@@ -33,6 +33,9 @@ void launch_dpir_matvec_multi(const DpirMvTask* tasks, size_t ntasks, const Dpir
 int dpir_mv_ksplit(size_t ntasks, size_t cols, int sm_count);
 // dst[i] = byte-swapped src[i]
 void launch_dpir_bswap(uint32_t* dst, const uint32_t* src, size_t words, cudaStream_t s);
+// dst[i] = byte-swapped (sum over g < nparts of parts[g * stride + i]) mod 2^32, for i < words: a sharded server's partial
+// responses, one buffer of stride words per shard, into the wire-order response
+void launch_dpir_sum_be(uint32_t* dst, const uint32_t* parts, size_t stride, size_t nparts, size_t words, cudaStream_t s);
 
 // ---- the same passes on the tensor cores (dpir_tc.cu, index maps in dpir_tc_layout.cuh): tasks of up to DTC_ROWS rows and
 // DTC_VECS vectors, whose DpirMvVec::b points at the vector's query image (dtc_img_bytes(cols) bytes, 16-byte aligned) instead of

@@ -267,6 +267,16 @@ __global__ void k_dpir_bswap(uint32_t* __restrict__ dst, const uint32_t* __restr
   if (i < words) dst[i] = bswap32(src[i]);
 }
 
+// dst[i] = byte-swapped (sum over g < nparts of parts[g * stride + i]), wrapping: the partial responses of a sharded server's
+// shards into the wire-order response
+__global__ void k_dpir_sum_be(uint32_t* __restrict__ dst, const uint32_t* __restrict__ parts, size_t stride, int nparts, size_t words) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (size_t)gridDim.x * blockDim.x) {
+    uint32_t v = 0;
+    for (int g = 0; g < nparts; g++) v += parts[(size_t)g * stride + i];
+    dst[i] = bswap32(v);
+  }
+}
+
 template <int V>
 void launch_mv(const DpirMvTask* tasks, size_t ntasks, const DpirMvVec* vecs, size_t cols, int ksplit, int flags, cudaStream_t s) {
   constexpr int U = V >= 8 ? 2 : 4;
@@ -338,6 +348,13 @@ void launch_dpir_bswap(uint32_t* dst, const uint32_t* src, size_t words, cudaStr
   if (words == 0) return;
   ++g_kernel_launches;
   k_dpir_bswap<<<(unsigned)((words + 255) / 256), 256, 0, s>>>(dst, src, words);
+}
+
+void launch_dpir_sum_be(uint32_t* dst, const uint32_t* parts, size_t stride, size_t nparts, size_t words, cudaStream_t s) {
+  if (words == 0) return;
+  if (nparts > 0x7FFFFFFF) throw Error(-2, "dpir: too many partial responses");
+  ++g_kernel_launches;
+  k_dpir_sum_be<<<(unsigned)std::min<size_t>((words + 255) / 256, 132 * 16), 256, 0, s>>>(dst, parts, stride, (int)nparts, words);
 }
 
 }  // namespace b200pir

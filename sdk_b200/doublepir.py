@@ -23,13 +23,30 @@ class PackedMatrix:
             check(LIB.b200pir_dpir_create(device, a.ctypes.data, rows, cols, C.byref(h)))
         else:
             check(LIB.b200pir_dpir_create_synthetic(device, rows, cols, int(synthetic_seed), C.byref(h)))
-        self._h, self.rows, self.cols = h, rows, cols
+        self._h, self.rows, self.cols, self.row_begin = h, rows, cols, 0
 
     @classmethod
-    def _adopt(cls, h, rows, cols):
+    def _adopt(cls, h, rows, cols, row_begin=0):
         m = cls.__new__(cls)
-        m._h, m.rows, m.cols = h, rows, cols
+        m._h, m.rows, m.cols, m.row_begin = h, rows, cols, row_begin
         return m
+
+    @classmethod
+    def shard(cls, a, row_begin, device=0):
+        """A row shard from host words (b200pir_dpir_create_shard): a (rows, cols) uint32 array holding the layout rows
+        [row_begin, row_begin + rows) of a database, e.g. rows of the store a load returned or save_to_files wrote."""
+        a = np.ascontiguousarray(a, dtype=np.uint32)
+        if a.ndim != 2:
+            raise TypeError("a must be a (rows, cols) array")
+        h = C.c_void_p()
+        check(LIB.b200pir_dpir_create_shard(device, a.ctypes.data, int(row_begin), a.shape[0], a.shape[1], C.byref(h)))
+        return cls._adopt(h, a.shape[0], a.shape[1], int(row_begin))
+
+    def shard_info(self):
+        """dict(row_begin, rows, cols, device) as the handle reports it (b200pir_dpir_shard_info)."""
+        r0, rows, cols, dev = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_int()
+        check(LIB.b200pir_dpir_shard_info(self._h, C.byref(r0), C.byref(rows), C.byref(cols), C.byref(dev)))
+        return dict(row_begin=r0.value, rows=rows.value, cols=cols.value, device=dev.value)
 
     def download(self):
         """The packed words back from HBM (rows x cols u32): what server.rs:147-153 saves as `.dbp`."""
@@ -160,8 +177,10 @@ def deserialize_state(buf):
 
 class Server:
     """DoublePirServer::answer / answer_inline (doublepir/server.rs:167-180, 235-247) served from HBM.  db: the PackedMatrix
-    `load` returns (or one chunk's rows, for answer(.., chunk_idx)); borrowed, it must stay open while the server is.
-    h1_squished / a2_t: the host matrices `load` / `setup` return, uploaded once.  max_queries bounds the queries of one call."""
+    `load` returns (or one chunk's rows, for answer(.., chunk_idx)), or the list of row shards `load_sharded` returns, which
+    may live on several devices (answers are byte for byte the one-GPU server's; no chunked answers); borrowed, it must stay
+    open while the server is.  h1_squished / a2_t: the host matrices `load` / `setup` return, uploaded once.  max_queries
+    bounds the queries of one call.  device: that of a single db (a sharded server uses its shards' devices)."""
 
     def __init__(self, db, h1_squished, a2_t, params, num_entries, bits_per_entry, max_queries=32, device=0):
         self.db = db
@@ -169,8 +188,13 @@ class Server:
         h1 = np.ascontiguousarray(h1_squished, dtype=np.uint32)
         a2 = np.ascontiguousarray(a2_t, dtype=np.uint32)
         h = C.c_void_p()
-        check(LIB.b200pir_dpir_server_create(device, C.byref(_params(params)), num_entries, bits_per_entry, db._h, h1.ctypes.data,
-                                             a2.ctypes.data, max_queries, C.byref(h)))
+        if isinstance(db, (list, tuple)):
+            dbs = (C.c_void_p * max(len(db), 1))(*[d._h for d in db])
+            check(LIB.b200pir_dpir_server_create_sharded(C.byref(_params(params)), num_entries, bits_per_entry, dbs, len(db),
+                                                         h1.ctypes.data, a2.ctypes.data, max_queries, C.byref(h)))
+        else:
+            check(LIB.b200pir_dpir_server_create(device, C.byref(_params(params)), num_entries, bits_per_entry, db._h,
+                                                 h1.ctypes.data, a2.ctypes.data, max_queries, C.byref(h)))
         self._h = h
         self._h1_shape = h1.shape
         self._h2_words = h1.shape[0] * int(params["n"]) if h1.ndim == 2 else None     # h2: (n delta x) x n
@@ -341,3 +365,48 @@ def band_bytes(params, num_entries, bits_per_entry, rows, entry_format=ENTRY_BIT
     out = C.c_uint64()
     check(LIB.b200pir_dpir_band_bytes(C.byref(_params(params)), num_entries, bits_per_entry, entry_format, rows, C.byref(out)))
     return out.value
+
+
+def shard_rows(params, num_entries, bits_per_entry, shards):
+    """The row split of a sharded load (b200pir_dpir_shard_rows): [(row_begin, rows)] of each of `shards` shards, whole units
+    of 3x rows, the first U mod G shards one unit longer."""
+    out = []
+    for g in range(shards):
+        r0, rows = C.c_uint64(), C.c_uint64()
+        check(LIB.b200pir_dpir_shard_rows(C.byref(_params(params)), num_entries, bits_per_entry, shards, g, C.byref(r0), C.byref(rows)))
+        out.append((r0.value, rows.value))
+    return out
+
+
+def _sharded(fn, params, num_entries, bits_per_entry, src, src_len, devices, entry_format, scratch_bytes):
+    info = db_info(params, num_entries, bits_per_entry)
+    out = _load_outputs(params, info)
+    k = len(devices)
+    devs = (C.c_int * max(k, 1))(*[int(d) for d in devices])
+    hs = (C.c_void_p * max(k, 1))()
+    args = [devs, k, C.byref(_params(params)), num_entries, bits_per_entry, src] + ([src_len] if src_len is not None else [])
+    check(fn(*args, entry_format, int(scratch_bytes), hs, out["h1_squished"].ctypes.data, out["a2_t"].ctypes.data,
+             out["h2"].ctypes.data))
+    cols = (int(params["m"]) + 2) // 3
+    mats = []
+    for h in hs[:k]:
+        m = PackedMatrix._adopt(C.c_void_p(h), 0, cols)
+        si = m.shard_info()
+        m.rows, m.row_begin = si["rows"], si["row_begin"]
+        mats.append(m)
+    return mats, out, info
+
+
+def load_sharded(params, num_entries, bits_per_entry, data, devices, entry_format=ENTRY_BYTES, scratch_bytes=0):
+    """load() split by rows over len(devices) shards, shard g on devices[g] (a device may repeat): returns (list of
+    PackedMatrix row shards, dict(h1_squished, a2_t, h2), db_info dict), the dict byte for byte load()'s and the shards'
+    downloads, concatenated, its store.  Distinct devices load at once."""
+    data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
+    return _sharded(LIB.b200pir_dpir_load_sharded, params, num_entries, bits_per_entry, data.ctypes.data, data.size, devices,
+                    entry_format, scratch_bytes)
+
+
+def load_file_sharded(params, num_entries, bits_per_entry, path, devices, entry_format=ENTRY_BITS, scratch_bytes=0):
+    """load_sharded() with the raw bytes read from the file at `path`, each shard its own byte range."""
+    return _sharded(LIB.b200pir_dpir_load_file_sharded, params, num_entries, bits_per_entry, os.fsencode(path), None, devices,
+                    entry_format, scratch_bytes)
