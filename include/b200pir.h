@@ -81,6 +81,32 @@ int b200pir_ctx_sizes(b200pir_ctx* ctx, uint64_t* setup_bytes, uint64_t* query_b
  * Multi-GPU row sharding (DESIGN.md): with shard_count = G (a power of two dividing num_per) this GPU holds
  * the second-dimension rows ii = shard_index (mod G); pass 0,1 for the whole database. */
 int b200pir_db_create(b200pir_ctx* ctx, uint64_t shard_index, uint64_t shard_count, b200pir_db** out);
+/* One database over several contexts, served and written from one process: shard g holds the rows ii = g (mod G) on ctxs[g],
+ * laid out as b200pir_db_create(ctxs[g], g, G) lays them out, G = `shards` (a power of two dividing num_per).  The contexts must
+ * be distinct and have identical parameters; their devices may differ or repeat (several shards on one device is valid).  The
+ * layout is resolved once from ctxs[0]'s "db_format" and used for every shard.  G = 1 gives an ordinary database on ctxs[0].
+ * The handle belongs to ctxs[0], the home context, and the member contexts must outlive it; b200pir_db_destroy frees each shard
+ * on its own device.  Peer access is enabled between the home device and each other device where the hardware allows it.
+ *
+ * Queries (process_query, process_query_bytes, process_query_batch, process_queries, process_query_batch_dev), called with the
+ * home context or any context b200pir_db_* accepts for it: the home context expands, each shard runs the first dimension and
+ * the fold rounds nu_2-1 .. log2 G over its rows on its own context's stream (a shard on another device receives the operand by
+ * copy engine), and the home context folds across the shards, packs and encodes.  Responses are byte for byte those of an
+ * unsharded database with the same contents; "sparse_fold" is read from the calling context for every shard.  The _dev call
+ * stays stream-ordered on the calling context's stream.  A call takes the calling context's lock and every member context's,
+ * in creation order.  Workspace: the survivor and receive buffers belong to the database and are sized for 32 queries, growing
+ * for a larger batch; b200pir_ctx_reserve(ctxs[g], Q, num_per / G) sizes each member's, and b200pir_ctx_reserve(ctxs[0], Q,
+ * max(num_per / G, G)) the home's.
+ * Writers (upload, upload_slice, load_file, load_raw_file, fill_synthetic, upsert_item, update_item_raw, update_many_items)
+ * read their input once and give each shard its rows; a single-item write touches only the owning shard.  download,
+ * download_slice and save_file assemble every shard's rows; present_items sums over the shards (capacity = the whole database);
+ * db_info reports local_rows = num_per and hbm_bytes summed over the shards.
+ * Refused with B200PIR_E_UNSUPPORTED: multiply_reg_by_database, query_stage_a_dev, first_dim_fold_dev and
+ * first_dim_fold_images_dev (the multi-process building blocks take rank shards from b200pir_db_create).
+ * Errors: null pointers, a repeated context or contexts with different parameters -> B200PIR_E_BADARG; a shard count that is not
+ * a power of two dividing num_per -> B200PIR_E_BADARG as b200pir_db_create; no handle is returned and no device memory stays
+ * allocated on any error. */
+int b200pir_db_create_sharded(b200pir_ctx* const* ctxs, size_t shards, b200pir_db** out);
 void b200pir_db_destroy(b200pir_db* db);
 /* Upload one (instance,trial) slice in the reference layout [z][ii][j] (server.rs:263-266). */
 int b200pir_db_upload_slice(b200pir_ctx* ctx, b200pir_db* db, uint64_t slice, const uint64_t* words, size_t n_words);
@@ -127,7 +153,8 @@ int b200pir_db_download(b200pir_ctx* ctx, b200pir_db* db, uint64_t* words, size_
 /* Write the whole database to `path` as the native-endian u64 stream that b200pir_db_load_file and the reference's
  * load_preprocessed_db_from_file read.  Atomic: the words go to a temporary file in the same directory (mode 0600), which is
  * fsync'ed and renamed over `path`; if the save fails, an earlier file at `path` is intact and no temporary file is left.
- * Locking as b200pir_db_download.  Unsharded databases only (B200PIR_E_UNSUPPORTED otherwise); a file that cannot be created
+ * Locking as b200pir_db_download.  Whole databases only, unsharded or from b200pir_db_create_sharded (whose chunks are
+ * assembled on the host from every shard's export, one staging chunk at a time); a rank shard -> B200PIR_E_UNSUPPORTED; a file that cannot be created
  * or written -> B200PIR_E_BADARG, with the path in b200pir_last_error(). */
 int b200pir_db_save_file(b200pir_ctx* ctx, b200pir_db* db, const char* path);
 /* Synthetic database generated on the GPU: plaintext coefficient = splitmix64(seed, ((slice*items+item)*2048+z)) % p,

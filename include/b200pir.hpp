@@ -80,6 +80,13 @@ struct Database {
   explicit Database(const Params& p, uint64_t shard_index = 0, uint64_t shard_count = 1) : params(p) {
     check(b200pir_db_create(p.ctx, shard_index, shard_count, &h));
   }
+  // one database in row shards over several contexts (b200pir_db_create_sharded): shard g on members[g], the first one the
+  // home context that the query functions are called with
+  explicit Database(const std::vector<const Params*>& members) : params(*members.at(0)) {
+    std::vector<b200pir_ctx*> ctxs;
+    for (const Params* m : members) ctxs.push_back(m->ctx);
+    check(b200pir_db_create_sharded(ctxs.data(), ctxs.size(), &h));
+  }
   Database(const Params& p, const uint64_t* words, size_t n_words) : Database(p) {
     check(b200pir_db_upload(p.ctx, h, words, n_words));
   }
@@ -102,7 +109,7 @@ struct Database {
     download(w.data(), w.size());
     return w;
   }
-  // the file b200pir_db_load_file reads, written atomically (unsharded databases)
+  // the file b200pir_db_load_file reads, written atomically (whole databases: unsharded or over several contexts)
   void save_file(const char* path) const { check(b200pir_db_save_file(params.ctx, h, path)); }
 };
 

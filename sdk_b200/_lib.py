@@ -44,6 +44,7 @@ def _load():
         "b200pir_ctx_reserve": (C.c_int, [vp, C.c_size_t, C.c_size_t]),
         "b200pir_ctx_sizes": (C.c_int, [vp, C.POINTER(C.c_uint64)] + [C.POINTER(C.c_uint64)] * 2),
         "b200pir_db_create": (C.c_int, [vp, C.c_uint64, C.c_uint64, C.POINTER(vp)]),
+        "b200pir_db_create_sharded": (C.c_int, [C.POINTER(vp), C.c_size_t, C.POINTER(vp)]),
         "b200pir_db_destroy": (None, [vp]),
         "b200pir_db_upload_slice": (C.c_int, [vp, vp, C.c_uint64, u64p, C.c_size_t]),
         "b200pir_db_upload": (C.c_int, [vp, vp, u64p, C.c_size_t]),

@@ -5,6 +5,7 @@
 #include "spiral_api.hpp"
 #include "ntt_tables.hpp"
 #include "gadget.hpp"
+#include <atomic>
 #include <cmath>
 #include <memory>
 #include <set>
@@ -191,15 +192,16 @@ void run_fold(b200pir_ctx* c, uint64_t* cts, size_t batch, size_t batch_stride, 
 }
 
 // Fast path on residue-form ciphertexts: ping-pong between `a` (input of the first round) and `b`.
-// Returns the buffer holding the survivors (entry 0 of each batch element).
+// Returns the buffer holding the survivors (entry 0 of each batch element).  `sparse`: lib/server's fold shortcut (the
+// "sparse_fold" option of the context whose call this is).
 const uint32_t* run_fold_res(b200pir_ctx* c, uint32_t* a, uint32_t* b, size_t batch, size_t batch_stride, size_t num,
-                             int k0, const uint32_t* vfold, int slices_per_query) {
+                             int k0, const uint32_t* vfold, int slices_per_query, bool sparse) {
   const size_t mat = (size_t)2 * 2 * c->hp.t_gsw * 2 * POLY;
   int k = k0;
   uint32_t* src = a;
   uint32_t* dst = b;
   uint32_t* zero_flags = nullptr;                      // lib/server's fold shortcut (fold.rs:37-43) when "sparse_fold" is set
-  if (c->sparse_fold) {
+  if (sparse) {
     c->w_zflags.ensure(batch * num);
     zero_flags = c->w_zflags.p;
   }
@@ -277,10 +279,10 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
   }
 }
 
-// first dimension (operand qdev or `images`) + from_ntt + local fold with the folding matrices vfold; returns the survivors
-// (in w_mult or w_cts), one per (query, slice)
+// first dimension (operand qdev or `images`) + from_ntt + local fold with the folding matrices vfold (fold shortcut when
+// `sparse`); returns the survivors (in w_mult or w_cts), one per (query, slice)
 Survivors run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, Images images,
-                                 const uint32_t* vfold) {
+                                 const uint32_t* vfold, bool sparse) {
   const int rows = db->rows;
   const size_t out_stride = (size_t)c->slices * rows * 4 * POLY;
   // server.rs:707-709 from_ntt, minus the CRT lift, into w_mult in residue form: a z-major product goes to w_cts (free until
@@ -294,7 +296,7 @@ Survivors run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, c
   }
   b200pir_ctx::Scope sc(c, ST_FOLD);
   Survivors s{c->w_mult.p, (size_t)rows * 4 * POLY};
-  if (rows > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, rows, (int)c->hp.nu_2 - 1, vfold, c->slices);
+  if (rows > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, rows, (int)c->hp.nu_2 - 1, vfold, c->slices, sparse);
   return s;
 }
 
@@ -334,6 +336,8 @@ int b200pir_ctx_create(const b200pir_params* params, int device, b200pir_ctx** o
   if (!params || !out) throw Error(B200PIR_E_BADARG, "null argument");
   use_device(device);
   std::unique_ptr<b200pir_ctx> c(new b200pir_ctx());
+  static std::atomic<uint64_t> next_seq{0};
+  c->seq = next_seq++;
   c->device = device;
   B200_CUDA(cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device));
   c->hp = *params;
@@ -728,6 +732,7 @@ int b200pir_multiply_reg_by_database(b200pir_ctx* c, b200pir_db* db, uint64_t sl
   if (!c || !v_firstdim || !out) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
+  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "multiply_reg_by_database: not on a sharded database");
   if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
   const int rows = db->rows;
   const bool zmajor = db->zmajor_product();
@@ -900,14 +905,90 @@ struct Responses {
   size_t* len = nullptr;
 };
 
+// the survivors `s`, [count][slices], into partial_dev as a dense buffer of residue-form ciphertexts; partial_dev may be on
+// another device (a part of a sharded database gathering to the home device)
+void gather_survivors(b200pir_ctx* c, Survivors s, size_t count, uint32_t* partial_dev) {
+  B200_CUDA(cudaMemcpy2DAsync(partial_dev, 4 * POLY * 4, s.p, s.stride * 4, 4 * POLY * 4, count * c->slices,
+                              cudaMemcpyDefault, c->stream));
+}
+
+// The last phase for queries [first, first + count) of the `total_count` whose partial survivors `world` ranks gathered: their
+// fold across the ranks with the folding matrices v_folding, then pack and encode into out_dev
+void run_finish(b200pir_ctx* c, Keys keys, const uint32_t* gathered_dev, size_t world, size_t total_count, size_t first,
+                size_t count, const uint32_t* v_folding, uint8_t* out_dev) {
+  // gathered: [world][total_count][slices][ct]  ->  w_mult as [count][slices][world][ct]   (ct = 4*2048 u32)
+  const size_t ct = 4 * POLY;
+  for (size_t w = 0; w < world; w++)
+    B200_CUDA(cudaMemcpy2DAsync(c->w_mult.p + w * ct, world * ct * 4, gathered_dev + (w * total_count + first) * c->slices * ct,
+                                ct * 4, ct * 4, count * c->slices, cudaMemcpyDeviceToDevice, c->stream));
+  int dims = 0;
+  while (((size_t)1 << dims) < world) dims++;
+  Survivors s{c->w_mult.p, world * ct};
+  {
+    b200pir_ctx::Scope sc(c, ST_FOLD);
+    if (world > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, world, dims - 1, v_folding, c->slices, c->sparse_fold);
+  }
+  run_pack_encode(c, keys, s, count, out_dev);
+}
+
+// The query schedule of a sharded database (b200pir_db_create_sharded) once the calling context c, the home, has put the
+// call's first-dimension operand (`images`, or c->w_qdev) and folding matrices (c->w_vfold) in place: every part runs the
+// first dimension and the fold rounds nu_2 - 1 .. log2 G on its rows, on its own context's stream, and gathers its survivors
+// into slot g of db->gathered; c then folds across the parts (rounds log2 G - 1 .. 0), packs and encodes into out_dev.  A part
+// on c's device reads c's buffers directly; a part on another device receives them in its own buffers by copy engine.
+// Options that change the response bytes ("sparse_fold") are c's for every part.
+//
+// Stream order, with no host synchronisation:
+//  - Every part's stream waits on db->expanded, recorded on c's stream after the expansion, before it copies or reads the
+//    operands; c's stream waits on every part's `done`, recorded after the part's gather, before the finish.  So the next
+//    call's expansion, queued on c's stream after this finish, cannot overwrite an operand a part is still copying or reading.
+//    A call from another context on the home device first waits on db->finished, which carries the same order over.
+//  - A part's receive buffers are written only by copies on the part's own stream, queued after that stream's previous first
+//    dimension, which read them: the copies of the next call cannot overtake it.
+//  - db->gathered is written by the parts after db->expanded and read by the finish before db->finished, so the next call's
+//    gathers come after this call's finish has read it.
+void run_shards(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, Images images, uint8_t* out_dev) {
+  const size_t G = db->parts.size();
+  db->ensure_exchange(count);
+  const size_t op_bytes = db->operand_bytes(count), fold_bytes = count * c->fold_words() * 4;
+  const uint8_t* op = images.p ? images.p : reinterpret_cast<const uint8_t*>(c->w_qdev.p);
+  B200_CUDA(cudaEventRecord(db->expanded, c->stream));
+  for (size_t g = 0; g < G; g++) {
+    b200pir_db::Part& part = db->parts[g];
+    b200pir_ctx* x = part.db->ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    if (x->stream != c->stream) B200_CUDA(cudaStreamWaitEvent(x->stream, db->expanded, 0));
+    const uint8_t* xop = op;
+    const uint32_t* xfold = c->w_vfold.p;
+    if (x->device != c->device) {
+      B200_CUDA(cudaMemcpyPeerAsync(part.operand.p, x->device, op, c->device, op_bytes, x->stream));
+      if (fold_bytes) B200_CUDA(cudaMemcpyPeerAsync(part.vfold.p, x->device, c->w_vfold.p, c->device, fold_bytes, x->stream));
+      xop = part.operand.p;
+      xfold = part.vfold.p;
+    }
+    x->ensure_workspace_lite(count, part.db->rows);
+    const Images xim{images.p ? xop : nullptr, images.per_group};
+    const Survivors s = run_first_dim_and_fold(x, part.db.get(), count, images.p ? nullptr : reinterpret_cast<const uint4*>(xop),
+                                               xim, xfold, c->sparse_fold);
+    gather_survivors(x, s, count, db->gathered.p + g * count * c->slices * 4 * POLY);
+    B200_CUDA(cudaEventRecord(part.done, x->stream));
+  }
+  B200_CUDA(cudaSetDevice(c->device));
+  for (const auto& part : db->parts)
+    if (part.db->ctx->stream != c->stream) B200_CUDA(cudaStreamWaitEvent(c->stream, part.done, 0));
+  run_finish(c, keys, db->gathered.p, G, count, 0, count, c->w_vfold.p, out_dev);
+  B200_CUDA(cudaEventRecord(db->finished, c->stream));
+}
+
 // One single-GPU query call on `count` queries: the checks, stage(), which puts the queries into the workspace (w_query, or
 // w_qdev and w_vfold for direct upload), one database pass and the responses.  `keys.each`: a multi-client batch, whose
 // workspace is sized once for a full coalesced batch (batch sizes vary from call to call, the buffers do not).
 // `needs_expand`: the queries are ciphertexts, which only an expanding context takes.
+// A sharded database runs the same checks and staging and then run_shards in place of the one-context database pass.
 template <typename Stage>
 void run_queries(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, bool needs_expand, Stage stage,
                  const Responses& out) {
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   if (keys.each)
     for (size_t i = 0; i < count; i++) check_pp(c, keys.each[i]);
@@ -917,14 +998,19 @@ void run_queries(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, bool n
   if (needs_expand && !c->hp.expand_queries)
     throw Error(B200PIR_E_BADARG, keys.each ? "multi-client batches need expand_queries" : "batch entry point needs expand_queries");
   if (count == 0) return;
-  c->ensure_workspace(keys.each && c->coalesce ? std::max(count, b200pir_ctx::kCoalesceMax) : count, db->rows);
+  // a sharded database's home workspace holds the finish's G survivors per (query, slice), not local rows
+  const size_t rows = db->sharded() ? db->parts.size() : (size_t)db->rows;
+  c->ensure_workspace(keys.each && c->coalesce ? std::max(count, b200pir_ctx::kCoalesceMax) : count, rows);
   c->prof_reset();
+  if (db->sharded()) B200_CUDA(cudaStreamWaitEvent(c->stream, db->finished, 0));
   stage();
   // format-2 databases get their operand as tile images straight from the expansion
   const bool images = db->layout.format == 2 && c->hp.expand_queries;
   run_prepare(c, keys, count, images);
-  const Survivors s = run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{images ? c->w_qt.p : nullptr, 16}, c->w_vfold.p);
-  run_pack_encode(c, keys, s, count, out.dev ? out.dev : c->w_resp.p);
+  const Images im{images ? c->w_qt.p : nullptr, 16};
+  uint8_t* resp = out.dev ? out.dev : c->w_resp.p;
+  if (db->sharded()) run_shards(c, db, keys, count, im, resp);
+  else run_pack_encode(c, keys, run_first_dim_and_fold(c, db, count, c->w_qdev.p, im, c->w_vfold.p, c->sparse_fold), count, resp);
   if (!out.dev) {
     const size_t rb = c->response_bytes;
     if (out.each)
@@ -1094,31 +1180,6 @@ int b200pir_process_query(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, const 
 // ---- multi-GPU building blocks: the three phases with caller-owned device buffers in between, so the host can put a
 // collective between them (bench.py: queries are expanded by the rank that received them, everything is all-gathered)
 namespace {
-// the survivors `s`, [count][slices], into partial_dev as a dense buffer of residue-form ciphertexts
-void gather_survivors(b200pir_ctx* c, Survivors s, size_t count, uint32_t* partial_dev) {
-  B200_CUDA(cudaMemcpy2DAsync(partial_dev, 4 * POLY * 4, s.p, s.stride * 4, 4 * POLY * 4, count * c->slices,
-                              cudaMemcpyDeviceToDevice, c->stream));
-}
-
-// The last phase for queries [first, first + count) of the `total_count` whose partial survivors `world` ranks gathered: their
-// fold across the ranks with the folding matrices v_folding, then pack and encode into out_dev
-void run_finish(b200pir_ctx* c, Keys keys, const uint32_t* gathered_dev, size_t world, size_t total_count, size_t first,
-                size_t count, const uint32_t* v_folding, uint8_t* out_dev) {
-  // gathered: [world][total_count][slices][ct]  ->  w_mult as [count][slices][world][ct]   (ct = 4*2048 u32)
-  const size_t ct = 4 * POLY;
-  for (size_t w = 0; w < world; w++)
-    B200_CUDA(cudaMemcpy2DAsync(c->w_mult.p + w * ct, world * ct * 4, gathered_dev + (w * total_count + first) * c->slices * ct,
-                                ct * 4, ct * 4, count * c->slices, cudaMemcpyDeviceToDevice, c->stream));
-  int dims = 0;
-  while (((size_t)1 << dims) < world) dims++;
-  Survivors s{c->w_mult.p, world * ct};
-  {
-    b200pir_ctx::Scope sc(c, ST_FOLD);
-    if (world > 1) s.p = run_fold_res(c, c->w_mult.p, c->w_cts.p, count * c->slices, s.stride, world, dims - 1, v_folding, c->slices);
-  }
-  run_pack_encode(c, keys, s, count, out_dev);
-}
-
 // The expansion phase of `count` queries into the caller's buffers: the first-dimension operand as q_dev or, with `images`, as
 // the tile images of one group of 1..16 queries; the folding matrices into v_folding_dev
 int expand_dev(b200pir_ctx* c, b200pir_pp* pp, const uint64_t* query_cts_dev, size_t count, void* operand_dev,
@@ -1152,6 +1213,7 @@ int first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* operand_dev, 
   if (!c || !operand_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
+  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "a sharded database runs its own schedule: use the query entry points");
   if (images) {
     if (db->layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
     if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
@@ -1160,7 +1222,7 @@ int first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* operand_dev, 
   c->ensure_workspace_lite(count, db->rows);
   const uint4* qdev = images ? nullptr : (const uint4*)operand_dev;
   const Images im{images ? (const uint8_t*)operand_dev : nullptr, per_group};
-  gather_survivors(c, run_first_dim_and_fold(c, db, count, qdev, im, v_folding_dev), count, partial_dev);
+  gather_survivors(c, run_first_dim_and_fold(c, db, count, qdev, im, v_folding_dev, c->sparse_fold), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -1207,12 +1269,13 @@ int b200pir_query_stage_a_dev(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, co
   Guard gd(c);
   check_db(c, db);
   check_pp(c, pp);
+  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "a sharded database runs its own schedule: use the query entry points");
   if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "needs expand_queries");
   c->ensure_workspace(count, db->rows);
   c->prof_reset();
   B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_cts_dev, count * 2 * POLY * 8, cudaMemcpyDeviceToDevice, c->stream));
   run_prepare(c, Keys{pp}, count, false);
-  gather_survivors(c, run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{}, c->w_vfold.p), count, partial_dev);
+  gather_survivors(c, run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{}, c->w_vfold.p, c->sparse_fold), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }

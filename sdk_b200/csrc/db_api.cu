@@ -1,6 +1,7 @@
 // C-ABI implementation of the HBM-resident database handle (include/b200pir.h): creation, bulk uploads and file loads,
 // exports, the item writers and the presence map.  Every writer places items through the same three decisions: which GPU owns
 // an item (Shard::local_item), the context's write staging (w_wbytes) and the presence update (mark_items / mark_slices).
+// A sharded handle (b200pir_db_create_sharded) runs each of them once per part, on the part's context, from inputs read once.
 #include "spiral_api.hpp"
 #include "update_body.hpp"
 #include <cstdio>
@@ -39,7 +40,60 @@ void b200pir_db::mark_slices(int slice_begin, int slice_end, cudaStream_t s) {
   B200_CUDA(cudaMemcpyAsync(tile_mask.p + w0, &h_tile_mask[w0], (w1 - w0) * 4, cudaMemcpyHostToDevice, s));
 }
 
+b200pir_db::~b200pir_db() {
+  if (parts.empty()) return;
+  for (auto& p : parts) {
+    if (!p.db) continue;
+    cudaSetDevice(p.db->ctx->device);
+    if (p.done) cudaEventDestroy(p.done);
+    p.operand.release();
+    p.vfold.release();
+    p.db.reset();
+  }
+  cudaSetDevice(ctx->device);
+  if (expanded) cudaEventDestroy(expanded);
+  if (finished) cudaEventDestroy(finished);
+}
+
+// Bytes of the first-dimension operand of `queries` queries as the query path hands it to a part: tile images of 16 queries
+// for a format-2 database whose queries are expanded, q_dev otherwise
+size_t b200pir_db::operand_bytes(size_t queries) const {
+  if (layout.format == 2 && ctx->hp.expand_queries) return (queries + 15) / 16 * tc5_query_bytes(make_tc5_geom(ctx->dim0, 32));
+  return queries * ctx->dim0 * POLY * sizeof(uint4);
+}
+
+// The survivor buffer and the receive buffers of the other-device parts, for `queries` queries.  Replacing them waits for every
+// part's stream and the last finish, so no call still in flight uses them.  Leaves the home device current.
+void b200pir_db::ensure_exchange(size_t queries) {
+  if (queries <= exchange_queries) return;
+  for (auto& p : parts) {
+    B200_CUDA(cudaSetDevice(p.db->ctx->device));
+    B200_CUDA(cudaStreamSynchronize(p.db->ctx->stream));
+  }
+  B200_CUDA(cudaSetDevice(ctx->device));
+  B200_CUDA(cudaEventSynchronize(finished));
+  gathered.alloc(parts.size() * queries * ctx->slices * 4 * POLY);
+  for (auto& p : parts) {
+    if (p.db->ctx->device == ctx->device) continue;
+    B200_CUDA(cudaSetDevice(p.db->ctx->device));
+    p.operand.alloc(operand_bytes(queries));
+    p.vfold.alloc(queries * ctx->fold_words());
+  }
+  B200_CUDA(cudaSetDevice(ctx->device));
+  exchange_queries = queries;
+}
+
 namespace {
+
+// Where a writer or an export of `db` called on context c does its work: (c, db) for an ordinary database or a rank shard,
+// (part context, part) for every part of a sharded one
+struct Member { b200pir_ctx* ctx; b200pir_db* db; };
+std::vector<Member> members(b200pir_ctx* c, b200pir_db* db) {
+  if (!db->sharded()) return {Member{c, db}};
+  std::vector<Member> ms;
+  for (auto& p : db->parts) ms.push_back(Member{p.db->ctx, p.db.get()});
+  return ms;
+}
 
 // One slice in the reference's z-major layout, delivered chunk by chunk: fetch(word_offset, n_words) returns a host pointer
 // to that range of the slice (valid until the next call).
@@ -47,19 +101,31 @@ template <typename Fetch>
 void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fetch) {
   // reference layout is z-major: stage a range of z at a time in the writers' staging (w_wbytes, at least 64 MiB).  An export
   // may still be copying its last chunk out of it; that copy is queued on the context's stream, ahead of this upload's copies.
+  // Each range is fetched once and staged to every member (a pageable copy has taken its source when it returns).
+  const std::vector<Member> ms = members(c, db);
   const size_t per_z = (size_t)c->dim0 * c->num_per;
   int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
-  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, per_z * zc * 8));
-  uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
+  for (const Member& m : ms) {
+    B200_CUDA(cudaSetDevice(m.ctx->device));
+    m.ctx->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, per_z * zc * 8));
+  }
   for (int z0 = 0; z0 < POLY; z0 += zc) {
     int cur = std::min(zc, POLY - z0);
     const uint64_t* src = fetch((size_t)z0 * per_z, per_z * cur);
-    B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, c->stream));
-    launch_db_import(db->layout, db->shard, (int)slice, stage, z0, cur, c->stream);
-    B200_CUDA(cudaStreamSynchronize(c->stream));
+    for (const Member& m : ms) {
+      B200_CUDA(cudaSetDevice(m.ctx->device));
+      uint64_t* stage = reinterpret_cast<uint64_t*>(m.ctx->w_wbytes.p);
+      B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, m.ctx->stream));
+      launch_db_import(m.db->layout, m.db->shard, (int)slice, stage, z0, cur, m.ctx->stream);
+    }
+    for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   }
-  db->mark_slices((int)slice, (int)slice + 1, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));
+  for (const Member& m : ms) {
+    B200_CUDA(cudaSetDevice(m.ctx->device));
+    m.db->mark_slices((int)slice, (int)slice + 1, m.ctx->stream);
+    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
+  }
+  B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
 }
 
@@ -80,52 +146,76 @@ void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t spa
 // [zc][rows][dim0] u64 there and the chunk is queued for a copy to one of the two pinned buffers; the lock is then released and
 // `sink(slice, z0, zc, words)` consumes the previous chunk once its copy has landed, while the GPU un-tiles and copies this
 // one.  Everything is ordered on the context's stream, so a chunk's un-tiling never overwrites staging its copy still reads.
+// A sharded database exports each chunk from every part, on the part's context, and `words[g]` is part g's.
 template <typename Sink>
 void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
-  std::lock_guard<std::mutex> ex(c->export_mu);
-  const size_t per_z = (size_t)db->rows * c->dim0;
+  const std::vector<Member> ms = members(c, db);
+  std::vector<b200pir_ctx*> order;
+  for (const Member& m : ms) order.push_back(m.ctx);
+  std::sort(order.begin(), order.end(), [](const b200pir_ctx* a, const b200pir_ctx* b) { return a->seq < b->seq; });
+  std::vector<std::unique_lock<std::mutex>> ex;
+  for (b200pir_ctx* x : order) ex.emplace_back(x->export_mu);
+  const size_t per_z = (size_t)ms[0].db->rows * c->dim0;
   const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
   struct Chunk { int slice, z0, zc; };
   std::vector<Chunk> chunks;
   for (int s = slice_begin; s < slice_end; s++)
     for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
-  {
-    Guard gd(c);
-    c->ensure_export_staging(per_z * zc * 8);
+  for (const Member& m : ms) {
+    Guard gd(m.ctx);
+    m.ctx->ensure_export_staging(per_z * zc * 8);
   }
+  std::vector<const uint64_t*> src(ms.size());
   auto consume = [&](size_t k) {
     const int b = (int)(k & 1);
-    B200_CUDA(cudaEventSynchronize(c->export_done[b]));
-    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<const uint64_t*>(c->h_export[b]));
+    for (size_t g = 0; g < ms.size(); g++) {
+      B200_CUDA(cudaEventSynchronize(ms[g].ctx->export_done[b]));
+      src[g] = reinterpret_cast<const uint64_t*>(ms[g].ctx->h_export[b]);
+    }
+    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, src);
   };
   try {
     for (size_t k = 0; k < chunks.size(); k++) {
-      {
-        Guard gd(c);
-        uint64_t* stage = reinterpret_cast<uint64_t*>(c->w_wbytes.p);
-        launch_db_export(db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, c->stream);
-        B200_CUDA(cudaMemcpyAsync(c->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, c->stream));
-        B200_CUDA(cudaEventRecord(c->export_done[k & 1], c->stream));
+      for (const Member& m : ms) {
+        Guard gd(m.ctx);
+        b200pir_ctx* x = m.ctx;
+        uint64_t* stage = reinterpret_cast<uint64_t*>(x->w_wbytes.p);
+        launch_db_export(m.db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, x->stream);
+        B200_CUDA(cudaMemcpyAsync(x->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, x->stream));
+        B200_CUDA(cudaEventRecord(x->export_done[k & 1], x->stream));
       }
       if (k > 0) consume(k - 1);
     }
     if (!chunks.empty()) consume(chunks.size() - 1);
   } catch (...) {
-    for (auto e : c->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
+    for (const Member& m : ms)
+      for (auto e : m.ctx->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
+    cudaSetDevice(c->device);
     throw;
   }
+  B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
+}
+
+// Chunk (zc values of z) of every member, `src[g]` being member g's [zc][rows][dim0], scattered into `dst`, the same range of z
+// of a slice in the reference layout [z][num_per][dim0]
+void scatter_rows(b200pir_ctx* c, const std::vector<Member>& ms, int zc, const std::vector<const uint64_t*>& src, uint64_t* dst) {
+  const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per;
+  for (size_t g = 0; g < ms.size(); g++) {
+    const b200pir_db* m = ms[g].db;
+    const size_t rows = (size_t)m->rows;
+    if (m->shard.count == 1) { std::memcpy(dst, src[g], (size_t)zc * rows * d0 * 8); continue; }
+    for (size_t zl = 0; zl < (size_t)zc; zl++)
+      for (size_t il = 0; il < rows; il++)
+        std::memcpy(dst + (zl * npg + m->shard.global_row(il)) * d0, src[g] + (zl * rows + il) * d0, d0 * 8);
+  }
 }
 
 // the local rows of slices [slice_begin, slice_end) into `words` (the reference layout of those slices)
 void download_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, uint64_t* words) {
-  const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per, rows = (size_t)db->rows;
-  export_impl(c, db, slice_begin, slice_end, [&](int s, int z0, int zc, const uint64_t* src) {
-    uint64_t* dst = words + (size_t)(s - slice_begin) * c->slice_words + (size_t)z0 * npg * d0;
-    if (db->shard.count == 1) { std::memcpy(dst, src, (size_t)zc * rows * d0 * 8); return; }
-    for (size_t zl = 0; zl < (size_t)zc; zl++)
-      for (size_t il = 0; il < rows; il++)
-        std::memcpy(dst + (zl * npg + db->shard.global_row(il)) * d0, src + (zl * rows + il) * d0, d0 * 8);
+  const std::vector<Member> ms = members(c, db);
+  export_impl(c, db, slice_begin, slice_end, [&](int s, int z0, int zc, const std::vector<const uint64_t*>& src) {
+    scatter_rows(c, ms, zc, src, words + (size_t)(s - slice_begin) * c->slice_words + (size_t)z0 * c->num_per * c->dim0);
   });
 }
 
@@ -142,13 +232,11 @@ std::pair<std::unique_ptr<FILE, int (*)(FILE*)>, off_t> open_sized(const char* p
 
 extern "C" {
 
-int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, b200pir_db** out) {
-  API_BEGIN
-  if (!c || !out) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
-  if (shard_count == 0) { shard_count = 1; shard_index = 0; }
-  if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)c->num_per % shard_count)
-    throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+}  // extern "C"
+
+namespace {
+// Rows ii = shard_index (mod shard_count) on context c in layout `format` (-1: automatic); c's lock is held
+std::unique_ptr<b200pir_db> create_db(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, int format) {
   std::unique_ptr<b200pir_db> db(new b200pir_db());
   db->ctx = c;
   db->shard = Shard{(int)shard_index, (int)shard_count};
@@ -157,7 +245,7 @@ int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count
   L.G = c->geom(db->rows);
   L.F = make_imma_geom(c->dim0, db->rows);
   L.T = make_tc5_geom(c->dim0, db->rows);
-  L.format = c->db_format >= 0 ? c->db_format : (tc5_supported(L.T) ? 2 : 1);
+  L.format = format >= 0 ? format : (tc5_supported(L.T) ? 2 : 1);
   db->present.assign((db->capacity() + 63) / 64, 0);
   db->h_tile_mask.assign((size_t)c->slices * L.T.mt, 0u);
   db->tile_mask.alloc(db->h_tile_mask.size());
@@ -169,19 +257,92 @@ int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count
   L.base = db->store.p;
   B200_CUDA(cudaMemsetAsync(db->store.p, 0, db->store.n, c->stream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
+  return db;
+}
+
+void check_shard_count(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count) {
+  if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)c->num_per % shard_count)
+    throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+}
+
+// lets the current device reach `peer`'s memory directly where the hardware allows it
+void enable_peer(int device, int peer) {
+  int can = 0;
+  B200_CUDA(cudaDeviceCanAccessPeer(&can, device, peer));
+  if (!can) return;
+  B200_CUDA(cudaSetDevice(device));
+  const cudaError_t e = cudaDeviceEnablePeerAccess(peer, 0);
+  if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+  else B200_CUDA(e);
+}
+}  // namespace
+
+extern "C" {
+
+int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, b200pir_db** out) {
+  API_BEGIN
+  if (!c || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  Guard gd(c);
+  if (shard_count == 0) { shard_count = 1; shard_index = 0; }
+  check_shard_count(c, shard_index, shard_count);
+  *out = create_db(c, shard_index, shard_count, c->db_format).release();
+  API_END
+}
+int b200pir_db_create_sharded(b200pir_ctx* const* ctxs, size_t shards, b200pir_db** out) {
+  API_BEGIN
+  if (!ctxs || !out) throw Error(B200PIR_E_BADARG, "null argument");
+  if (shards == 0) throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+  for (size_t g = 0; g < shards; g++) {
+    if (!ctxs[g]) throw Error(B200PIR_E_BADARG, "null context");
+    for (size_t h = 0; h < g; h++)
+      if (ctxs[h] == ctxs[g]) throw Error(B200PIR_E_BADARG, "a context appears more than once");
+    if (std::memcmp(&ctxs[g]->hp, &ctxs[0]->hp, sizeof(b200pir_params)) != 0)
+      throw Error(B200PIR_E_BADARG, "the contexts of a sharded database must have identical parameters");
+  }
+  b200pir_ctx* home = ctxs[0];
+  int format;
+  {
+    Guard gd(home);
+    check_shard_count(home, 0, shards);
+    format = home->db_format;
+    if (shards == 1) { *out = create_db(home, 0, 1, format).release(); return 0; }
+  }
+  std::unique_ptr<b200pir_db> db(new b200pir_db());
+  db->ctx = home;
+  db->shard = Shard{0, 1};
+  db->rows = home->num_per;
+  db->parts = std::vector<b200pir_db::Part>(shards);     // Part holds device buffers: built in place, never moved
+  for (size_t g = 0; g < shards; g++) {
+    b200pir_ctx* c = ctxs[g];
+    Guard gd(c);
+    b200pir_db::Part& p = db->parts[g];
+    p.db = create_db(c, g, shards, format);
+    B200_CUDA(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
+    if (c->device != home->device) {
+      enable_peer(c->device, home->device);
+      enable_peer(home->device, c->device);
+    }
+  }
+  Guard gd(home, db.get());
+  db->layout = db->parts[0].db->layout;
+  db->layout.base = nullptr;
+  B200_CUDA(cudaEventCreateWithFlags(&db->expanded, cudaEventDisableTiming));
+  B200_CUDA(cudaEventCreateWithFlags(&db->finished, cudaEventDisableTiming));
+  B200_CUDA(cudaEventRecord(db->finished, home->stream));
+  db->ensure_exchange(b200pir_ctx::kCoalesceMax);
   *out = db.release();
   API_END
 }
 void b200pir_db_destroy(b200pir_db* db) {
   if (!db) return;
   cudaSetDevice(db->ctx->device);
-  delete db;
+  delete db;                                  // a sharded database frees each part on its own device
 }
 
 int b200pir_db_upload_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, const uint64_t* words, size_t n_words) {
   API_BEGIN
   if (!c || !words) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
   if (n_words != c->slice_words) throw Error(B200PIR_E_SHAPE, "slice must hold dim0*num_per*2048 words");
@@ -193,7 +354,7 @@ int b200pir_db_upload_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, cons
 int b200pir_db_load_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   API_BEGIN
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   const auto [file, bytes] = open_sized(path);
   if (bytes < 0 || (uint64_t)bytes != (uint64_t)c->slice_words * c->slices * 8)
@@ -243,6 +404,7 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
   check_db(c, db);
   if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
+  const std::vector<Member> ms = members(c, db);
   const std::string target(path);
   std::string tmp = target + ".tmp.XXXXXX";
   const int fd = mkstemp(&tmp[0]);
@@ -258,9 +420,17 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   };
   if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
   try {
-    export_impl(c, db, 0, c->slices, [&](int, int, int zc, const uint64_t* src) {
-      const size_t n = (size_t)zc * db->rows * c->dim0;
-      if (fwrite(src, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
+    // a sharded database's chunk is assembled from its parts' exports first: host memory stays bounded by the staging
+    std::vector<uint64_t> whole;
+    export_impl(c, db, 0, c->slices, [&](int, int, int zc, const std::vector<const uint64_t*>& src) {
+      const size_t n = (size_t)zc * c->num_per * c->dim0;
+      const uint64_t* words = src[0];
+      if (db->sharded()) {
+        whole.resize(n);
+        scatter_rows(c, ms, zc, src, whole.data());
+        words = whole.data();
+      }
+      if (fwrite(words, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
     });
   } catch (const Error& e) {
     discard(e.what(), e.code);
@@ -282,36 +452,45 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
 int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
   API_BEGIN
   if (!c || !poly) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   if (slice >= (uint64_t)c->slices || item_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "index out of range");
-  int il, j;
-  if (!db->shard.local_item(item_idx, c->num_per, il, j)) return 0;       // row lives on another GPU
-  c->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like write_items
-  B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, poly, POLY * 8, cudaMemcpyHostToDevice, c->stream));
-  launch_db_upsert(db->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(c->w_wbytes.p), c->stream);
-  const ItemWrite item{0, 0, (uint32_t)il, (uint32_t)j};
-  db->mark_items(&item, 1, (int)slice, (int)slice + 1, c->stream);
-  // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
-  B200_CUDA(cudaStreamSynchronize(c->stream));
+  for (const Member& m : members(c, db)) {
+    int il, j;
+    if (!m.db->shard.local_item(item_idx, c->num_per, il, j)) continue;   // row lives on another GPU
+    b200pir_ctx* x = m.ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    x->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like write_items
+    B200_CUDA(cudaMemcpyAsync(x->w_wbytes.p, poly, POLY * 8, cudaMemcpyHostToDevice, x->stream));
+    launch_db_upsert(m.db->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(x->w_wbytes.p), x->stream);
+    const ItemWrite item{0, 0, (uint32_t)il, (uint32_t)j};
+    m.db->mark_items(&item, 1, (int)slice, (int)slice + 1, x->stream);
+    // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
+    B200_CUDA(cudaStreamSynchronize(x->stream));
+    B200_CUDA(cudaSetDevice(c->device));
+  }
   API_END
 }
 int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, const uint8_t* data, size_t len) {
   API_BEGIN
   if (!c || (!data && len)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
   if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
   if (len > (size_t)c->slices * c->bytes_per_chunk) throw Error(B200PIR_E_SHAPE, "update longer than instances*n^2*bytes_per_chunk");   // loading.rs:308-310
   if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
-  int il, j;
-  if (!db->shard.local_item(db_idx, c->num_per, il, j)) return 0;         // row lives on another GPU
-  const ItemWrite item{0, (uint32_t)len, (uint32_t)il, (uint32_t)j};
-  write_items(c, db, data, len, &item, 1);
-  db->mark_items(&item, 1, 0, c->slices, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
-  B200_CUDA(cudaGetLastError());
+  for (const Member& m : members(c, db)) {
+    int il, j;
+    if (!m.db->shard.local_item(db_idx, c->num_per, il, j)) continue;     // row lives on another GPU
+    B200_CUDA(cudaSetDevice(m.ctx->device));
+    const ItemWrite item{0, (uint32_t)len, (uint32_t)il, (uint32_t)j};
+    write_items(m.ctx, m.db, data, len, &item, 1);
+    m.db->mark_items(&item, 1, 0, c->slices, m.ctx->stream);
+    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));                          // writers hold the host write lock
+    B200_CUDA(cudaSetDevice(c->device));
+    B200_CUDA(cudaGetLastError());
+  }
   API_END
 }
 
@@ -322,32 +501,43 @@ int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, 
 int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* body, size_t len, uint64_t* largest_update) {
   API_BEGIN
   if (!c || (!body && len)) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   const BodyParse parsed = parse_update_body(body, len, 4 + (size_t)c->slices * c->bytes_per_chunk, (uint64_t)c->dim0 * c->num_per);
   // the reference reaches convert_pt_to_poly, which asserts logp == 8 (loading.rs:291), at the first well-formed entry
   if (c->hp.p != 256 && !parsed.entries.empty()) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
   if (c->bytes_per_chunk > (size_t)POLY && !parsed.entries.empty()) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
   const std::vector<BodyEntry> kept = keep_last_occurrence(parsed.entries);
-  std::vector<ItemWrite> all, group;
+  const std::vector<Member> ms = members(c, db);
+  std::vector<std::vector<ItemWrite>> all(ms.size()), group(ms.size());
   for (size_t k = 0; k < kept.size();) {
     // one staging group: whole entries in body order, their bytes (dropped duplicates in between included) within the budget
     const size_t k0 = k, base = kept[k].data_pos();
-    size_t end = base;
-    group.clear();
-    for (; k < kept.size() && group.size() < b200pir_ctx::kWriteStageItems; k++) {
+    size_t end = base, most = 0;
+    for (auto& g : group) g.clear();
+    for (; k < kept.size() && most < b200pir_ctx::kWriteStageItems; k++) {
       const size_t e = kept[k].data_pos() + kept[k].data_len();
       if (k > k0 && e - base > b200pir_ctx::kWriteStageBytes) break;
       end = e;
-      int il, j;
-      if (!db->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
-      group.push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)il, (uint32_t)j});
+      for (size_t g = 0; g < ms.size(); g++) {
+        int il, j;
+        if (!ms[g].db->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
+        group[g].push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)il, (uint32_t)j});
+        most = std::max(most, group[g].size());
+      }
     }
-    write_items(c, db, body + base, end - base, group.data(), group.size());
-    all.insert(all.end(), group.begin(), group.end());
+    for (size_t g = 0; g < ms.size(); g++) {
+      B200_CUDA(cudaSetDevice(ms[g].ctx->device));
+      write_items(ms[g].ctx, ms[g].db, body + base, end - base, group[g].data(), group[g].size());
+      all[g].insert(all[g].end(), group[g].begin(), group[g].end());
+    }
   }
-  db->mark_items(all.data(), all.size(), 0, c->slices, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));                                // writers hold the host write lock
+  for (size_t g = 0; g < ms.size(); g++) {
+    B200_CUDA(cudaSetDevice(ms[g].ctx->device));
+    ms[g].db->mark_items(all[g].data(), all[g].size(), 0, c->slices, ms[g].ctx->stream);
+    B200_CUDA(cudaStreamSynchronize(ms[g].ctx->stream));                        // writers hold the host write lock
+  }
+  B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
   if (parsed.error) throw Error(parsed.error, parsed.message);
   if (largest_update) *largest_update = parsed.largest_update;
@@ -362,7 +552,7 @@ int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* 
 int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   API_BEGIN
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
   if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "load_item_from_seek is restated for logp == 8 only");
   if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");     // server.rs:292
@@ -373,6 +563,7 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   const size_t item_span = (size_t)c->slices * c->bytes_per_chunk, isz = c->hp.db_item_size;
   const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems,
                                                     b200pir_ctx::kWriteStageBytes / std::max<size_t>(1, std::max(isz, item_span))));
+  const std::vector<Member> ms = members(c, db);
   std::vector<uint8_t> host;
   std::vector<ItemWrite> items;
   for (size_t i0 = 0; i0 < num_items; i0 += group) {
@@ -382,18 +573,25 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
     host.resize(span);
     if (span && (fseeko(file.get(), (off_t)lo, SEEK_SET) || fread(host.data(), 1, span, file.get()) != span))
       throw Error(B200PIR_E_SHAPE, "short read from the database file");
-    items.clear();
-    for (size_t k = 0; k < cnt; k++) {
-      const size_t idx = i0 + k, pos = idx * isz;
-      int il, j;
-      if (!db->shard.local_item(idx, c->num_per, il, j)) continue;           // row lives on another GPU
-      const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0;   // clipped at the end of the file
-      items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)il, (uint32_t)j});
+    for (const Member& m : ms) {                                              // one read, staged to every member
+      items.clear();
+      for (size_t k = 0; k < cnt; k++) {
+        const size_t idx = i0 + k, pos = idx * isz;
+        int il, j;
+        if (!m.db->shard.local_item(idx, c->num_per, il, j)) continue;       // row lives on another GPU
+        const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0; // clipped at the end of the file
+        items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)il, (uint32_t)j});
+      }
+      B200_CUDA(cudaSetDevice(m.ctx->device));
+      write_items(m.ctx, m.db, host.data(), span, items.data(), items.size()); // pageable `host`: staged before the call returns
     }
-    write_items(c, db, host.data(), span, items.data(), items.size());        // pageable `host`: staged before the call returns
   }
-  db->mark_slices(0, c->slices, c->stream);                                   // load_db_from_seek builds a dense database
-  B200_CUDA(cudaStreamSynchronize(c->stream));
+  for (const Member& m : ms) {
+    B200_CUDA(cudaSetDevice(m.ctx->device));
+    m.db->mark_slices(0, c->slices, m.ctx->stream);                           // load_db_from_seek builds a dense database
+    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
+  }
+  B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -401,8 +599,13 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
 int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity) {
   API_BEGIN
   if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  if (items) *items = db->present_count;
-  if (capacity) *capacity = db->capacity();
+  uint64_t n = db->present_count, cap = db->capacity();
+  if (db->sharded()) {
+    n = cap = 0;
+    for (const auto& p : db->parts) { n += p.db->present_count; cap += p.db->capacity(); }
+  }
+  if (items) *items = n;
+  if (capacity) *capacity = cap;
   API_END
 }
 int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes) {
@@ -410,17 +613,24 @@ int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t*
   if (!db) throw Error(B200PIR_E_BADARG, "null db");
   if (format) *format = db->layout.format;
   if (local_rows) *local_rows = (uint64_t)db->rows;
-  if (hbm_bytes) *hbm_bytes = (uint64_t)db->store.n;
+  uint64_t bytes = db->store.n;
+  for (const auto& p : db->parts) bytes += p.db->store.n;
+  if (hbm_bytes) *hbm_bytes = bytes;
   API_END
 }
 int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
   API_BEGIN
   if (!c) throw Error(B200PIR_E_BADARG, "null ctx");
-  Guard gd(c);
+  Guard gd(c, db);
   check_db(c, db);
-  launch_write_synthetic(c->dp, db->layout, db->shard, seed, c->hp.p, c->stream);
-  db->mark_slices(0, c->slices, c->stream);
-  B200_CUDA(cudaStreamSynchronize(c->stream));
+  const std::vector<Member> ms = members(c, db);
+  for (const Member& m : ms) {                                  // distinct devices fill at the same time
+    B200_CUDA(cudaSetDevice(m.ctx->device));
+    launch_write_synthetic(m.ctx->dp, m.db->layout, m.db->shard, seed, c->hp.p, m.ctx->stream);
+    m.db->mark_slices(0, c->slices, m.ctx->stream);
+  }
+  for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
+  B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
   API_END
 }

@@ -7,6 +7,7 @@
 #include <condition_variable>
 #include <cstring>
 #include <deque>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -15,6 +16,7 @@ using namespace b200pir;     // the handle structs below live outside the namesp
 enum Stage { ST_EXPAND = 0, ST_MUL, ST_FROMNTT, ST_FOLD, ST_PACK, ST_ENCODE, ST_QIMG /* query operand re-tiling */, ST_COUNT };
 
 struct b200pir_ctx {
+  uint64_t seq = 0;          // creation order: the order in which a call that spans several contexts takes their locks
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
@@ -193,13 +195,48 @@ struct b200pir_db {
   uint64_t capacity() const { return (uint64_t)ctx->slices * rows * ctx->dim0; }
   void mark_items(const ItemWrite* items, size_t count, int slice_begin, int slice_end, cudaStream_t s);
   void mark_slices(int slice_begin, int slice_end, cudaStream_t s);
+
+  // A database over several contexts (b200pir_db_create_sharded): parts[g] is row shard g on its own context and this handle,
+  // owned by the home context `ctx`, holds no rows itself (empty store, rows = num_per).  A query call expands on the home
+  // context, hands the operand to every part, and finishes on the home context from the survivors the parts gather in
+  // `gathered` (db_api.cu creates the buffers, api.cu's run_shards uses them).
+  struct Part {
+    std::unique_ptr<b200pir_db> db;
+    DevBuf<uint8_t> operand;      // the call's first-dimension operand, on a part whose device is not the home device
+    DevBuf<uint32_t> vfold;       // the call's folding matrices, likewise
+    cudaEvent_t done = nullptr;   // recorded on the part's stream after its survivors are gathered
+  };
+  std::vector<Part> parts;
+  size_t exchange_queries = 0;    // queries the buffers below and the parts' receive buffers hold
+  DevBuf<uint32_t> gathered;      // on the home device: [G][count][slices][4 * 2048] survivors
+  cudaEvent_t expanded = nullptr; // recorded on the calling context's stream once the operands are in place
+  cudaEvent_t finished = nullptr; // recorded after the finish: the next call's calling stream waits on it
+  bool sharded() const { return !parts.empty(); }
+  size_t operand_bytes(size_t queries) const;
+  void ensure_exchange(size_t queries);
+  ~b200pir_db();
 };
 
 namespace b200pir {
 
+// The calling context's lock and, for a sharded database, every part's context lock, taken in creation order so that calls on
+// databases that share contexts, and direct calls on a member context, cannot deadlock; the current device becomes c's.
 struct Guard {
-  std::lock_guard<std::recursive_mutex> lk;
-  explicit Guard(b200pir_ctx* c) : lk(c->mu) { cudaSetDevice(c->device); }
+  std::vector<b200pir_ctx*> held;
+  explicit Guard(b200pir_ctx* c, const b200pir_db* db = nullptr) {
+    held.push_back(c);
+    if (db)
+      for (const auto& p : db->parts) held.push_back(p.db->ctx);
+    std::sort(held.begin(), held.end(), [](const b200pir_ctx* a, const b200pir_ctx* b) { return a->seq < b->seq; });
+    held.erase(std::unique(held.begin(), held.end()), held.end());
+    for (auto* h : held) h->mu.lock();
+    cudaSetDevice(c->device);
+  }
+  ~Guard() {
+    for (auto it = held.rbegin(); it != held.rend(); ++it) (*it)->mu.unlock();
+  }
+  Guard(const Guard&) = delete;
+  Guard& operator=(const Guard&) = delete;
 };
 
 // handles may be used from any context with identical parameters on the same device (one context per host

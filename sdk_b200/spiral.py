@@ -129,23 +129,58 @@ class Database:
         self.shard_index, self.shard_count = shard_index, shard_count
 
     @classmethod
-    def from_words(cls, params, db, fmt=None):
-        """db: the reference's dense layout [instance][trial][z][ii][j] (server.rs:263-266)."""
-        self = cls(params, fmt=fmt)
+    def sharded(cls, contexts, fmt=None):
+        """One database in row shards over several contexts (b200pir_db_create_sharded): shard g holds the rows
+        ii = g (mod G) on contexts[g] (distinct Params with identical parameters; devices may repeat).  The first context is
+        the home: pass it, as this database's `params`, to the query functions.  fmt as for the constructor, resolved once on
+        the home context for every shard."""
+        contexts = list(contexts)
+        if not contexts:
+            raise ValueError("a sharded database needs at least one context")
+        params = contexts[0]
+        self = cls.__new__(cls)
+        self.params = params
+        self._members = contexts          # the member contexts must outlive the handle
+        h = C.c_void_p()
+        arr = (C.c_void_p * len(contexts))(*[p._h for p in contexts])
+        if fmt is not None:
+            params.set_option("db_format", fmt)
+        try:
+            check(LIB.b200pir_db_create_sharded(arr, len(contexts), C.byref(h)))
+        finally:
+            if fmt is not None:
+                params.set_option("db_format", -1)
+        self._h = h
+        self.shard_index, self.shard_count = 0, 1
+        return self
+
+    @classmethod
+    def _create(cls, params, fmt, shard_index=0, shard_count=1, contexts=None):
+        if contexts is None:
+            return cls(params, shard_index=shard_index, shard_count=shard_count, fmt=fmt)
+        if contexts[0] is not params:
+            raise ValueError("contexts[0] must be `params`, the home context")
+        return cls.sharded(contexts, fmt=fmt)
+
+    @classmethod
+    def from_words(cls, params, db, fmt=None, contexts=None):
+        """db: the reference's dense layout [instance][trial][z][ii][j] (server.rs:263-266).  contexts: shard the database
+        over these contexts (Database.sharded; contexts[0] is params)."""
+        self = cls._create(params, fmt, contexts=contexts)
         check(LIB.b200pir_db_upload(params._h, self._h, _ptr(db), db.size))
         return self
 
     @classmethod
-    def from_file(cls, params, path, fmt=None, shard_index=0, shard_count=1):
+    def from_file(cls, params, path, fmt=None, shard_index=0, shard_count=1, contexts=None):
         """load_preprocessed_db_from_file (server.rs:373-386): native-endian u64 stream of the whole database."""
-        self = cls(params, shard_index=shard_index, shard_count=shard_count, fmt=fmt)
+        self = cls._create(params, fmt, shard_index, shard_count, contexts)
         check(LIB.b200pir_db_load_file(params._h, self._h, str(path).encode()))
         return self
 
     @classmethod
-    def from_raw_file(cls, params, path, fmt=None, shard_index=0, shard_count=1):
+    def from_raw_file(cls, params, path, fmt=None, shard_index=0, shard_count=1, contexts=None):
         """load_db_from_seek (server.rs:320-357): raw item bytes, item i at byte i * db_item_size."""
-        self = cls(params, shard_index=shard_index, shard_count=shard_count, fmt=fmt)
+        self = cls._create(params, fmt, shard_index, shard_count, contexts)
         check(LIB.b200pir_db_load_raw_file(params._h, self._h, str(path).encode()))
         return self
 
@@ -196,7 +231,7 @@ class Database:
 
     def save_file(self, path):
         """Write the file from_file (load_preprocessed_db_from_file) reads, atomically (temporary file, fsync, rename).
-        Unsharded databases only."""
+        Whole databases only: unsharded, or sharded over several contexts (not a rank shard)."""
         check(LIB.b200pir_db_save_file(self.params._h, self._h, str(path).encode()))
 
     def fill_synthetic(self, seed):
