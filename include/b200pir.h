@@ -157,6 +157,35 @@ int b200pir_db_download(b200pir_ctx* ctx, b200pir_db* db, uint64_t* words, size_
  * assembled on the host from every shard's export, one staging chunk at a time); a rank shard -> B200PIR_E_UNSUPPORTED; a file that cannot be created
  * or written -> B200PIR_E_BADARG, with the path in b200pir_last_error(). */
 int b200pir_db_save_file(b200pir_ctx* ctx, b200pir_db* db, const char* path);
+/* Bits of the per-item flags of b200pir_db_read_items */
+#define B200PIR_ITEM_PRESENT 1u        /* the item is present (b200pir_db_present_items counts it) */
+#define B200PIR_ITEM_NOT_PLAINTEXT 2u  /* some coefficient of some slice is not the image of a byte (e.g. after upsert_item of an
+                                          arbitrary polynomial); it reads as 0 */
+#define B200PIR_ITEM_PAST_CHUNK 4u     /* some coefficient at index >= bytes_per_chunk is a nonzero byte, which is not returned
+                                          (fill_synthetic fills all 2048) */
+/* The inverse of the raw writers (update_item_raw, update_many_items, load_raw_file): item db_idx[k] read back as bytes, on
+ * the GPU.  Each slice's polynomial is inverse-transformed mod both CRT moduli and every coefficient decoded to the byte x whose
+ * recenter_mod(x, 256, q) it is (convert_pt_to_poly, loading.rs:278-299).  out receives count x instances*n^2*bytes_per_chunk
+ * bytes: chunk c of item k at k*span + c*bytes_per_chunk, which is the zero-padded bucket update_item_raw stores
+ * (loading.rs:327-329).  flags[k] (flags may be NULL) gets the B200PIR_ITEM_* bits; an absent item reads as zero bytes with
+ * flags 0.  count has no limit (the items are decoded in staging groups); on a sharded database each item is read from the
+ * shard that holds it.  Read-only, locking as b200pir_db_download.
+ * Errors, with nothing written: null pointers -> B200PIR_E_BADARG; db_idx >= num_items, or on a rank shard (b200pir_db_create
+ * with shard_count > 1) an item whose row it does not hold -> B200PIR_E_SHAPE; p != 256 -> B200PIR_E_UNSUPPORTED;
+ * bytes_per_chunk > 2048 -> B200PIR_E_SHAPE. */
+int b200pir_db_read_items(b200pir_ctx* ctx, b200pir_db* db, const uint64_t* db_idx, size_t count, uint8_t* out, uint8_t* flags);
+/* Write the raw database file that b200pir_db_load_raw_file and the reference's load_db_from_seek read: num_items x
+ * db_item_size bytes, file byte o being byte o - i*db_item_size of item i = o / db_item_size (read as b200pir_db_read_items
+ * does).  8 times smaller than b200pir_db_save_file's snapshot.  The raw format has no presence map: b200pir_db_load_raw_file
+ * builds a dense database (every item present), so present_items and the tiles the wgmma pass skips differ from the source's,
+ * while every response byte is the same.  Streamed in groups of whole items: the host writes one group while the GPU decodes
+ * the next.  Atomic as b200pir_db_save_file; locking as b200pir_db_download.
+ * Refused with B200PIR_E_UNSUPPORTED, `path` untouched and no temporary file left, when no raw file loads back to this
+ * database: an item flagged NOT_PLAINTEXT or PAST_CHUNK, or, where instances*n^2*bytes_per_chunk > db_item_size, two
+ * consecutive items that disagree on a byte they share in the file (the last item's bytes past the end must be zero);
+ * b200pir_last_error() names the first such item.  A rank shard -> B200PIR_E_UNSUPPORTED; other errors as
+ * b200pir_db_read_items and b200pir_db_save_file. */
+int b200pir_db_save_raw_file(b200pir_ctx* ctx, b200pir_db* db, const char* path);
 /* Synthetic database generated on the GPU: plaintext coefficient = splitmix64(seed, ((slice*items+item)*2048+z)) % p,
  * then recenter_mod / NTT / pack as generate_random_db_and_get_item does (server.rs:223-275). */
 int b200pir_db_fill_synthetic(b200pir_ctx* ctx, b200pir_db* db, uint64_t seed);

@@ -111,6 +111,13 @@ struct Database {
   }
   // the file b200pir_db_load_file reads, written atomically (whole databases: unsharded or over several contexts)
   void save_file(const char* path) const { check(b200pir_db_save_file(params.ctx, h, path)); }
+  // the inverse of the raw writers: items db_idx as bytes, count x instances*n^2*bytes_per_chunk into `out`, and their
+  // B200PIR_ITEM_* flags (b200pir_db_read_items; flags may be null)
+  void read_items(const uint64_t* db_idx, size_t count, uint8_t* out, uint8_t* flags = nullptr) const {
+    check(b200pir_db_read_items(params.ctx, h, db_idx, count, out, flags));
+  }
+  // the raw file b200pir_db_load_raw_file reads, written atomically (refused when no raw file loads back to this database)
+  void save_raw_file(const char* path) const { check(b200pir_db_save_raw_file(params.ctx, h, path)); }
 };
 
 namespace ntt {

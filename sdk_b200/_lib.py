@@ -56,6 +56,8 @@ def _load():
         "b200pir_db_download_slice": (C.c_int, [vp, vp, C.c_uint64, u64p, C.c_size_t]),
         "b200pir_db_download": (C.c_int, [vp, vp, u64p, C.c_size_t]),
         "b200pir_db_save_file": (C.c_int, [vp, vp, C.c_char_p]),
+        "b200pir_db_read_items": (C.c_int, [vp, vp, u64p, C.c_size_t, u8p, u8p]),
+        "b200pir_db_save_raw_file": (C.c_int, [vp, vp, C.c_char_p]),
         "b200pir_db_fill_synthetic": (C.c_int, [vp, vp, C.c_uint64]),
         "b200pir_db_info": (C.c_int, [vp, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
         "b200pir_db_present_items": (C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),

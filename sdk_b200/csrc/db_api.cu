@@ -1,6 +1,7 @@
 // C-ABI implementation of the HBM-resident database handle (include/b200pir.h): creation, bulk uploads and file loads,
-// exports, the item writers and the presence map.  Every writer places items through the same three decisions: which GPU owns
-// an item (Shard::local_item), the context's write staging (w_wbytes) and the presence update (mark_items / mark_slices).
+// exports, the plaintext read-back (read_items, save_raw_file), the item writers and the presence map.  Every writer places
+// items through the same three decisions: which GPU owns an item (Shard::local_item), the context's write staging (w_wbytes)
+// and the presence update (mark_items / mark_slices).
 // A sharded handle (b200pir_db_create_sharded) runs each of them once per part, on the part's context, from inputs read once.
 #include "spiral_api.hpp"
 #include "update_body.hpp"
@@ -10,6 +11,9 @@
 #include <unistd.h>
 #include <memory>
 #include <utility>
+
+static_assert(B200PIR_ITEM_NOT_PLAINTEXT == kReadNotPlaintext && B200PIR_ITEM_PAST_CHUNK == kReadPastChunk &&
+              (B200PIR_ITEM_PRESENT & (kReadNotPlaintext | kReadPastChunk)) == 0, "k_read_items' flag bits are the ABI's");
 
 // ---------------------------------------------------------------- presence
 // every item of `items` written in slices [slice_begin, slice_end): one upload of the whole mask when any word changed
@@ -141,52 +145,46 @@ void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t spa
   launch_write_items(c->dp, db->layout, c->w_wbytes.p, c->w_witems.p, (int)count, c->slices, (int)c->bytes_per_chunk, c->hp.p, c->stream);
 }
 
-// Database export, shared by b200pir_db_download(_slice) and b200pir_db_save_file.  A chunk is one slice and a range of z of
-// the local rows, at most the writers' 64 MiB device staging (w_wbytes).  Under the context lock one launch un-tiles it into
-// [zc][rows][dim0] u64 there and the chunk is queued for a copy to one of the two pinned buffers; the lock is then released and
-// `sink(slice, z0, zc, words)` consumes the previous chunk once its copy has landed, while the GPU un-tiles and copies this
-// one.  Everything is ordered on the context's stream, so a chunk's un-tiling never overwrites staging its copy still reads.
-// A sharded database exports each chunk from every part, on the part's context, and `words[g]` is part g's.
-template <typename Sink>
-void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
+// Device-to-host streaming, shared by the exports (b200pir_db_download(_slice), b200pir_db_save_file) and the item readers
+// (b200pir_db_read_items, b200pir_db_save_raw_file).  Under each member's context lock, fill(k, g, stage) queues the device
+// work that leaves chunk k of member g in its writers' staging (w_wbytes, at least `stage_bytes`, the 64 MiB minimum) and
+// returns its size; the chunk is queued for a copy to one of the two pinned buffers, the locks are released, and
+// sink(k - 1, src) consumes the previous chunk once its copies have landed (src[g] = member g's bytes) while the GPU produces
+// and copies this one.  Everything is ordered on each context's stream, so a chunk never overwrites staging that the previous
+// chunk's copy still reads.  A sharded database produces each chunk on every part, on the part's context.
+template <typename Fill, typename Sink>
+void stream_out(b200pir_ctx* c, b200pir_db* db, size_t chunks, size_t stage_bytes, Fill fill, Sink sink) {
   const std::vector<Member> ms = members(c, db);
   std::vector<b200pir_ctx*> order;
   for (const Member& m : ms) order.push_back(m.ctx);
   std::sort(order.begin(), order.end(), [](const b200pir_ctx* a, const b200pir_ctx* b) { return a->seq < b->seq; });
   std::vector<std::unique_lock<std::mutex>> ex;
   for (b200pir_ctx* x : order) ex.emplace_back(x->export_mu);
-  const size_t per_z = (size_t)ms[0].db->rows * c->dim0;
-  const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
-  struct Chunk { int slice, z0, zc; };
-  std::vector<Chunk> chunks;
-  for (int s = slice_begin; s < slice_end; s++)
-    for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
   for (const Member& m : ms) {
     Guard gd(m.ctx);
-    m.ctx->ensure_export_staging(per_z * zc * 8);
+    m.ctx->ensure_export_staging(stage_bytes);
   }
-  std::vector<const uint64_t*> src(ms.size());
+  std::vector<const uint8_t*> src(ms.size());
   auto consume = [&](size_t k) {
     const int b = (int)(k & 1);
     for (size_t g = 0; g < ms.size(); g++) {
       B200_CUDA(cudaEventSynchronize(ms[g].ctx->export_done[b]));
-      src[g] = reinterpret_cast<const uint64_t*>(ms[g].ctx->h_export[b]);
+      src[g] = ms[g].ctx->h_export[b];
     }
-    sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, src);
+    sink(k, src);
   };
   try {
-    for (size_t k = 0; k < chunks.size(); k++) {
-      for (const Member& m : ms) {
-        Guard gd(m.ctx);
-        b200pir_ctx* x = m.ctx;
-        uint64_t* stage = reinterpret_cast<uint64_t*>(x->w_wbytes.p);
-        launch_db_export(m.db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, stage, x->stream);
-        B200_CUDA(cudaMemcpyAsync(x->h_export[k & 1], stage, per_z * chunks[k].zc * 8, cudaMemcpyDeviceToHost, x->stream));
+    for (size_t k = 0; k < chunks; k++) {
+      for (size_t g = 0; g < ms.size(); g++) {
+        Guard gd(ms[g].ctx);
+        b200pir_ctx* x = ms[g].ctx;
+        const size_t bytes = fill(k, g, x->w_wbytes.p);
+        if (bytes) B200_CUDA(cudaMemcpyAsync(x->h_export[k & 1], x->w_wbytes.p, bytes, cudaMemcpyDeviceToHost, x->stream));
         B200_CUDA(cudaEventRecord(x->export_done[k & 1], x->stream));
       }
       if (k > 0) consume(k - 1);
     }
-    if (!chunks.empty()) consume(chunks.size() - 1);
+    if (chunks) consume(chunks - 1);
   } catch (...) {
     for (const Member& m : ms)
       for (auto e : m.ctx->export_done) cudaEventSynchronize(e);     // no copy may still land in the pinned buffers
@@ -195,6 +193,134 @@ void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end,
   }
   B200_CUDA(cudaSetDevice(c->device));
   B200_CUDA(cudaGetLastError());
+}
+
+// Database export.  A chunk is one slice and a range of z of the local rows, at most the writers' 64 MiB staging: one launch
+// un-tiles it into [zc][rows][dim0] u64 there, and `sink(slice, z0, zc, words)` consumes it, `words[g]` being member g's.
+template <typename Sink>
+void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
+  const std::vector<Member> ms = members(c, db);
+  const size_t per_z = (size_t)ms[0].db->rows * c->dim0;
+  const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
+  struct Chunk { int slice, z0, zc; };
+  std::vector<Chunk> chunks;
+  for (int s = slice_begin; s < slice_end; s++)
+    for (int z0 = 0; z0 < POLY; z0 += zc) chunks.push_back(Chunk{s, z0, std::min(zc, POLY - z0)});
+  std::vector<const uint64_t*> words(ms.size());
+  stream_out(c, db, chunks.size(), per_z * zc * 8,
+             [&](size_t k, size_t g, uint8_t* stage) {
+               launch_db_export(ms[g].db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<uint64_t*>(stage),
+                                ms[g].ctx->stream);
+               return per_z * chunks[k].zc * 8;
+             },
+             [&](size_t k, const std::vector<const uint8_t*>& src) {
+               for (size_t g = 0; g < ms.size(); g++) words[g] = reinterpret_cast<const uint64_t*>(src[g]);
+               sink(chunks[k].slice, chunks[k].z0, chunks[k].zc, words);
+             });
+}
+
+// Items read back as the bytes the raw writers take (b200pir_db_read_items, b200pir_db_save_raw_file): the `count` global
+// indices idx(0 .. count-1), which the caller has checked, in groups of whole items that fit the staging.  For each group every
+// member decodes the items it holds with one k_read_items launch: its m-th item of the group goes to slot m of its staging
+// (span = slices * bytes_per_chunk bytes), followed by one flag byte per (slot, slice).  Then sink(k0, n, bytes, flags)
+// consumes items k0 .. k0+n-1: bytes(k) points at item k's span, flags(k) is its B200PIR_ITEM_* bits.
+template <typename Index, typename Sink>
+void read_items_impl(b200pir_ctx* c, b200pir_db* db, size_t count, Index idx, Sink sink) {
+  const std::vector<Member> ms = members(c, db);
+  const size_t slices = (size_t)c->slices, span = slices * c->bytes_per_chunk;
+  const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems, b200pir_ctx::kWriteStageBytes / (span + slices)));
+  // where each item of the groups in flight (two: one being filled, one being consumed) lives
+  struct Where { uint32_t g, slot; uint8_t present; };
+  std::vector<Where> where[2];
+  std::vector<size_t> held[2];                     // items of the group per member
+  std::vector<ItemWrite> items;
+  for (auto& h : held) h.assign(ms.size(), 0);
+  stream_out(c, db, (count + group - 1) / group, group * (span + slices),
+             [&](size_t k, size_t g, uint8_t* stage) -> size_t {
+               const size_t k0 = k * group, n = std::min(group, count - k0);
+               std::vector<Where>& w = where[k & 1];
+               w.resize(n);
+               const b200pir_db* m = ms[g].db;
+               items.clear();
+               for (size_t i = 0; i < n; i++) {
+                 int il, j;
+                 if (!m->shard.local_item(idx(k0 + i), c->num_per, il, j)) continue;   // row lives on another GPU
+                 uint8_t present = 0;
+                 for (size_t sl = 0; sl < slices; sl++) {
+                   const uint64_t bit = ((uint64_t)sl * m->rows + il) * c->dim0 + j;
+                   present |= (m->present[bit >> 6] >> (bit & 63)) & 1;
+                 }
+                 w[i] = Where{(uint32_t)g, (uint32_t)items.size(), present ? (uint8_t)B200PIR_ITEM_PRESENT : (uint8_t)0};
+                 items.push_back(ItemWrite{(uint32_t)items.size(), 0, (uint32_t)il, (uint32_t)j});
+               }
+               held[k & 1][g] = items.size();
+               if (items.empty()) return 0;
+               b200pir_ctx* x = ms[g].ctx;
+               x->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, items.size()));
+               // pageable: staged before the call returns, so `items` may be refilled for the next member
+               B200_CUDA(cudaMemcpyAsync(x->w_witems.p, items.data(), items.size() * sizeof(ItemWrite), cudaMemcpyHostToDevice, x->stream));
+               launch_read_items(x->dp, m->layout, x->w_witems.p, (int)items.size(), (int)slices, (int)c->bytes_per_chunk, stage,
+                                 stage + items.size() * span, x->stream);
+               return items.size() * (span + slices);
+             },
+             [&](size_t k, const std::vector<const uint8_t*>& src) {
+               const std::vector<Where>& w = where[k & 1];
+               const std::vector<size_t>& h = held[k & 1];
+               sink(k * group, w.size(),
+                    [&](size_t i) { return src[w[i - k * group].g] + (size_t)w[i - k * group].slot * span; },
+                    [&](size_t i) {
+                      const Where& e = w[i - k * group];
+                      const uint8_t* f = src[e.g] + h[e.g] * span + (size_t)e.slot * slices;
+                      uint8_t bits = e.present;
+                      for (size_t sl = 0; sl < slices; sl++) bits |= f[sl];
+                      return bits;
+                    });
+             });
+}
+
+// Write `path` atomically: write(f) fills a temporary file in the same directory (mode 0600), which is flushed, fsync'ed and
+// renamed over `path`, and the directory is fsync'ed.  On any failure the temporary file is removed and `path` keeps its
+// earlier content; an Error from write(f) keeps its code, a failed file operation is B200PIR_E_BADARG naming the path.
+template <typename Write>
+void write_atomically(const char* path, Write write) {
+  const std::string target(path);
+  std::string tmp = target + ".tmp.XXXXXX";
+  const int fd = mkstemp(&tmp[0]);
+  if (fd < 0) throw Error(B200PIR_E_BADARG, "cannot create a temporary file next to " + target + ": " + std::strerror(errno));
+  FILE* f = fdopen(fd, "wb");
+  if (!f) close(fd);
+  // drop the temporary file and report `why`: `path` is left as it was
+  auto discard = [&](const std::string& why, int code) {
+    if (f) fclose(f);
+    f = nullptr;
+    unlink(tmp.c_str());
+    throw Error(code, code == B200PIR_E_BADARG ? "cannot write " + target + ": " + why : why);
+  };
+  if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
+  try {
+    write(f);
+  } catch (const Error& e) {
+    discard(e.what(), e.code);
+  } catch (const std::exception& e) {
+    discard(e.what(), B200PIR_E_CUDA);
+  }
+  if (fflush(f) != 0 || fsync(fileno(f)) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  const int closed = fclose(f);
+  f = nullptr;
+  if (closed != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  if (rename(tmp.c_str(), target.c_str()) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
+  // make the rename itself durable
+  const size_t slash = target.find_last_of('/');
+  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : target.substr(0, slash));
+  const int dfd = open(dir.c_str(), O_RDONLY);
+  if (dfd >= 0) { fsync(dfd); close(dfd); }
+}
+
+// the checks the raw writers make (update_item_raw, load_raw_file): bytes <-> coefficients is defined for p = 256 and chunks of
+// at most poly_len bytes
+void check_raw_params(const b200pir_ctx* c) {
+  if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
+  if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
 }
 
 // Chunk (zc values of z) of every member, `src[g]` being member g's [zc][rows][dim0], scattered into `dst`, the same range of z
@@ -405,21 +531,7 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   check_db(c, db);
   if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
   const std::vector<Member> ms = members(c, db);
-  const std::string target(path);
-  std::string tmp = target + ".tmp.XXXXXX";
-  const int fd = mkstemp(&tmp[0]);
-  if (fd < 0) throw Error(B200PIR_E_BADARG, "cannot create a temporary file next to " + target + ": " + std::strerror(errno));
-  FILE* f = fdopen(fd, "wb");
-  if (!f) close(fd);
-  // drop the temporary file and report `why`: `path` is left as it was
-  auto discard = [&](const std::string& why, int code) {
-    if (f) fclose(f);
-    f = nullptr;
-    unlink(tmp.c_str());
-    throw Error(code, code == B200PIR_E_BADARG ? "cannot write " + target + ": " + why : why);
-  };
-  if (!f) discard(std::strerror(errno), B200PIR_E_BADARG);
-  try {
+  write_atomically(path, [&](FILE* f) {
     // a sharded database's chunk is assembled from its parts' exports first: host memory stays bounded by the staging
     std::vector<uint64_t> whole;
     export_impl(c, db, 0, c->slices, [&](int, int, int zc, const std::vector<const uint64_t*>& src) {
@@ -432,21 +544,66 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
       }
       if (fwrite(words, 8, n, f) != n) throw Error(B200PIR_E_BADARG, std::strerror(errno));
     });
-  } catch (const Error& e) {
-    discard(e.what(), e.code);
-  } catch (const std::exception& e) {
-    discard(e.what(), B200PIR_E_CUDA);
+  });
+  API_END
+}
+int b200pir_db_read_items(b200pir_ctx* c, b200pir_db* db, const uint64_t* db_idx, size_t count, uint8_t* out, uint8_t* flags) {
+  API_BEGIN
+  if (!c || (count && (!db_idx || !out))) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  check_raw_params(c);
+  const uint64_t num_items = (uint64_t)c->dim0 * c->num_per;
+  for (size_t k = 0; k < count; k++) {
+    int il, j;
+    if (db_idx[k] >= num_items) throw Error(B200PIR_E_SHAPE, "bad db idx " + std::to_string(db_idx[k]));
+    if (!db->shard.local_item(db_idx[k], c->num_per, il, j))
+      throw Error(B200PIR_E_SHAPE, "db idx " + std::to_string(db_idx[k]) + " lies in a row this shard does not hold");
   }
-  if (fflush(f) != 0 || fsync(fileno(f)) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  const int closed = fclose(f);
-  f = nullptr;
-  if (closed != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  if (rename(tmp.c_str(), target.c_str()) != 0) discard(std::strerror(errno), B200PIR_E_BADARG);
-  // make the rename itself durable
-  const size_t slash = target.find_last_of('/');
-  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : target.substr(0, slash));
-  const int dfd = open(dir.c_str(), O_RDONLY);
-  if (dfd >= 0) { fsync(dfd); close(dfd); }
+  const size_t span = (size_t)c->slices * c->bytes_per_chunk;
+  read_items_impl(c, db, count, [&](size_t k) { return db_idx[k]; },
+                  [&](size_t k0, size_t n, auto bytes, auto bits) {
+                    for (size_t k = k0; k < k0 + n; k++) {
+                      std::memcpy(out + k * span, bytes(k), span);
+                      if (flags) flags[k] = bits(k);
+                    }
+                  });
+  API_END
+}
+// The raw file b200pir_db_load_raw_file reads: item i's first db_item_size bytes at i * db_item_size.  When an item's span
+// (slices * bytes_per_chunk) is longer than db_item_size, its last bytes are the next item's first ones in the file, so they
+// must agree, and the last item's must be zero (load_raw_file reads zeros past the end of the file).
+int b200pir_db_save_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
+  API_BEGIN
+  if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
+  check_db(c, db);
+  check_raw_params(c);
+  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: a shard holds only part of the database");
+  const size_t num_items = (size_t)c->dim0 * c->num_per, isz = c->hp.db_item_size;
+  const size_t span = (size_t)c->slices * c->bytes_per_chunk, tail = span - isz;   // span >= isz: bytes_per_chunk rounds up
+  write_atomically(path, [&](FILE* f) {
+    std::vector<uint8_t> carry(tail, 0), file;                // carry: the last `tail` bytes of the previous item
+    read_items_impl(c, db, num_items, [](size_t k) { return (uint64_t)k; },
+                    [&](size_t k0, size_t n, auto bytes, auto bits) {
+                      file.resize(n * isz);
+                      for (size_t i = k0; i < k0 + n; i++) {
+                        const uint8_t fl = bits(i);
+                        if (fl & B200PIR_ITEM_NOT_PLAINTEXT)
+                          throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: item " + std::to_string(i) + " holds a coefficient that is not a byte");
+                        if (fl & B200PIR_ITEM_PAST_CHUNK)
+                          throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: item " + std::to_string(i) + " has bytes past bytes_per_chunk");
+                        const uint8_t* b = bytes(i);
+                        if (tail && i > 0 && std::memcmp(carry.data(), b, tail) != 0)
+                          throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: the last bytes of item " + std::to_string(i - 1) +
+                                                                 " differ from the first bytes of item " + std::to_string(i) + ", which the raw file shares");
+                        std::memcpy(carry.data(), b + isz, tail);
+                        std::memcpy(file.data() + (i - k0) * isz, b, isz);
+                      }
+                      if (k0 + n == num_items && std::any_of(carry.begin(), carry.end(), [](uint8_t v) { return v != 0; }))
+                        throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: the last bytes of item " + std::to_string(num_items - 1) +
+                                                               " lie past the end of the raw file and are not zero");
+                      if (fwrite(file.data(), 1, file.size(), f) != file.size()) throw Error(B200PIR_E_BADARG, std::strerror(errno));
+                    });
+  });
   API_END
 }
 int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint64_t item_idx, const uint64_t* poly) {
@@ -476,8 +633,7 @@ int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, 
   if (!c || (!data && len)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c, db);
   check_db(c, db);
-  if (c->hp.p != 256) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
-  if (c->bytes_per_chunk > (size_t)POLY) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
+  check_raw_params(c);
   if (len > (size_t)c->slices * c->bytes_per_chunk) throw Error(B200PIR_E_SHAPE, "update longer than instances*n^2*bytes_per_chunk");   // loading.rs:308-310
   if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
   for (const Member& m : members(c, db)) {

@@ -1,7 +1,8 @@
 // Where one NTT coordinate z of one database item lives in each device layout, and how it is read back.  Item (slice, local
 // row il, column j) holds, at every z, the residue mod q0 (`lo`) and mod q1 (`hi`) of the packed word lo | hi << 32
 // (loading.rs:34-41 pack_ntt_poly).  The single-item upsert (mul_kernels.cu), the batched item writer (k_write_items in
-// poly_kernels.cu: raw bytes or the synthetic database) and the import and export kernels (export_kernels.cu) all address the database through these maps, so
+// poly_kernels.cu: raw bytes or the synthetic database), its inverse (k_read_items) and the import and export kernels
+// (export_kernels.cu) all address the database through these maps, so
 // every writer and reader agrees on the layouts; the host sizes the store with db_bytes.  The maps are __host__ __device__
 // and use no CUDA types: tests/cpp/db_layout_inverse.cpp checks on the CPU that place and fetch are mutually inverse, that no
 // two items share a byte and that every byte a writer touches lies inside db_bytes.
@@ -146,6 +147,22 @@ TC5_HD uint64_t fetch_item(const DbLayout& L, int slice, int il, int j, int z) {
   if (L.format == 0) return fetch_imad(L.G, reinterpret_cast<const uint32_t*>(L.base), slice, il, j, z);
   if (L.format == 2) return fetch_tc5(L.T, L.base, slice, il, j, z);
   return fetch_frag(L.F, L.base, slice, il, j, z);
+}
+
+// ---- plaintext bytes of an item (p = 256).  convert_pt_to_poly (loading.rs:278-299) stores coefficient byte x as
+// recenter_mod(x, 256, q) (arith.rs:415) mod both q_n: x for x <= 128, q - (256 - x) above.  The item reader (k_read_items)
+// inverts it coefficient by coefficient; tests/cpp/pt_byte_decode.cpp checks the rule on the CPU.
+TC5_HD uint32_t pt_byte_residue(uint32_t x, uint32_t q) { return x <= 128 ? x : q - (256 - x); }
+// The byte x whose residues mod q0 and q1 are r0 and r1, or -1 when the pair is not the image of one byte ("not plaintext").
+// Any 32-bit words are accepted: each is reduced mod its modulus first (format 0 keeps uploaded halves verbatim).
+TC5_HD int pt_byte_decode(uint32_t r0, uint32_t r1, uint32_t q0, uint32_t q1) {
+  r0 %= q0;
+  r1 %= q1;
+  uint32_t x;
+  if (r0 <= 128) x = r0;
+  else if (r0 >= q0 - 127) x = r0 - (q0 - 256);
+  else return -1;
+  return r1 == pt_byte_residue(x, q1) ? (int)x : -1;
 }
 
 }  // namespace b200pir

@@ -113,6 +113,16 @@ struct ItemWrite { uint32_t off, len, il, j; };
 // (recenter_mod, NTT, pack: loading.rs:278-299, 34-41) and placed at the item's cell of slice c.  One launch.
 void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* bytes, const ItemWrite* items, int count, int chunks,
                         int bpc, uint64_t pt_modulus, cudaStream_t s);
+// the inverse on raw bytes: every (item, chunk c < chunks) pair of `items` (local row il, column j; off = the item's output
+// slot) fetched from slice c, inverse-transformed mod both q_n and decoded coefficient by coefficient (pt_byte_decode,
+// item_place.cuh).  Coefficient i < bpc becomes byte (off * chunks + c) * bpc + i of `out`, 0 where it does not decode; flag
+// byte off * chunks + c of `flags` is written with the bits below.  One launch; p = 256 only.
+enum : uint8_t {
+  kReadNotPlaintext = 2,   // some coefficient of the chunk is not the image of a byte
+  kReadPastChunk = 4,      // some coefficient at index >= bpc decodes to a nonzero byte (not returned)
+};
+void launch_read_items(const DevParams& P, const DbLayout& L, const ItemWrite* items, int count, int chunks, int bpc, uint8_t* out,
+                       uint8_t* flags, cudaStream_t s);
 // the synthetic database: plaintext coefficient i of slice c of item = j * num_per_global + ii is
 // splitmix64(seed, ((c * items + item) * 2048 + i)) % p, converted and placed like raw bytes (server.rs:223-275 with a counter
 // PRNG).  Every local item of every slice, one launch.

@@ -387,6 +387,45 @@ k_write_items(DevParams P, DbLayout L, Src src, uint64_t pt) {
   __syncthreads();
   for (int z = threadIdx.x; z < POLY; z += 512) place_item(L, slice, it.il, it.j, z, halves[0][z], halves[1][z]);
 }
+// The inverse of k_write_items on raw bytes.  CTA = (item, slice c): the item's two residues at every z from its place in the
+// database (fetch_item), reduced mod q_n (format 0 keeps uploaded halves verbatim), inverse NTT mod both q_n, and each
+// coefficient decoded back to the byte convert_pt_to_poly took it from (pt_byte_decode; 0 where it does not decode).
+// Coefficient i < bpc is byte c * bpc + i of the item's slot items[b].off in `out` (span = slices * bpc bytes per slot);
+// flag byte off * slices + c gets kReadNotPlaintext / kReadPastChunk.  Launch shape and budget as k_write_items.
+__global__ void __launch_bounds__(512, 2)
+k_read_items(DevParams P, DbLayout L, const ItemWrite* __restrict__ items, int bpc, uint8_t* out, uint8_t* flags) {
+  __shared__ __align__(16) uint32_t ntt_smem[2 * NTT_SMEM_WORDS];
+  __shared__ __align__(16) uint32_t halves[2][POLY];
+  const int n = threadIdx.x >> 8, tid = threadIdx.x & 255;
+  const int slice = blockIdx.y;
+  const uint32_t q = n ? P.q[1] : P.q[0];
+  const ItemWrite it = items[blockIdx.x];
+  for (int z = threadIdx.x; z < POLY; z += 512) {
+    const uint64_t w = fetch_item(L, slice, (int)it.il, (int)it.j, z);
+    halves[0][z] = (uint32_t)w % P.q[0];
+    halves[1][z] = (uint32_t)(w >> 32) % P.q[1];
+  }
+  __syncthreads();
+  uint32_t x[8];
+  ld8(x, halves[n] + tid * 8);
+  ntt_inverse_group_nh(tid, x, ntt_smem + n * NTT_SMEM_WORDS, TwConst{n, 2}, TwGlobal{n ? P.inv_lz[1] : P.inv_lz[0]}, q, CtaSync());
+#pragma unroll
+  for (int a = 0; a < 8; a++) halves[n][a * 256 + tid] = x[a];      // every read of halves was before the transform's barriers
+  __syncthreads();
+  uint8_t* dst = out + ((size_t)it.off * gridDim.y + slice) * bpc;
+  bool bad = false, past = false;
+#pragma unroll
+  for (int m = 0; m < POLY / 512; m++) {
+    const int i = m * 512 + threadIdx.x;
+    const int b = pt_byte_decode(halves[0][i], halves[1][i], P.q[0], P.q[1]);
+    bad |= b < 0;
+    past |= i >= bpc && b > 0;
+    if (i < bpc) dst[i] = b < 0 ? 0 : (uint8_t)b;
+  }
+  bad = __syncthreads_or(bad);
+  past = __syncthreads_or(past);
+  if (threadIdx.x == 0) flags[(size_t)it.off * gridDim.y + slice] = (bad ? kReadNotPlaintext : 0) | (past ? kReadPastChunk : 0);
+}
 // raw u64 coefficients -> residue form u32 [poly][n][z] (coefficient domain), and back (CRT lift)
 __global__ void k_raw_to_res(DevParams P, uint32_t* out, const uint64_t* raw, size_t polys) {
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;     // over polys * 2048
@@ -1157,6 +1196,13 @@ void launch_write_items(const DevParams& P, const DbLayout& L, const uint8_t* by
   if (chunks > 65535) throw Error(-2, "write_items: more than 65535 slices");
   ++g_kernel_launches;
   k_write_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, ItemBytes{bytes, items, bpc}, pt_modulus);
+}
+void launch_read_items(const DevParams& P, const DbLayout& L, const ItemWrite* items, int count, int chunks, int bpc, uint8_t* out,
+                       uint8_t* flags, cudaStream_t s) {
+  if (count == 0) return;
+  if (chunks > 65535) throw Error(-2, "read_items: more than 65535 slices");
+  ++g_kernel_launches;
+  k_read_items<<<dim3((unsigned)count, (unsigned)chunks), 512, 0, s>>>(P, L, items, bpc, out, flags);
 }
 void launch_write_synthetic(const DevParams& P, const DbLayout& L, Shard sh, uint64_t seed, uint64_t pt_modulus, cudaStream_t s) {
   const size_t count = (size_t)L.G.num_per * L.G.dim0;

@@ -14,6 +14,8 @@ from ._lib import LIB, CParams, check, B200PirError  # noqa: F401
 POLY_LEN = 2048          # lib/spiral-rs/src/util.rs:246
 CRT_COUNT = 2
 MODULI = (268369921, 249561089)   # util.rs:247
+# flags of Database.read_items (B200PIR_ITEM_* in include/b200pir.h)
+ITEM_PRESENT, ITEM_NOT_PLAINTEXT, ITEM_PAST_CHUNK = 1, 2, 4
 
 
 def _ptr(a, dtype=np.uint64):
@@ -233,6 +235,24 @@ class Database:
         """Write the file from_file (load_preprocessed_db_from_file) reads, atomically (temporary file, fsync, rename).
         Whole databases only: unsharded, or sharded over several contexts (not a rank shard)."""
         check(LIB.b200pir_db_save_file(self.params._h, self._h, str(path).encode()))
+
+    def read_items(self, indices):
+        """The inverse of update_item_raw / load_raw_file: items `indices` read back as bytes -> (uint8 [count][span], uint8
+        flags [count]), span = instances * n^2 * bytes_per_chunk (the zero-padded bucket update_item_raw stores).  Flags are
+        bits of ITEM_PRESENT, ITEM_NOT_PLAINTEXT and ITEM_PAST_CHUNK; an absent item is zero bytes with flags 0."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint64).reshape(-1)
+        P = self.params
+        span = P.slices * ((P.db_item_size + P.slices - 1) // P.slices)
+        out = np.zeros((idx.size, span), dtype=np.uint8)
+        flags = np.zeros(idx.size, dtype=np.uint8)
+        check(LIB.b200pir_db_read_items(P._h, self._h, _ptr(idx), idx.size, out.ctypes.data, flags.ctypes.data))
+        return out, flags
+
+    def save_raw_file(self, path):
+        """Write the raw file from_raw_file (load_db_from_seek) reads, atomically: num_items x db_item_size bytes.  Refused
+        (B200PirError, E_UNSUPPORTED) when no raw file loads back to this database.  A database loaded back from it is dense:
+        every item is present."""
+        check(LIB.b200pir_db_save_raw_file(self.params._h, self._h, str(path).encode()))
 
     def fill_synthetic(self, seed):
         check(LIB.b200pir_db_fill_synthetic(self.params._h, self._h, seed))
