@@ -224,12 +224,12 @@ void run_prepare(b200pir_ctx* c, Keys keys, size_t count, bool images) {
 }
 
 // The first-dimension product of `count` queries (operands qdev + qi * dim0 * POLY, or `images`) over slices [slice_begin,
-// slice_begin + slice_count), into `out` (queries slices * rows * 4 * POLY words apart) in the form db->zmajor_product() names.
-void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, Images images, uint32_t* out,
+// slice_begin + slice_count), into `out` (queries slices * rows * 4 * POLY words apart) in the form db.zmajor_product() names.
+void run_first_dim(b200pir_ctx* c, const DbStore& db, size_t count, const uint4* qdev, Images images, uint32_t* out,
                    int slice_begin, int slice_count) {
-  const DbLayout& L = db->layout;
+  const DbLayout& L = db.layout;
   const size_t q_stride = (size_t)c->dim0 * POLY;
-  const size_t out_stride = (size_t)c->slices * db->rows * 4 * POLY;
+  const size_t out_stride = (size_t)c->slices * db.rows * 4 * POLY;
   if (L.format == 0) {
     // IMAD path: 4, 2 or 1 queries per database pass
     b200pir_ctx::Scope sc(c, ST_MUL);
@@ -255,7 +255,7 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
         launch_query_to_tc5(L.T, qdev + qi * q_stride, q_stride, nq, c->w_qt.p, c->stream);
       }
       b200pir_ctx::Scope sc(c, ST_MUL);
-      launch_multiply_tc5(c->dp, L.T, L.base, db->tile_mask.p, qt, out + qi * out_stride, out_stride, nq, slice_begin,
+      launch_multiply_tc5(c->dp, L.T, L.base, db.tile_mask.p, qt, out + qi * out_stride, out_stride, nq, slice_begin,
                           slice_count, c->sm_count, c->stream);
       c->mul_launches++;
     }
@@ -281,17 +281,17 @@ void run_first_dim(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qd
 
 // first dimension (operand qdev or `images`) + from_ntt + local fold with the folding matrices vfold (fold shortcut when
 // `sparse`); returns the survivors (in w_mult or w_cts), one per (query, slice)
-Survivors run_first_dim_and_fold(b200pir_ctx* c, b200pir_db* db, size_t count, const uint4* qdev, Images images,
+Survivors run_first_dim_and_fold(b200pir_ctx* c, const DbStore& db, size_t count, const uint4* qdev, Images images,
                                  const uint32_t* vfold, bool sparse) {
-  const int rows = db->rows;
+  const int rows = db.rows;
   const size_t out_stride = (size_t)c->slices * rows * 4 * POLY;
   // server.rs:707-709 from_ntt, minus the CRT lift, into w_mult in residue form: a z-major product goes to w_cts (free until
   // the fold starts) and is inverse-transformed from there; an ntt32 product is inverse-transformed in place
-  const bool zmajor = db->zmajor_product();
+  const bool zmajor = db.zmajor_product();
   run_first_dim(c, db, count, qdev, images, zmajor ? c->w_cts.p : c->w_mult.p, 0, c->slices);
   {
     b200pir_ctx::Scope sc(c, ST_FROMNTT);
-    if (zmajor) launch_intt_from_zmajor(c->dp, db->layout.F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
+    if (zmajor) launch_intt_from_zmajor(c->dp, db.layout.F, c->w_cts.p, out_stride, c->w_mult.p, (int)count, c->slices, c->stream);
     else launch_ntt32(c->dp, c->w_mult.p, count * c->slices * rows * 2, true, c->stream);
   }
   b200pir_ctx::Scope sc(c, ST_FOLD);
@@ -732,18 +732,18 @@ int b200pir_multiply_reg_by_database(b200pir_ctx* c, b200pir_db* db, uint64_t sl
   if (!c || !v_firstdim || !out) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
-  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "multiply_reg_by_database: not on a sharded database");
+  const DbStore& s = db->single("multiply_reg_by_database: not on a sharded database");
   if (slice >= (uint64_t)c->slices) throw Error(B200PIR_E_SHAPE, "slice out of range");
-  const int rows = db->rows;
-  const bool zmajor = db->zmajor_product();
+  const int rows = s.rows;
+  const bool zmajor = s.zmajor_product();
   DevBuf<uint64_t> vq((size_t)c->dim0 * 2 * POLY);
   DevBuf<uint4> qd((size_t)c->dim0 * POLY);
   DevBuf<uint32_t> o((size_t)c->slices * rows * 4 * POLY), zm(zmajor ? o.n : 0);
   B200_CUDA(cudaMemcpyAsync(vq.p, v_firstdim, vq.n * 8, cudaMemcpyHostToDevice, c->stream));
-  launch_query_to_dev(db->layout.G, qd.p, vq.p, c->stream);
-  run_first_dim(c, db, 1, qd.p, Images{}, zmajor ? zm.p : o.p, (int)slice, 1);
+  launch_query_to_dev(s.layout.G, qd.p, vq.p, c->stream);
+  run_first_dim(c, s, 1, qd.p, Images{}, zmajor ? zm.p : o.p, (int)slice, 1);
   uint32_t* o_slice = o.p + (size_t)slice * rows * 4 * POLY;          // ntt32 [row][ct_row][n][z] of this slice
-  if (zmajor) launch_zmajor_to_ntt32(db->layout.F, zm.p, o_slice, (int)slice, c->stream);
+  if (zmajor) launch_zmajor_to_ntt32(s.layout.F, zm.p, o_slice, (int)slice, c->stream);
   download_widen(c, out, o_slice, (size_t)rows * 4 * POLY);
   B200_CUDA(cudaGetLastError());
   API_END
@@ -933,9 +933,10 @@ void run_finish(b200pir_ctx* c, Keys keys, const uint32_t* gathered_dev, size_t 
 
 // The query schedule of a sharded database (b200pir_db_create_sharded) once the calling context c, the home, has put the
 // call's first-dimension operand (`images`, or c->w_qdev) and folding matrices (c->w_vfold) in place: every part runs the
-// first dimension and the fold rounds nu_2 - 1 .. log2 G on its rows, on its own context's stream, and gathers its survivors
-// into slot g of db->gathered; c then folds across the parts (rounds log2 G - 1 .. 0), packs and encodes into out_dev.  A part
-// on c's device reads c's buffers directly; a part on another device receives them in its own buffers by copy engine.
+// first dimension and the fold rounds nu_2 - 1 .. log2 G on its store, on the stream of its own context (db->worker), and
+// gathers its survivors into slot g of db->gathered; c then folds across the parts (rounds log2 G - 1 .. 0), packs and
+// encodes into out_dev.  A part on c's device reads c's buffers directly; a part on another device receives them in its own
+// buffers by copy engine.
 // Options that change the response bytes ("sparse_fold") are c's for every part.
 //
 // Stream order, with no host synchronisation:
@@ -955,7 +956,7 @@ void run_shards(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, Images 
   B200_CUDA(cudaEventRecord(db->expanded, c->stream));
   for (size_t g = 0; g < G; g++) {
     b200pir_db::Part& part = db->parts[g];
-    b200pir_ctx* x = part.db->ctx;
+    b200pir_ctx* x = db->worker(c, g);
     B200_CUDA(cudaSetDevice(x->device));
     if (x->stream != c->stream) B200_CUDA(cudaStreamWaitEvent(x->stream, db->expanded, 0));
     const uint8_t* xop = op;
@@ -966,16 +967,16 @@ void run_shards(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, Images 
       xop = part.operand.p;
       xfold = part.vfold.p;
     }
-    x->ensure_workspace_lite(count, part.db->rows);
+    x->ensure_workspace_lite(count, part.store->rows);
     const Images xim{images.p ? xop : nullptr, images.per_group};
-    const Survivors s = run_first_dim_and_fold(x, part.db.get(), count, images.p ? nullptr : reinterpret_cast<const uint4*>(xop),
+    const Survivors s = run_first_dim_and_fold(x, *part.store, count, images.p ? nullptr : reinterpret_cast<const uint4*>(xop),
                                                xim, xfold, c->sparse_fold);
     gather_survivors(x, s, count, db->gathered.p + g * count * c->slices * 4 * POLY);
     B200_CUDA(cudaEventRecord(part.done, x->stream));
   }
   B200_CUDA(cudaSetDevice(c->device));
-  for (const auto& part : db->parts)
-    if (part.db->ctx->stream != c->stream) B200_CUDA(cudaStreamWaitEvent(c->stream, part.done, 0));
+  for (size_t g = 0; g < G; g++)
+    if (db->worker(c, g)->stream != c->stream) B200_CUDA(cudaStreamWaitEvent(c->stream, db->parts[g].done, 0));
   run_finish(c, keys, db->gathered.p, G, count, 0, count, c->w_vfold.p, out_dev);
   B200_CUDA(cudaEventRecord(db->finished, c->stream));
 }
@@ -994,23 +995,23 @@ void run_queries(b200pir_ctx* c, b200pir_db* db, Keys keys, size_t count, bool n
     for (size_t i = 0; i < count; i++) check_pp(c, keys.each[i]);
   else
     check_pp(c, keys.one);
-  if (db->shard.count != 1) throw Error(B200PIR_E_BADARG, "sharded database: use the stage_a / stage_b entry points");
+  if (!db->whole()) throw Error(B200PIR_E_BADARG, "sharded database: use the stage_a / stage_b entry points");
   if (needs_expand && !c->hp.expand_queries)
     throw Error(B200PIR_E_BADARG, keys.each ? "multi-client batches need expand_queries" : "batch entry point needs expand_queries");
   if (count == 0) return;
   // a sharded database's home workspace holds the finish's G survivors per (query, slice), not local rows
-  const size_t rows = db->sharded() ? db->parts.size() : (size_t)db->rows;
+  const size_t rows = db->sharded() ? db->parts.size() : (size_t)db->parts[0].store->rows;
   c->ensure_workspace(keys.each && c->coalesce ? std::max(count, b200pir_ctx::kCoalesceMax) : count, rows);
   c->prof_reset();
   if (db->sharded()) B200_CUDA(cudaStreamWaitEvent(c->stream, db->finished, 0));
   stage();
   // format-2 databases get their operand as tile images straight from the expansion
-  const bool images = db->layout.format == 2 && c->hp.expand_queries;
+  const bool images = db->parts[0].store->layout.format == 2 && c->hp.expand_queries;
   run_prepare(c, keys, count, images);
   const Images im{images ? c->w_qt.p : nullptr, 16};
   uint8_t* resp = out.dev ? out.dev : c->w_resp.p;
   if (db->sharded()) run_shards(c, db, keys, count, im, resp);
-  else run_pack_encode(c, keys, run_first_dim_and_fold(c, db, count, c->w_qdev.p, im, c->w_vfold.p, c->sparse_fold), count, resp);
+  else run_pack_encode(c, keys, run_first_dim_and_fold(c, *db->parts[0].store, count, c->w_qdev.p, im, c->w_vfold.p, c->sparse_fold), count, resp);
   if (!out.dev) {
     const size_t rb = c->response_bytes;
     if (out.each)
@@ -1166,7 +1167,7 @@ int b200pir_process_query(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, const 
     // server.rs:666-678: v_reg_reoriented = query.v_buf ; v_folding = v_ct.map(ntt)
     vq.alloc((size_t)c->dim0 * 2 * POLY);
     B200_CUDA(cudaMemcpyAsync(vq.p, v_buf, vq.n * 8, cudaMemcpyHostToDevice, c->stream));
-    launch_query_to_dev(c->geom(db->rows), c->w_qdev.p, vq.p, c->stream);
+    launch_query_to_dev(db->parts[0].store->layout.G, c->w_qdev.p, vq.p, c->stream);
     const size_t npolys = (size_t)c->hp.nu_2 * 2 * 2 * c->hp.t_gsw;
     raw.alloc(std::max<size_t>(npolys, 1) * POLY);
     if (npolys) {
@@ -1213,16 +1214,16 @@ int first_dim_fold_dev(b200pir_ctx* c, b200pir_db* db, const void* operand_dev, 
   if (!c || !operand_dev || !partial_dev || (!v_folding_dev && c->hp.nu_2)) throw Error(B200PIR_E_BADARG, "null argument");
   Guard gd(c);
   check_db(c, db);
-  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "a sharded database runs its own schedule: use the query entry points");
+  const DbStore& s = db->single("a sharded database runs its own schedule: use the query entry points");
   if (images) {
-    if (db->layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
+    if (s.layout.format != 2) throw Error(B200PIR_E_BADARG, "tile images need a wgmma-layout database (db_format 2)");
     if (per_group == 0 || per_group > 16) throw Error(B200PIR_E_SHAPE, "one image holds 1..16 queries");
   }
   if (count == 0) return 0;
-  c->ensure_workspace_lite(count, db->rows);
+  c->ensure_workspace_lite(count, s.rows);
   const uint4* qdev = images ? nullptr : (const uint4*)operand_dev;
   const Images im{images ? (const uint8_t*)operand_dev : nullptr, per_group};
-  gather_survivors(c, run_first_dim_and_fold(c, db, count, qdev, im, v_folding_dev, c->sparse_fold), count, partial_dev);
+  gather_survivors(c, run_first_dim_and_fold(c, s, count, qdev, im, v_folding_dev, c->sparse_fold), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }
@@ -1269,13 +1270,13 @@ int b200pir_query_stage_a_dev(b200pir_ctx* c, b200pir_db* db, b200pir_pp* pp, co
   Guard gd(c);
   check_db(c, db);
   check_pp(c, pp);
-  if (db->sharded()) throw Error(B200PIR_E_UNSUPPORTED, "a sharded database runs its own schedule: use the query entry points");
+  const DbStore& s = db->single("a sharded database runs its own schedule: use the query entry points");
   if (!c->hp.expand_queries) throw Error(B200PIR_E_BADARG, "needs expand_queries");
-  c->ensure_workspace(count, db->rows);
+  c->ensure_workspace(count, s.rows);
   c->prof_reset();
   B200_CUDA(cudaMemcpyAsync(c->w_query.p, query_cts_dev, count * 2 * POLY * 8, cudaMemcpyDeviceToDevice, c->stream));
   run_prepare(c, Keys{pp}, count, false);
-  gather_survivors(c, run_first_dim_and_fold(c, db, count, c->w_qdev.p, Images{}, c->w_vfold.p, c->sparse_fold), count, partial_dev);
+  gather_survivors(c, run_first_dim_and_fold(c, s, count, c->w_qdev.p, Images{}, c->w_vfold.p, c->sparse_fold), count, partial_dev);
   B200_CUDA(cudaGetLastError());
   API_END
 }

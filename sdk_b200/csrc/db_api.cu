@@ -2,7 +2,8 @@
 // exports, the plaintext read-back (read_items, save_raw_file), the item writers and the presence map.  Every writer places
 // items through the same three decisions: which GPU owns an item (Shard::local_item), the context's write staging (w_wbytes)
 // and the presence update (mark_items / mark_slices).
-// A sharded handle (b200pir_db_create_sharded) runs each of them once per part, on the part's context, from inputs read once.
+// They run once per part of the handle (several for b200pir_db_create_sharded), on the context members() names, from inputs
+// read once.
 #include "spiral_api.hpp"
 #include "update_body.hpp"
 #include <cstdio>
@@ -17,7 +18,7 @@ static_assert(B200PIR_ITEM_NOT_PLAINTEXT == kReadNotPlaintext && B200PIR_ITEM_PA
 
 // ---------------------------------------------------------------- presence
 // every item of `items` written in slices [slice_begin, slice_end): one upload of the whole mask when any word changed
-void b200pir_db::mark_items(const ItemWrite* items, size_t count, int slice_begin, int slice_end, cudaStream_t s) {
+void DbStore::mark_items(const ItemWrite* items, size_t count, int slice_begin, int slice_end, cudaStream_t s) {
   bool changed = false;
   for (size_t k = 0; k < count; k++)
     for (int sl = slice_begin; sl < slice_end; sl++) {
@@ -33,7 +34,7 @@ void b200pir_db::mark_items(const ItemWrite* items, size_t count, int slice_begi
 }
 // whole slices [slice_begin, slice_end) written at once (bulk upload, file load, synthetic fill): every item of them exists
 // from now on
-void b200pir_db::mark_slices(int slice_begin, int slice_end, cudaStream_t s) {
+void DbStore::mark_slices(int slice_begin, int slice_end, cudaStream_t s) {
   const uint64_t lo = (uint64_t)slice_begin * rows * ctx->dim0, hi = (uint64_t)slice_end * rows * ctx->dim0;
   for (uint64_t b = lo; b < hi; b++)
     if (!((present[b >> 6] >> (b & 63)) & 1)) { present[b >> 6] |= 1ull << (b & 63); present_count++; }
@@ -45,14 +46,13 @@ void b200pir_db::mark_slices(int slice_begin, int slice_end, cudaStream_t s) {
 }
 
 b200pir_db::~b200pir_db() {
-  if (parts.empty()) return;
   for (auto& p : parts) {
-    if (!p.db) continue;
-    cudaSetDevice(p.db->ctx->device);
+    if (!p.store) continue;                   // a creation that failed before this part
+    cudaSetDevice(p.store->ctx->device);
     if (p.done) cudaEventDestroy(p.done);
     p.operand.release();
     p.vfold.release();
-    p.db.reset();
+    p.store.reset();
   }
   cudaSetDevice(ctx->device);
   if (expanded) cudaEventDestroy(expanded);
@@ -62,7 +62,7 @@ b200pir_db::~b200pir_db() {
 // Bytes of the first-dimension operand of `queries` queries as the query path hands it to a part: tile images of 16 queries
 // for a format-2 database whose queries are expanded, q_dev otherwise
 size_t b200pir_db::operand_bytes(size_t queries) const {
-  if (layout.format == 2 && ctx->hp.expand_queries) return (queries + 15) / 16 * tc5_query_bytes(make_tc5_geom(ctx->dim0, 32));
+  if (parts[0].store->layout.format == 2 && ctx->hp.expand_queries) return (queries + 15) / 16 * tc5_query_bytes(make_tc5_geom(ctx->dim0, 32));
   return queries * ctx->dim0 * POLY * sizeof(uint4);
 }
 
@@ -71,15 +71,15 @@ size_t b200pir_db::operand_bytes(size_t queries) const {
 void b200pir_db::ensure_exchange(size_t queries) {
   if (queries <= exchange_queries) return;
   for (auto& p : parts) {
-    B200_CUDA(cudaSetDevice(p.db->ctx->device));
-    B200_CUDA(cudaStreamSynchronize(p.db->ctx->stream));
+    B200_CUDA(cudaSetDevice(p.store->ctx->device));
+    B200_CUDA(cudaStreamSynchronize(p.store->ctx->stream));
   }
   B200_CUDA(cudaSetDevice(ctx->device));
   B200_CUDA(cudaEventSynchronize(finished));
   gathered.alloc(parts.size() * queries * ctx->slices * 4 * POLY);
   for (auto& p : parts) {
-    if (p.db->ctx->device == ctx->device) continue;
-    B200_CUDA(cudaSetDevice(p.db->ctx->device));
+    if (p.store->ctx->device == ctx->device) continue;
+    B200_CUDA(cudaSetDevice(p.store->ctx->device));
     p.operand.alloc(operand_bytes(queries));
     p.vfold.alloc(queries * ctx->fold_words());
   }
@@ -89,13 +89,12 @@ void b200pir_db::ensure_exchange(size_t queries) {
 
 namespace {
 
-// Where a writer or an export of `db` called on context c does its work: (c, db) for an ordinary database or a rank shard,
-// (part context, part) for every part of a sharded one
-struct Member { b200pir_ctx* ctx; b200pir_db* db; };
+// Where a writer or an export of `db` called on context c does its work: every part's store, on the context
+// b200pir_db::worker names
+struct Member { b200pir_ctx* ctx; DbStore* store; };
 std::vector<Member> members(b200pir_ctx* c, b200pir_db* db) {
-  if (!db->sharded()) return {Member{c, db}};
   std::vector<Member> ms;
-  for (auto& p : db->parts) ms.push_back(Member{p.db->ctx, p.db.get()});
+  for (size_t g = 0; g < db->parts.size(); g++) ms.push_back(Member{db->worker(c, g), db->parts[g].store.get()});
   return ms;
 }
 
@@ -120,13 +119,13 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
       B200_CUDA(cudaSetDevice(m.ctx->device));
       uint64_t* stage = reinterpret_cast<uint64_t*>(m.ctx->w_wbytes.p);
       B200_CUDA(cudaMemcpyAsync(stage, src, per_z * cur * 8, cudaMemcpyHostToDevice, m.ctx->stream));
-      launch_db_import(m.db->layout, m.db->shard, (int)slice, stage, z0, cur, m.ctx->stream);
+      launch_db_import(m.store->layout, m.store->shard, (int)slice, stage, z0, cur, m.ctx->stream);
     }
     for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   }
   for (const Member& m : ms) {
     B200_CUDA(cudaSetDevice(m.ctx->device));
-    m.db->mark_slices((int)slice, (int)slice + 1, m.ctx->stream);
+    m.store->mark_slices((int)slice, (int)slice + 1, m.ctx->stream);
     B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   }
   B200_CUDA(cudaSetDevice(c->device));
@@ -136,13 +135,13 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
 // Stage `span` raw bytes from host memory `host` and write the `count` items that lie in them (ItemWrite offsets are relative
 // to `host`): one conversion-and-placement launch over (item, slice).  Presence is the caller's.  Stream-ordered: the staging
 // buffers are only overwritten by the next group's copies, which run after this launch.
-void write_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
+void write_items(b200pir_ctx* c, const DbStore& s, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
   if (count == 0) return;
   c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
   c->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, count));
   if (span) B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, host, span, cudaMemcpyHostToDevice, c->stream));
   B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
-  launch_write_items(c->dp, db->layout, c->w_wbytes.p, c->w_witems.p, (int)count, c->slices, (int)c->bytes_per_chunk, c->hp.p, c->stream);
+  launch_write_items(c->dp, s.layout, c->w_wbytes.p, c->w_witems.p, (int)count, c->slices, (int)c->bytes_per_chunk, c->hp.p, c->stream);
 }
 
 // Device-to-host streaming, shared by the exports (b200pir_db_download(_slice), b200pir_db_save_file) and the item readers
@@ -200,7 +199,7 @@ void stream_out(b200pir_ctx* c, b200pir_db* db, size_t chunks, size_t stage_byte
 template <typename Sink>
 void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end, Sink sink) {
   const std::vector<Member> ms = members(c, db);
-  const size_t per_z = (size_t)ms[0].db->rows * c->dim0;
+  const size_t per_z = (size_t)ms[0].store->rows * c->dim0;
   const int zc = (int)std::max<size_t>(1, std::min<size_t>(POLY, b200pir_ctx::kWriteStageBytes / (per_z * 8)));
   struct Chunk { int slice, z0, zc; };
   std::vector<Chunk> chunks;
@@ -209,7 +208,7 @@ void export_impl(b200pir_ctx* c, b200pir_db* db, int slice_begin, int slice_end,
   std::vector<const uint64_t*> words(ms.size());
   stream_out(c, db, chunks.size(), per_z * zc * 8,
              [&](size_t k, size_t g, uint8_t* stage) {
-               launch_db_export(ms[g].db->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<uint64_t*>(stage),
+               launch_db_export(ms[g].store->layout, chunks[k].slice, chunks[k].z0, chunks[k].zc, reinterpret_cast<uint64_t*>(stage),
                                 ms[g].ctx->stream);
                return per_z * chunks[k].zc * 8;
              },
@@ -240,7 +239,7 @@ void read_items_impl(b200pir_ctx* c, b200pir_db* db, size_t count, Index idx, Si
                const size_t k0 = k * group, n = std::min(group, count - k0);
                std::vector<Where>& w = where[k & 1];
                w.resize(n);
-               const b200pir_db* m = ms[g].db;
+               const DbStore* m = ms[g].store;
                items.clear();
                for (size_t i = 0; i < n; i++) {
                  int il, j;
@@ -328,7 +327,7 @@ void check_raw_params(const b200pir_ctx* c) {
 void scatter_rows(b200pir_ctx* c, const std::vector<Member>& ms, int zc, const std::vector<const uint64_t*>& src, uint64_t* dst) {
   const size_t d0 = (size_t)c->dim0, npg = (size_t)c->num_per;
   for (size_t g = 0; g < ms.size(); g++) {
-    const b200pir_db* m = ms[g].db;
+    const DbStore* m = ms[g].store;
     const size_t rows = (size_t)m->rows;
     if (m->shard.count == 1) { std::memcpy(dst, src[g], (size_t)zc * rows * d0 * 8); continue; }
     for (size_t zl = 0; zl < (size_t)zc; zl++)
@@ -354,41 +353,29 @@ std::pair<std::unique_ptr<FILE, int (*)(FILE*)>, off_t> open_sized(const char* p
   return {std::move(f), bytes};
 }
 
-}  // namespace
-
-extern "C" {
-
-}  // extern "C"
-
-namespace {
-// Rows ii = shard_index (mod shard_count) on context c in layout `format` (-1: automatic); c's lock is held
-std::unique_ptr<b200pir_db> create_db(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, int format) {
-  std::unique_ptr<b200pir_db> db(new b200pir_db());
-  db->ctx = c;
-  db->shard = Shard{(int)shard_index, (int)shard_count};
-  db->rows = c->num_per / (int)shard_count;
-  DbLayout& L = db->layout;
-  L.G = c->geom(db->rows);
-  L.F = make_imma_geom(c->dim0, db->rows);
-  L.T = make_tc5_geom(c->dim0, db->rows);
+// Rows ii = shard.index (mod shard.count) on context c in layout `format` (-1: automatic); c's lock is held
+std::unique_ptr<DbStore> create_store(b200pir_ctx* c, Shard shard, int format) {
+  std::unique_ptr<DbStore> s(new DbStore());
+  s->ctx = c;
+  s->shard = shard;
+  s->rows = c->num_per / shard.count;
+  DbLayout& L = s->layout;
+  L.G = c->geom(s->rows);
+  L.F = make_imma_geom(c->dim0, s->rows);
+  L.T = make_tc5_geom(c->dim0, s->rows);
   L.format = format >= 0 ? format : (tc5_supported(L.T) ? 2 : 1);
-  db->present.assign((db->capacity() + 63) / 64, 0);
-  db->h_tile_mask.assign((size_t)c->slices * L.T.mt, 0u);
-  db->tile_mask.alloc(db->h_tile_mask.size());
+  s->present.assign((s->capacity() + 63) / 64, 0);
+  s->h_tile_mask.assign((size_t)c->slices * L.T.mt, 0u);
+  s->tile_mask.alloc(s->h_tile_mask.size());
   // on the context's stream: a cudaMemset would queue on the legacy default stream, behind whatever the caller has there,
   // and could land after the first writer's mask upload on the context's stream
-  B200_CUDA(cudaMemsetAsync(db->tile_mask.p, 0, db->h_tile_mask.size() * 4, c->stream));
+  B200_CUDA(cudaMemsetAsync(s->tile_mask.p, 0, s->h_tile_mask.size() * 4, c->stream));
   if (L.format == 2 && !tc5_supported(L.T)) throw Error(B200PIR_E_UNSUPPORTED, "db_format 2: dim0 too large for the wgmma kernel");
-  db->store.alloc(db_bytes(L, c->slices));
-  L.base = db->store.p;
-  B200_CUDA(cudaMemsetAsync(db->store.p, 0, db->store.n, c->stream));
+  s->store.alloc(db_bytes(L, c->slices));
+  L.base = s->store.p;
+  B200_CUDA(cudaMemsetAsync(s->store.p, 0, s->store.n, c->stream));
   B200_CUDA(cudaStreamSynchronize(c->stream));
-  return db;
-}
-
-void check_shard_count(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count) {
-  if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)c->num_per % shard_count)
-    throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+  return s;
 }
 
 // lets the current device reach `peer`'s memory directly where the hardware allows it
@@ -401,6 +388,41 @@ void enable_peer(int device, int peer) {
   if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
   else B200_CUDA(e);
 }
+
+// The handle whose part g is row shard shard_index + g of shard_count on ctxs[g], for `parts` = 1 (b200pir_db_create) or
+// shard_count parts from shard 0 (b200pir_db_create_sharded), in the home context's db_format; the exchange state only with
+// several parts
+std::unique_ptr<b200pir_db> create_db(b200pir_ctx* const* ctxs, size_t parts, uint64_t shard_index, uint64_t shard_count) {
+  b200pir_ctx* home = ctxs[0];
+  int format;
+  {
+    Guard gd(home);
+    if (shard_index >= shard_count || (shard_count & (shard_count - 1)) || (uint64_t)home->num_per % shard_count)
+      throw Error(B200PIR_E_BADARG, "shard_count must be a power of two dividing num_per");
+    format = home->db_format;
+  }
+  std::unique_ptr<b200pir_db> db(new b200pir_db());
+  db->ctx = home;
+  db->parts = std::vector<b200pir_db::Part>(parts);     // Part holds device buffers: built in place, never moved
+  for (size_t g = 0; g < parts; g++) {
+    b200pir_ctx* c = ctxs[g];
+    Guard gd(c);
+    b200pir_db::Part& p = db->parts[g];
+    p.store = create_store(c, Shard{(int)(shard_index + g), (int)shard_count}, format);
+    if (parts == 1) return db;
+    B200_CUDA(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
+    if (c->device != home->device) {
+      enable_peer(c->device, home->device);
+      enable_peer(home->device, c->device);
+    }
+  }
+  Guard gd(home, db.get());
+  B200_CUDA(cudaEventCreateWithFlags(&db->expanded, cudaEventDisableTiming));
+  B200_CUDA(cudaEventCreateWithFlags(&db->finished, cudaEventDisableTiming));
+  B200_CUDA(cudaEventRecord(db->finished, home->stream));
+  db->ensure_exchange(b200pir_ctx::kCoalesceMax);
+  return db;
+}
 }  // namespace
 
 extern "C" {
@@ -408,10 +430,8 @@ extern "C" {
 int b200pir_db_create(b200pir_ctx* c, uint64_t shard_index, uint64_t shard_count, b200pir_db** out) {
   API_BEGIN
   if (!c || !out) throw Error(B200PIR_E_BADARG, "null argument");
-  Guard gd(c);
   if (shard_count == 0) { shard_count = 1; shard_index = 0; }
-  check_shard_count(c, shard_index, shard_count);
-  *out = create_db(c, shard_index, shard_count, c->db_format).release();
+  *out = create_db(&c, 1, shard_index, shard_count).release();
   API_END
 }
 int b200pir_db_create_sharded(b200pir_ctx* const* ctxs, size_t shards, b200pir_db** out) {
@@ -425,44 +445,11 @@ int b200pir_db_create_sharded(b200pir_ctx* const* ctxs, size_t shards, b200pir_d
     if (std::memcmp(&ctxs[g]->hp, &ctxs[0]->hp, sizeof(b200pir_params)) != 0)
       throw Error(B200PIR_E_BADARG, "the contexts of a sharded database must have identical parameters");
   }
-  b200pir_ctx* home = ctxs[0];
-  int format;
-  {
-    Guard gd(home);
-    check_shard_count(home, 0, shards);
-    format = home->db_format;
-    if (shards == 1) { *out = create_db(home, 0, 1, format).release(); return 0; }
-  }
-  std::unique_ptr<b200pir_db> db(new b200pir_db());
-  db->ctx = home;
-  db->shard = Shard{0, 1};
-  db->rows = home->num_per;
-  db->parts = std::vector<b200pir_db::Part>(shards);     // Part holds device buffers: built in place, never moved
-  for (size_t g = 0; g < shards; g++) {
-    b200pir_ctx* c = ctxs[g];
-    Guard gd(c);
-    b200pir_db::Part& p = db->parts[g];
-    p.db = create_db(c, g, shards, format);
-    B200_CUDA(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
-    if (c->device != home->device) {
-      enable_peer(c->device, home->device);
-      enable_peer(home->device, c->device);
-    }
-  }
-  Guard gd(home, db.get());
-  db->layout = db->parts[0].db->layout;
-  db->layout.base = nullptr;
-  B200_CUDA(cudaEventCreateWithFlags(&db->expanded, cudaEventDisableTiming));
-  B200_CUDA(cudaEventCreateWithFlags(&db->finished, cudaEventDisableTiming));
-  B200_CUDA(cudaEventRecord(db->finished, home->stream));
-  db->ensure_exchange(b200pir_ctx::kCoalesceMax);
-  *out = db.release();
+  *out = create_db(ctxs, shards, 0, shards).release();
   API_END
 }
 void b200pir_db_destroy(b200pir_db* db) {
-  if (!db) return;
-  cudaSetDevice(db->ctx->device);
-  delete db;                                  // a sharded database frees each part on its own device
+  delete db;                                  // frees each part on its own device
 }
 
 int b200pir_db_upload_slice(b200pir_ctx* c, b200pir_db* db, uint64_t slice, const uint64_t* words, size_t n_words) {
@@ -529,15 +516,15 @@ int b200pir_db_save_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   API_BEGIN
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
   check_db(c, db);
-  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
+  if (!db->whole()) throw Error(B200PIR_E_UNSUPPORTED, "save_file: a shard holds only part of the database (use download)");
   const std::vector<Member> ms = members(c, db);
   write_atomically(path, [&](FILE* f) {
-    // a sharded database's chunk is assembled from its parts' exports first: host memory stays bounded by the staging
+    // a chunk of row shards is assembled from their exports first: host memory stays bounded by the staging
     std::vector<uint64_t> whole;
     export_impl(c, db, 0, c->slices, [&](int, int, int zc, const std::vector<const uint64_t*>& src) {
       const size_t n = (size_t)zc * c->num_per * c->dim0;
       const uint64_t* words = src[0];
-      if (db->sharded()) {
+      if (ms[0].store->shard.count != 1) {
         whole.resize(n);
         scatter_rows(c, ms, zc, src, whole.data());
         words = whole.data();
@@ -556,7 +543,7 @@ int b200pir_db_read_items(b200pir_ctx* c, b200pir_db* db, const uint64_t* db_idx
   for (size_t k = 0; k < count; k++) {
     int il, j;
     if (db_idx[k] >= num_items) throw Error(B200PIR_E_SHAPE, "bad db idx " + std::to_string(db_idx[k]));
-    if (!db->shard.local_item(db_idx[k], c->num_per, il, j))
+    if (!db->whole() && !db->parts[0].store->shard.local_item(db_idx[k], c->num_per, il, j))
       throw Error(B200PIR_E_SHAPE, "db idx " + std::to_string(db_idx[k]) + " lies in a row this shard does not hold");
   }
   const size_t span = (size_t)c->slices * c->bytes_per_chunk;
@@ -577,7 +564,7 @@ int b200pir_db_save_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   if (!c || !path) throw Error(B200PIR_E_BADARG, "null argument");
   check_db(c, db);
   check_raw_params(c);
-  if (db->shard.count != 1) throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: a shard holds only part of the database");
+  if (!db->whole()) throw Error(B200PIR_E_UNSUPPORTED, "save_raw_file: a shard holds only part of the database");
   const size_t num_items = (size_t)c->dim0 * c->num_per, isz = c->hp.db_item_size;
   const size_t span = (size_t)c->slices * c->bytes_per_chunk, tail = span - isz;   // span >= isz: bytes_per_chunk rounds up
   write_atomically(path, [&](FILE* f) {
@@ -614,14 +601,14 @@ int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint6
   if (slice >= (uint64_t)c->slices || item_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "index out of range");
   for (const Member& m : members(c, db)) {
     int il, j;
-    if (!m.db->shard.local_item(item_idx, c->num_per, il, j)) continue;   // row lives on another GPU
+    if (!m.store->shard.local_item(item_idx, c->num_per, il, j)) continue;   // row lives on another GPU
     b200pir_ctx* x = m.ctx;
     B200_CUDA(cudaSetDevice(x->device));
     x->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like write_items
     B200_CUDA(cudaMemcpyAsync(x->w_wbytes.p, poly, POLY * 8, cudaMemcpyHostToDevice, x->stream));
-    launch_db_upsert(m.db->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(x->w_wbytes.p), x->stream);
+    launch_db_upsert(m.store->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(x->w_wbytes.p), x->stream);
     const ItemWrite item{0, 0, (uint32_t)il, (uint32_t)j};
-    m.db->mark_items(&item, 1, (int)slice, (int)slice + 1, x->stream);
+    m.store->mark_items(&item, 1, (int)slice, (int)slice + 1, x->stream);
     // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
     B200_CUDA(cudaStreamSynchronize(x->stream));
     B200_CUDA(cudaSetDevice(c->device));
@@ -638,11 +625,11 @@ int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, 
   if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
   for (const Member& m : members(c, db)) {
     int il, j;
-    if (!m.db->shard.local_item(db_idx, c->num_per, il, j)) continue;     // row lives on another GPU
+    if (!m.store->shard.local_item(db_idx, c->num_per, il, j)) continue;     // row lives on another GPU
     B200_CUDA(cudaSetDevice(m.ctx->device));
     const ItemWrite item{0, (uint32_t)len, (uint32_t)il, (uint32_t)j};
-    write_items(m.ctx, m.db, data, len, &item, 1);
-    m.db->mark_items(&item, 1, 0, c->slices, m.ctx->stream);
+    write_items(m.ctx, *m.store, data, len, &item, 1);
+    m.store->mark_items(&item, 1, 0, c->slices, m.ctx->stream);
     B200_CUDA(cudaStreamSynchronize(m.ctx->stream));                          // writers hold the host write lock
     B200_CUDA(cudaSetDevice(c->device));
     B200_CUDA(cudaGetLastError());
@@ -677,20 +664,20 @@ int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* 
       end = e;
       for (size_t g = 0; g < ms.size(); g++) {
         int il, j;
-        if (!ms[g].db->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
+        if (!ms[g].store->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
         group[g].push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)il, (uint32_t)j});
         most = std::max(most, group[g].size());
       }
     }
     for (size_t g = 0; g < ms.size(); g++) {
       B200_CUDA(cudaSetDevice(ms[g].ctx->device));
-      write_items(ms[g].ctx, ms[g].db, body + base, end - base, group[g].data(), group[g].size());
+      write_items(ms[g].ctx, *ms[g].store, body + base, end - base, group[g].data(), group[g].size());
       all[g].insert(all[g].end(), group[g].begin(), group[g].end());
     }
   }
   for (size_t g = 0; g < ms.size(); g++) {
     B200_CUDA(cudaSetDevice(ms[g].ctx->device));
-    ms[g].db->mark_items(all[g].data(), all[g].size(), 0, c->slices, ms[g].ctx->stream);
+    ms[g].store->mark_items(all[g].data(), all[g].size(), 0, c->slices, ms[g].ctx->stream);
     B200_CUDA(cudaStreamSynchronize(ms[g].ctx->stream));                        // writers hold the host write lock
   }
   B200_CUDA(cudaSetDevice(c->device));
@@ -734,17 +721,17 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
       for (size_t k = 0; k < cnt; k++) {
         const size_t idx = i0 + k, pos = idx * isz;
         int il, j;
-        if (!m.db->shard.local_item(idx, c->num_per, il, j)) continue;       // row lives on another GPU
+        if (!m.store->shard.local_item(idx, c->num_per, il, j)) continue;       // row lives on another GPU
         const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0; // clipped at the end of the file
         items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)il, (uint32_t)j});
       }
       B200_CUDA(cudaSetDevice(m.ctx->device));
-      write_items(m.ctx, m.db, host.data(), span, items.data(), items.size()); // pageable `host`: staged before the call returns
+      write_items(m.ctx, *m.store, host.data(), span, items.data(), items.size()); // pageable `host`: staged before the call returns
     }
   }
   for (const Member& m : ms) {
     B200_CUDA(cudaSetDevice(m.ctx->device));
-    m.db->mark_slices(0, c->slices, m.ctx->stream);                           // load_db_from_seek builds a dense database
+    m.store->mark_slices(0, c->slices, m.ctx->stream);                           // load_db_from_seek builds a dense database
     B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   }
   B200_CUDA(cudaSetDevice(c->device));
@@ -755,11 +742,8 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
 int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity) {
   API_BEGIN
   if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  uint64_t n = db->present_count, cap = db->capacity();
-  if (db->sharded()) {
-    n = cap = 0;
-    for (const auto& p : db->parts) { n += p.db->present_count; cap += p.db->capacity(); }
-  }
+  uint64_t n = 0, cap = 0;
+  for (const auto& p : db->parts) { n += p.store->present_count; cap += p.store->capacity(); }
   if (items) *items = n;
   if (capacity) *capacity = cap;
   API_END
@@ -767,10 +751,10 @@ int b200pir_db_present_items(b200pir_db* db, uint64_t* items, uint64_t* capacity
 int b200pir_db_info(b200pir_db* db, int* format, uint64_t* local_rows, uint64_t* hbm_bytes) {
   API_BEGIN
   if (!db) throw Error(B200PIR_E_BADARG, "null db");
-  if (format) *format = db->layout.format;
-  if (local_rows) *local_rows = (uint64_t)db->rows;
-  uint64_t bytes = db->store.n;
-  for (const auto& p : db->parts) bytes += p.db->store.n;
+  uint64_t rows = 0, bytes = 0;
+  for (const auto& p : db->parts) { rows += p.store->rows; bytes += p.store->store.n; }
+  if (format) *format = db->parts[0].store->layout.format;
+  if (local_rows) *local_rows = rows;
   if (hbm_bytes) *hbm_bytes = bytes;
   API_END
 }
@@ -782,8 +766,8 @@ int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
   const std::vector<Member> ms = members(c, db);
   for (const Member& m : ms) {                                  // distinct devices fill at the same time
     B200_CUDA(cudaSetDevice(m.ctx->device));
-    launch_write_synthetic(m.ctx->dp, m.db->layout, m.db->shard, seed, c->hp.p, m.ctx->stream);
-    m.db->mark_slices(0, c->slices, m.ctx->stream);
+    launch_write_synthetic(m.ctx->dp, m.store->layout, m.store->shard, seed, c->hp.p, m.ctx->stream);
+    m.store->mark_slices(0, c->slices, m.ctx->stream);
   }
   for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   B200_CUDA(cudaSetDevice(c->device));

@@ -176,7 +176,8 @@ struct b200pir_ctx {
   }
 };
 
-struct b200pir_db {
+// One row shard's storage on the context that created it: rows ii = shard.index (mod shard.count) of every slice.
+struct DbStore {
   b200pir_ctx* ctx;
   Shard shard;
   int rows;                 // local second-dimension rows
@@ -195,23 +196,37 @@ struct b200pir_db {
   uint64_t capacity() const { return (uint64_t)ctx->slices * rows * ctx->dim0; }
   void mark_items(const ItemWrite* items, size_t count, int slice_begin, int slice_end, cudaStream_t s);
   void mark_slices(int slice_begin, int slice_end, cudaStream_t s);
+};
 
-  // A database over several contexts (b200pir_db_create_sharded): parts[g] is row shard g on its own context and this handle,
-  // owned by the home context `ctx`, holds no rows itself (empty store, rows = num_per).  A query call expands on the home
-  // context, hands the operand to every part, and finishes on the home context from the survivors the parts gather in
-  // `gathered` (db_api.cu creates the buffers, api.cu's run_shards uses them).
+// A database handle, owned by the home context `ctx`: a list of row-shard stores.  b200pir_db_create gives one part, the
+// whole database or one rank shard of it; b200pir_db_create_sharded gives G parts, part g holding shard g of G on its own
+// context.  With several parts a query call expands on the home context, hands the operand to every part, and finishes on the
+// home context from the survivors the parts gather in `gathered`: that exchange state exists only then (db_api.cu creates it,
+// api.cu's run_shards uses it).
+struct b200pir_db {
+  b200pir_ctx* ctx;
   struct Part {
-    std::unique_ptr<b200pir_db> db;
+    std::unique_ptr<DbStore> store;
     DevBuf<uint8_t> operand;      // the call's first-dimension operand, on a part whose device is not the home device
     DevBuf<uint32_t> vfold;       // the call's folding matrices, likewise
     cudaEvent_t done = nullptr;   // recorded on the part's stream after its survivors are gathered
   };
-  std::vector<Part> parts;
+  std::vector<Part> parts;        // at least one
   size_t exchange_queries = 0;    // queries the buffers below and the parts' receive buffers hold
   DevBuf<uint32_t> gathered;      // on the home device: [G][count][slices][4 * 2048] survivors
   cudaEvent_t expanded = nullptr; // recorded on the calling context's stream once the operands are in place
   cudaEvent_t finished = nullptr; // recorded after the finish: the next call's calling stream waits on it
-  bool sharded() const { return !parts.empty(); }
+  bool sharded() const { return parts.size() > 1; }
+  // every row of the database, not one rank shard of it
+  bool whole() const { return parts.size() == (size_t)parts[0].store->shard.count; }
+  // The context that does part g's work in a call on context c: c itself with one part, so that contexts sharing a database
+  // each run on their own stream; the part's own context with several
+  b200pir_ctx* worker(b200pir_ctx* c, size_t g) const { return sharded() ? parts[g].store->ctx : c; }
+  // The one store of a database that is not sharded; a sharded one runs its own schedule and is refused with `refusal`
+  const DbStore& single(const char* refusal) const {
+    if (sharded()) throw Error(B200PIR_E_UNSUPPORTED, refusal);
+    return *parts[0].store;
+  }
   size_t operand_bytes(size_t queries) const;
   void ensure_exchange(size_t queries);
   ~b200pir_db();
@@ -219,14 +234,15 @@ struct b200pir_db {
 
 namespace b200pir {
 
-// The calling context's lock and, for a sharded database, every part's context lock, taken in creation order so that calls on
-// databases that share contexts, and direct calls on a member context, cannot deadlock; the current device becomes c's.
+// The calling context's lock and the lock of every context that does a part's work (b200pir_db::worker: only c's for a
+// database of one part, which keeps contexts that share it concurrent), taken in creation order so that calls on databases
+// that share contexts, and direct calls on a member context, cannot deadlock; the current device becomes c's.
 struct Guard {
   std::vector<b200pir_ctx*> held;
   explicit Guard(b200pir_ctx* c, const b200pir_db* db = nullptr) {
     held.push_back(c);
     if (db)
-      for (const auto& p : db->parts) held.push_back(p.db->ctx);
+      for (size_t g = 0; g < db->parts.size(); g++) held.push_back(db->worker(c, g));
     std::sort(held.begin(), held.end(), [](const b200pir_ctx* a, const b200pir_ctx* b) { return a->seq < b->seq; });
     held.erase(std::unique(held.begin(), held.end()), held.end());
     for (auto* h : held) h->mu.lock();
