@@ -1,9 +1,9 @@
 // C-ABI implementation of the HBM-resident database handle (include/b200pir.h): creation, bulk uploads and file loads,
-// exports, the plaintext read-back (read_items, save_raw_file), the item writers and the presence map.  Every writer places
-// items through the same three decisions: which GPU owns an item (Shard::local_item), the context's write staging (w_wbytes)
-// and the presence update (mark_items / mark_slices).
-// They run once per part of the handle (several for b200pir_db_create_sharded), on the context members() names, from inputs
-// read once.
+// exports, the plaintext read-back (read_items, save_raw_file), the item writers and the presence map.  Every writer works over
+// the parts of the handle (several for b200pir_db_create_sharded), on the contexts members() names, from inputs read once,
+// and makes the same three decisions in one place each: which member holds an item (owner), how raw items are staged in
+// groups and written (RawWriter, in the context's write staging w_wbytes / w_witems), and how the call ends (settle: presence,
+// then a synchronise of each member written).
 #include "spiral_api.hpp"
 #include "update_body.hpp"
 #include <cstdio>
@@ -11,6 +11,7 @@
 #include <fcntl.h>
 #include <unistd.h>
 #include <memory>
+#include <optional>
 #include <utility>
 
 static_assert(B200PIR_ITEM_NOT_PLAINTEXT == kReadNotPlaintext && B200PIR_ITEM_PAST_CHUNK == kReadPastChunk &&
@@ -98,6 +99,34 @@ std::vector<Member> members(b200pir_ctx* c, b200pir_db* db) {
   return ms;
 }
 
+// The member of `ms` that holds global item idx, with the item's local row il and column j; none when the database is a rank
+// shard that does not hold the item's row
+struct Owner { size_t g; int il, j; };
+std::optional<Owner> owner(const std::vector<Member>& ms, uint64_t idx) {
+  for (size_t g = 0; g < ms.size(); g++) {
+    int il, j;
+    if (ms[g].store->shard.local_item(idx, ms[g].ctx->num_per, il, j)) return Owner{g, il, j};
+  }
+  return std::nullopt;
+}
+
+// How every writer ends.  On each member the call wrote, presence is marked on the member's stream and the stream is
+// synchronised: items[g], member g's written items, in slices [slice_begin, slice_end), or without `items` those whole slices
+// on every member.  A member that received nothing is not touched.  Writers hold the host write lock (bin/server.rs:35,49), so
+// a write is complete when the call returns.  Leaves the home device current.
+void settle(b200pir_ctx* c, const std::vector<Member>& ms, int slice_begin, int slice_end,
+            const std::vector<std::vector<ItemWrite>>* items = nullptr) {
+  for (size_t g = 0; g < ms.size(); g++) {
+    if (items && (*items)[g].empty()) continue;
+    B200_CUDA(cudaSetDevice(ms[g].ctx->device));
+    if (items) ms[g].store->mark_items((*items)[g].data(), (*items)[g].size(), slice_begin, slice_end, ms[g].ctx->stream);
+    else ms[g].store->mark_slices(slice_begin, slice_end, ms[g].ctx->stream);
+    B200_CUDA(cudaStreamSynchronize(ms[g].ctx->stream));
+  }
+  B200_CUDA(cudaSetDevice(c->device));
+  B200_CUDA(cudaGetLastError());
+}
+
 // One slice in the reference's z-major layout, delivered chunk by chunk: fetch(word_offset, n_words) returns a host pointer
 // to that range of the slice (valid until the next call).
 template <typename Fetch>
@@ -123,26 +152,49 @@ void upload_slice_impl(b200pir_ctx* c, b200pir_db* db, uint64_t slice, Fetch fet
     }
     for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
   }
-  for (const Member& m : ms) {
-    B200_CUDA(cudaSetDevice(m.ctx->device));
-    m.store->mark_slices((int)slice, (int)slice + 1, m.ctx->stream);
-    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
-  }
-  B200_CUDA(cudaSetDevice(c->device));
-  B200_CUDA(cudaGetLastError());
+  settle(c, ms, (int)slice, (int)slice + 1);
 }
 
-// Stage `span` raw bytes from host memory `host` and write the `count` items that lie in them (ItemWrite offsets are relative
-// to `host`): one conversion-and-placement launch over (item, slice).  Presence is the caller's.  Stream-ordered: the staging
-// buffers are only overwritten by the next group's copies, which run after this launch.
-void write_items(b200pir_ctx* c, const DbStore& s, const uint8_t* host, size_t span, const ItemWrite* items, size_t count) {
-  if (count == 0) return;
-  c->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
-  c->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, count));
-  if (span) B200_CUDA(cudaMemcpyAsync(c->w_wbytes.p, host, span, cudaMemcpyHostToDevice, c->stream));
-  B200_CUDA(cudaMemcpyAsync(c->w_witems.p, items, count * sizeof(ItemWrite), cudaMemcpyHostToDevice, c->stream));
-  launch_write_items(c->dp, s.layout, c->w_wbytes.p, c->w_witems.p, (int)count, c->slices, (int)c->bytes_per_chunk, c->hp.p, c->stream);
-}
+// The raw-item writer (update_item_raw, update_many_items, load_raw_file).  The caller adds the items of one group, whose bytes
+// lie in one host span, then writes the group from that span; finish() settles the call.  Presence: every written item in
+// every slice, or, `dense`, every slice of every member (a whole database was loaded).
+struct RawWriter {
+  b200pir_ctx* c;
+  std::vector<Member> ms;
+  bool dense;
+  std::vector<std::vector<ItemWrite>> group, written;   // per member: the group's items, and those of the groups written
+  bool full = false;                                    // some member's share of the group fills its item staging
+  RawWriter(b200pir_ctx* c, b200pir_db* db, bool dense) : c(c), ms(members(c, db)), dense(dense), group(ms.size()), written(ms.size()) {}
+  // item db_idx at bytes [off, off + len) of the group's span, for the member that holds it
+  void add(uint64_t db_idx, size_t off, uint32_t len) {
+    const std::optional<Owner> o = owner(ms, db_idx);
+    if (!o) return;
+    group[o->g].push_back(ItemWrite{(uint32_t)off, len, (uint32_t)o->il, (uint32_t)o->j});
+    full |= group[o->g].size() >= b200pir_ctx::kWriteStageItems;
+  }
+  // Stages `span` bytes from `host` to each member that received items of the group and writes them there: one
+  // conversion-and-placement launch over (item, slice).  Stream-ordered: the staging buffers are only overwritten by the next
+  // group's copies, which run after this launch.
+  void write(const uint8_t* host, size_t span) {
+    for (size_t g = 0; g < ms.size(); g++) {
+      std::vector<ItemWrite>& items = group[g];
+      if (items.empty()) continue;
+      b200pir_ctx* x = ms[g].ctx;
+      B200_CUDA(cudaSetDevice(x->device));
+      x->w_wbytes.ensure(std::max(b200pir_ctx::kWriteStageBytes, span));
+      x->w_witems.ensure(std::max(b200pir_ctx::kWriteStageItems, items.size()));
+      // pageable sources: staged before the copies return, so `host` and `items` may be refilled
+      if (span) B200_CUDA(cudaMemcpyAsync(x->w_wbytes.p, host, span, cudaMemcpyHostToDevice, x->stream));
+      B200_CUDA(cudaMemcpyAsync(x->w_witems.p, items.data(), items.size() * sizeof(ItemWrite), cudaMemcpyHostToDevice, x->stream));
+      launch_write_items(x->dp, ms[g].store->layout, x->w_wbytes.p, x->w_witems.p, (int)items.size(), x->slices,
+                         (int)x->bytes_per_chunk, x->hp.p, x->stream);
+      if (!dense) written[g].insert(written[g].end(), items.begin(), items.end());
+      items.clear();
+    }
+    full = false;
+  }
+  void finish() { settle(c, ms, 0, c->slices, dense ? nullptr : &written); }
+};
 
 // Device-to-host streaming, shared by the exports (b200pir_db_download(_slice), b200pir_db_save_file) and the item readers
 // (b200pir_db_read_items, b200pir_db_save_raw_file).  Under each member's context lock, fill(k, g, stage) queues the device
@@ -242,15 +294,15 @@ void read_items_impl(b200pir_ctx* c, b200pir_db* db, size_t count, Index idx, Si
                const DbStore* m = ms[g].store;
                items.clear();
                for (size_t i = 0; i < n; i++) {
-                 int il, j;
-                 if (!m->shard.local_item(idx(k0 + i), c->num_per, il, j)) continue;   // row lives on another GPU
+                 const std::optional<Owner> o = owner(ms, idx(k0 + i));
+                 if (!o || o->g != g) continue;                                // row lives on another member
                  uint8_t present = 0;
                  for (size_t sl = 0; sl < slices; sl++) {
-                   const uint64_t bit = ((uint64_t)sl * m->rows + il) * c->dim0 + j;
+                   const uint64_t bit = ((uint64_t)sl * m->rows + o->il) * c->dim0 + o->j;
                    present |= (m->present[bit >> 6] >> (bit & 63)) & 1;
                  }
                  w[i] = Where{(uint32_t)g, (uint32_t)items.size(), present ? (uint8_t)B200PIR_ITEM_PRESENT : (uint8_t)0};
-                 items.push_back(ItemWrite{(uint32_t)items.size(), 0, (uint32_t)il, (uint32_t)j});
+                 items.push_back(ItemWrite{(uint32_t)items.size(), 0, (uint32_t)o->il, (uint32_t)o->j});
                }
                held[k & 1][g] = items.size();
                if (items.empty()) return 0;
@@ -540,10 +592,10 @@ int b200pir_db_read_items(b200pir_ctx* c, b200pir_db* db, const uint64_t* db_idx
   check_db(c, db);
   check_raw_params(c);
   const uint64_t num_items = (uint64_t)c->dim0 * c->num_per;
+  const std::vector<Member> ms = members(c, db);
   for (size_t k = 0; k < count; k++) {
-    int il, j;
     if (db_idx[k] >= num_items) throw Error(B200PIR_E_SHAPE, "bad db idx " + std::to_string(db_idx[k]));
-    if (!db->whole() && !db->parts[0].store->shard.local_item(db_idx[k], c->num_per, il, j))
+    if (!owner(ms, db_idx[k]))
       throw Error(B200PIR_E_SHAPE, "db idx " + std::to_string(db_idx[k]) + " lies in a row this shard does not hold");
   }
   const size_t span = (size_t)c->slices * c->bytes_per_chunk;
@@ -599,20 +651,17 @@ int b200pir_db_upsert_item(b200pir_ctx* c, b200pir_db* db, uint64_t slice, uint6
   Guard gd(c, db);
   check_db(c, db);
   if (slice >= (uint64_t)c->slices || item_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "index out of range");
-  for (const Member& m : members(c, db)) {
-    int il, j;
-    if (!m.store->shard.local_item(item_idx, c->num_per, il, j)) continue;   // row lives on another GPU
-    b200pir_ctx* x = m.ctx;
+  const std::vector<Member> ms = members(c, db);
+  std::vector<std::vector<ItemWrite>> written(ms.size());
+  if (const std::optional<Owner> o = owner(ms, item_idx)) {
+    b200pir_ctx* x = ms[o->g].ctx;
     B200_CUDA(cudaSetDevice(x->device));
-    x->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like write_items
+    x->w_wbytes.ensure(b200pir_ctx::kWriteStageBytes);                     // the writers' staging, like RawWriter
     B200_CUDA(cudaMemcpyAsync(x->w_wbytes.p, poly, POLY * 8, cudaMemcpyHostToDevice, x->stream));
-    launch_db_upsert(m.store->layout, (int)slice, il, j, reinterpret_cast<const uint64_t*>(x->w_wbytes.p), x->stream);
-    const ItemWrite item{0, 0, (uint32_t)il, (uint32_t)j};
-    m.store->mark_items(&item, 1, (int)slice, (int)slice + 1, x->stream);
-    // the host RwLock gives upserts exclusive access (bin/server.rs:35,49): finish before returning
-    B200_CUDA(cudaStreamSynchronize(x->stream));
-    B200_CUDA(cudaSetDevice(c->device));
+    launch_db_upsert(ms[o->g].store->layout, (int)slice, o->il, o->j, reinterpret_cast<const uint64_t*>(x->w_wbytes.p), x->stream);
+    written[o->g].push_back(ItemWrite{0, 0, (uint32_t)o->il, (uint32_t)o->j});
   }
+  settle(c, ms, (int)slice, (int)slice + 1, &written);
   API_END
 }
 int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, const uint8_t* data, size_t len) {
@@ -623,17 +672,10 @@ int b200pir_db_update_item_raw(b200pir_ctx* c, b200pir_db* db, uint64_t db_idx, 
   check_raw_params(c);
   if (len > (size_t)c->slices * c->bytes_per_chunk) throw Error(B200PIR_E_SHAPE, "update longer than instances*n^2*bytes_per_chunk");   // loading.rs:308-310
   if (db_idx >= (uint64_t)c->dim0 * c->num_per) throw Error(B200PIR_E_SHAPE, "bad db idx");                      // loading.rs:333-340
-  for (const Member& m : members(c, db)) {
-    int il, j;
-    if (!m.store->shard.local_item(db_idx, c->num_per, il, j)) continue;     // row lives on another GPU
-    B200_CUDA(cudaSetDevice(m.ctx->device));
-    const ItemWrite item{0, (uint32_t)len, (uint32_t)il, (uint32_t)j};
-    write_items(m.ctx, *m.store, data, len, &item, 1);
-    m.store->mark_items(&item, 1, 0, c->slices, m.ctx->stream);
-    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));                          // writers hold the host write lock
-    B200_CUDA(cudaSetDevice(c->device));
-    B200_CUDA(cudaGetLastError());
-  }
+  RawWriter w(c, db, false);                                                  // a group of one item
+  w.add(db_idx, 0, (uint32_t)len);
+  w.write(data, len);
+  w.finish();
   API_END
 }
 
@@ -651,37 +693,20 @@ int b200pir_db_update_many_items(b200pir_ctx* c, b200pir_db* db, const uint8_t* 
   if (c->hp.p != 256 && !parsed.entries.empty()) throw Error(B200PIR_E_UNSUPPORTED, "convert_pt_to_poly asserts logp == 8 (loading.rs:291)");
   if (c->bytes_per_chunk > (size_t)POLY && !parsed.entries.empty()) throw Error(B200PIR_E_SHAPE, "bytes_per_chunk exceeds poly_len");
   const std::vector<BodyEntry> kept = keep_last_occurrence(parsed.entries);
-  const std::vector<Member> ms = members(c, db);
-  std::vector<std::vector<ItemWrite>> all(ms.size()), group(ms.size());
+  RawWriter w(c, db, false);
   for (size_t k = 0; k < kept.size();) {
     // one staging group: whole entries in body order, their bytes (dropped duplicates in between included) within the budget
     const size_t k0 = k, base = kept[k].data_pos();
-    size_t end = base, most = 0;
-    for (auto& g : group) g.clear();
-    for (; k < kept.size() && most < b200pir_ctx::kWriteStageItems; k++) {
+    size_t end = base;
+    for (; k < kept.size() && !w.full; k++) {
       const size_t e = kept[k].data_pos() + kept[k].data_len();
       if (k > k0 && e - base > b200pir_ctx::kWriteStageBytes) break;
       end = e;
-      for (size_t g = 0; g < ms.size(); g++) {
-        int il, j;
-        if (!ms[g].store->shard.local_item(kept[k].db_idx, c->num_per, il, j)) continue;   // row lives on another GPU
-        group[g].push_back(ItemWrite{(uint32_t)(kept[k].data_pos() - base), kept[k].data_len(), (uint32_t)il, (uint32_t)j});
-        most = std::max(most, group[g].size());
-      }
+      w.add(kept[k].db_idx, kept[k].data_pos() - base, kept[k].data_len());
     }
-    for (size_t g = 0; g < ms.size(); g++) {
-      B200_CUDA(cudaSetDevice(ms[g].ctx->device));
-      write_items(ms[g].ctx, *ms[g].store, body + base, end - base, group[g].data(), group[g].size());
-      all[g].insert(all[g].end(), group[g].begin(), group[g].end());
-    }
+    w.write(body + base, end - base);
   }
-  for (size_t g = 0; g < ms.size(); g++) {
-    B200_CUDA(cudaSetDevice(ms[g].ctx->device));
-    ms[g].store->mark_items(all[g].data(), all[g].size(), 0, c->slices, ms[g].ctx->stream);
-    B200_CUDA(cudaStreamSynchronize(ms[g].ctx->stream));                        // writers hold the host write lock
-  }
-  B200_CUDA(cudaSetDevice(c->device));
-  B200_CUDA(cudaGetLastError());
+  w.finish();
   if (parsed.error) throw Error(parsed.error, parsed.message);
   if (largest_update) *largest_update = parsed.largest_update;
   API_END
@@ -706,9 +731,8 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
   const size_t item_span = (size_t)c->slices * c->bytes_per_chunk, isz = c->hp.db_item_size;
   const size_t group = std::max<size_t>(1, std::min(b200pir_ctx::kWriteStageItems,
                                                     b200pir_ctx::kWriteStageBytes / std::max<size_t>(1, std::max(isz, item_span))));
-  const std::vector<Member> ms = members(c, db);
+  RawWriter w(c, db, true);                                                   // load_db_from_seek builds a dense database
   std::vector<uint8_t> host;
-  std::vector<ItemWrite> items;
   for (size_t i0 = 0; i0 < num_items; i0 += group) {
     const size_t cnt = std::min(group, num_items - i0);
     const size_t lo = i0 * isz, hi = std::min(flen, (i0 + cnt - 1) * isz + item_span);
@@ -716,26 +740,13 @@ int b200pir_db_load_raw_file(b200pir_ctx* c, b200pir_db* db, const char* path) {
     host.resize(span);
     if (span && (fseeko(file.get(), (off_t)lo, SEEK_SET) || fread(host.data(), 1, span, file.get()) != span))
       throw Error(B200PIR_E_SHAPE, "short read from the database file");
-    for (const Member& m : ms) {                                              // one read, staged to every member
-      items.clear();
-      for (size_t k = 0; k < cnt; k++) {
-        const size_t idx = i0 + k, pos = idx * isz;
-        int il, j;
-        if (!m.store->shard.local_item(idx, c->num_per, il, j)) continue;       // row lives on another GPU
-        const size_t len = pos < flen ? std::min(item_span, flen - pos) : 0; // clipped at the end of the file
-        items.push_back(ItemWrite{(uint32_t)(len ? pos - lo : 0), (uint32_t)len, (uint32_t)il, (uint32_t)j});
-      }
-      B200_CUDA(cudaSetDevice(m.ctx->device));
-      write_items(m.ctx, *m.store, host.data(), span, items.data(), items.size()); // pageable `host`: staged before the call returns
+    for (size_t idx = i0; idx < i0 + cnt; idx++) {
+      const size_t pos = idx * isz, len = pos < flen ? std::min(item_span, flen - pos) : 0;   // clipped at the end of the file
+      w.add(idx, len ? pos - lo : 0, (uint32_t)len);
     }
+    w.write(host.data(), span);                                               // one read, staged to every member
   }
-  for (const Member& m : ms) {
-    B200_CUDA(cudaSetDevice(m.ctx->device));
-    m.store->mark_slices(0, c->slices, m.ctx->stream);                           // load_db_from_seek builds a dense database
-    B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
-  }
-  B200_CUDA(cudaSetDevice(c->device));
-  B200_CUDA(cudaGetLastError());
+  w.finish();
   API_END
 }
 
@@ -764,14 +775,11 @@ int b200pir_db_fill_synthetic(b200pir_ctx* c, b200pir_db* db, uint64_t seed) {
   Guard gd(c, db);
   check_db(c, db);
   const std::vector<Member> ms = members(c, db);
-  for (const Member& m : ms) {                                  // distinct devices fill at the same time
-    B200_CUDA(cudaSetDevice(m.ctx->device));
+  for (const Member& m : ms) {                                  // every member launches before any is waited on: distinct
+    B200_CUDA(cudaSetDevice(m.ctx->device));                    // devices fill at the same time
     launch_write_synthetic(m.ctx->dp, m.store->layout, m.store->shard, seed, c->hp.p, m.ctx->stream);
-    m.store->mark_slices(0, c->slices, m.ctx->stream);
   }
-  for (const Member& m : ms) B200_CUDA(cudaStreamSynchronize(m.ctx->stream));
-  B200_CUDA(cudaSetDevice(c->device));
-  B200_CUDA(cudaGetLastError());
+  settle(c, ms, 0, c->slices);
   API_END
 }
 
